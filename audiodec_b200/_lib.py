@@ -1,6 +1,6 @@
 """ctypes binding of the C ABI declared in include/audiodec_b200.h.
 
-The shared library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_100a).  There is no
+The shared library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_90a).  There is no
 CPU or PyTorch fallback: if the library is missing, or no CUDA device is usable, every entry point
 raises."""
 from __future__ import annotations
@@ -70,7 +70,6 @@ SYMBOLS = {
     "adec_range_error": (c_int, [c_void_p, c_void_p]),
     "adec_launch_count": (c_int64, [c_void_p]),
     "adec_ktrace": (c_int, [c_void_p, ctypes.POINTER(ctypes.c_ulonglong), c_int]),
-    "adec_probe_mma_ex": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double)]),
     "adec_probe_mma": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double)]),
     "adec_profile": (c_int, [c_void_p, c_int]),
     "adec_profile_report": (c_int, [c_void_p, c_char_p, c_int]),

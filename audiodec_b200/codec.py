@@ -5,7 +5,7 @@
 keywords (``config.yml`` ``generator_params``), same methods with the same tensor shapes
 (``load_state_dict / eval / to / initial_encoder / initial_decoder / encode / quantize / lookup /
 decode / reset_buffer``), so the objects can be returned from ``AudioCodec._load_encoder /
-_load_decoder`` (bin/stream.py:38-45) unchanged.  All arithmetic happens in hand-written sm_100a
+_load_decoder`` (bin/stream.py:38-45) unchanged.  All arithmetic happens in hand-written sm_90a
 kernels (audiodec_b200/csrc); torch only provides device memory and the current stream.
 
 Differences from the reference, all extensions:
@@ -63,7 +63,7 @@ class _StreamGeneratorBase:
             return self._set_dtype(device)
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError("audiodec_b200 runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("audiodec_b200 runs on CUDA (sm_90a) only; there is no CPU fallback")
         if self._sd is None:
             raise RuntimeError("load_state_dict must be called before .to(device)")
         if self._h is not None:

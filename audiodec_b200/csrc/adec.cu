@@ -19,20 +19,13 @@
 
 #include "../../include/audiodec_b200.h"
 #include "kernels.cuh"
-#include "tc_kernels.cuh"
-#include "tc_persist.cuh"
-#include "tc_f16.cuh"
-#include "probe.cuh"
+#include "wg_conv.cuh"
 #include <cuda_fp16.h>
 #include <cuda_bf16.h>
 
 using namespace adec;
 
 namespace {
-#ifdef ADEC_TIMELINE
-unsigned int* g_tl_last = nullptr;
-#endif
-
 thread_local std::string g_create_error;
 
 std::string fmt(const char* f, ...) {
@@ -99,53 +92,16 @@ const ConvKernelCfg* find_conv_kernel(int CW, int CO, bool fuse) {
     return nullptr;
 }
 
-// tensor-core (tcgen05, 3xTF32; ADEC_CONV_PATH=tf32) instantiations: NT = output-channel tile (UMMA N)
-inline int TcpCfgStages(int NT) { return NT == 128 ? TcpCfg<128>::STAGES : NT == 64 ? TcpCfg<64>::STAGES : TcpCfg<32>::STAGES; }
-// persistent variant: one CTA per SM loops over (time tile, channel tile, stream) tiles
+// tensor-core engine (wg_conv.cuh): PREC_F16 = two fp16 pieces per operand, three products (fp32-grade, default); PREC_TF32 = 3xTF32
+// (ADEC_CONV_PATH=tf32); PREC_BF16 = bf16 operands, one product (the vocoder's bf16 mode).  Persistent: one CTA per SM loops over
+// (time tile, channel tile, stream) tiles.
 typedef cudaError_t (*TcPersistFn)(const ConvArgs&, int, int, int, int, int, cudaStream_t);
-template <int NT, bool F, int PRE>
-cudaError_t launch_tcp(const ConvArgs& a, int n_xtiles, int n_ytiles, int n_tiles, int n_ctas, int smem_bytes, cudaStream_t s) {
-    static bool configured[64] = {false};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    auto kern = tc_conv_persist_kernel<NT, F, PRE>;
-#ifdef ADEC_TIMELINE
-    constexpr int kMaxDyn = 227 * 1024 - 2048;
-#else
-    constexpr int kMaxDyn = 227 * 1024;
-#endif
-    if (dev < 64 && !configured[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn);
-        if (e != cudaSuccess) return e;
-        configured[dev] = true;
-    }
-    if (smem_bytes > kMaxDyn) return cudaErrorInvalidConfiguration;
-    kern<<<n_ctas, TcpCfg<NT>::THREADS, smem_bytes, s>>>(a, n_xtiles, n_ytiles, n_tiles);
-    return cudaGetLastError();
-}
-
-struct TcKernelCfg { int NT, KS, stages; bool fuse; int pre; TcPersistFn pfn; };
-#define ADEC_TC1(NT, F, PRE) {NT, TC_CP, TcCfg<NT>::STAGES, F, PRE, launch_tcp<NT, F, PRE>}
-#define ADEC_TC(NT) \
-    ADEC_TC1(NT, true, ACT_ELU), ADEC_TC1(NT, false, ACT_NONE), ADEC_TC1(NT, false, ACT_ELU), ADEC_TC1(NT, false, ACT_LRELU), \
-    ADEC_TC1(NT, false, ACT_NORM)
-const TcKernelCfg kTcKernels[] = {ADEC_TC(128), ADEC_TC(64), ADEC_TC(32)};
-int kTcMaxFuse = 128;    // residual units wider than this run as two launches on the tensor-core path (ADEC_TC_MAXFUSE)
-
-const TcKernelCfg* find_tc_kernel(int NT, bool fuse, int pre) {
-    for (const auto& k : kTcKernels)
-        if (k.NT == NT && k.fuse == fuse && k.pre == pre) return &k;
-    return nullptr;
-}
-
-// tcgen05 kind::f16 engine (tc_f16.cuh; default): PREC 3 = two fp16 pieces per operand, three products (fp32-grade);
-// PREC 1 = bf16 operands, one product (the vocoder's bf16 mode)
 template <int NT, bool F, int PRE, int PREC>
-cudaError_t launch_tcf(const ConvArgs& a, int n_xtiles, int n_ytiles, int n_tiles, int n_ctas, int smem_bytes, cudaStream_t s) {
+cudaError_t launch_wg(const ConvArgs& a, int n_xtiles, int n_ytiles, int n_tiles, int n_ctas, int smem_bytes, cudaStream_t s) {
     static bool configured[64] = {false};
     int dev = 0;
     cudaGetDevice(&dev);
-    auto kern = tc_conv_f16_kernel<NT, F, PRE, PREC>;
+    auto kern = wg_conv_kernel<NT, F, PRE, PREC>;
     constexpr int kMaxDyn = 227 * 1024;
     if (dev < 64 && !configured[dev]) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn);
@@ -153,13 +109,13 @@ cudaError_t launch_tcf(const ConvArgs& a, int n_xtiles, int n_ytiles, int n_tile
         configured[dev] = true;
     }
     if (smem_bytes > kMaxDyn) return cudaErrorInvalidConfiguration;
-    // Programmatic dependent launch: the next launch's CTAs may start (barrier init, TMEM allocation, first weight stages - weights are
-    // constants) while the tail of the previous kernel of the stream is still running; its producer and drain warps execute
-    // griddepcontrol.wait before they touch any activation or state (tc_f16.cuh), which blocks until the previous grid has completed.
+    // Programmatic dependent launch: the next launch's CTAs may start (barrier init, first weight stages - weights are constants) while
+    // the tail of the previous kernel of the stream is still running; its producer and consumer warps execute griddepcontrol.wait
+    // before they touch any activation or state (wg_conv.cuh), which blocks until the previous grid has completed.
     static const bool pdl = [] { const char* e = getenv("ADEC_PDL"); return !e || atoi(e) != 0; }();
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3((unsigned)n_ctas);
-    cfg.blockDim = dim3((unsigned)TcfCfg<NT, PREC>::threads(F));
+    cfg.blockDim = dim3((unsigned)WgCfg<NT, PREC>::THREADS);
     cfg.dynamicSmemBytes = (size_t)smem_bytes;
     cfg.stream = s;
     cudaLaunchAttribute attr[1];
@@ -169,18 +125,22 @@ cudaError_t launch_tcf(const ConvArgs& a, int n_xtiles, int n_ytiles, int n_tile
     cfg.numAttrs = pdl ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, kern, a, n_xtiles, n_ytiles, n_tiles);
 }
-typedef size_t (*TcfSmemFn)(int, bool);
-typedef int (*TcfWbufFn)(int, bool);
-struct TcfKernelCfg { int NT; bool fuse; int pre, prec, tap_bytes; TcPersistFn pfn; TcfSmemFn smem; TcfWbufFn n_wbuf; };
-#define ADEC_TCF1(NT, F, PRE, PREC) \
-    {NT, F, PRE, PREC, TcfCfg<NT, PREC>::TAP_BYTES, launch_tcf<NT, F, PRE, PREC>, TcfCfg<NT, PREC>::smem_bytes, TcfCfg<NT, PREC>::n_wbuf}
-#define ADEC_TCF(NT) \
-    ADEC_TCF1(NT, true, ACT_ELU, 3), ADEC_TCF1(NT, false, ACT_NONE, 3), ADEC_TCF1(NT, false, ACT_ELU, 3), ADEC_TCF1(NT, false, ACT_LRELU, 3), \
-    ADEC_TCF1(NT, false, ACT_NORM, 3), ADEC_TCF1(NT, false, ACT_NONE, 1), ADEC_TCF1(NT, false, ACT_LRELU, 1), ADEC_TCF1(NT, false, ACT_NORM, 1)
-const TcfKernelCfg kTcfKernels[] = {ADEC_TCF(128), ADEC_TCF(64), ADEC_TCF(32)};
+typedef size_t (*TcSmemFn)(int, bool);
+typedef int (*TcWbufFn)(int, bool);
+struct TcKernelCfg { int NT; bool fuse; int pre, prec, tap_bytes; TcPersistFn pfn; TcSmemFn smem; TcWbufFn n_wbuf; };
+#define ADEC_TC1(NT, F, PRE, PREC) \
+    {NT, F, PRE, PREC, WgCfg<NT, PREC>::TAP_BYTES, launch_wg<NT, F, PRE, PREC>, WgCfg<NT, PREC>::smem_bytes, WgCfg<NT, PREC>::n_wbuf}
+#define ADEC_TC_FP32(NT, PREC) \
+    ADEC_TC1(NT, true, ACT_ELU, PREC), ADEC_TC1(NT, false, ACT_NONE, PREC), ADEC_TC1(NT, false, ACT_ELU, PREC), ADEC_TC1(NT, false, ACT_LRELU, PREC), \
+    ADEC_TC1(NT, false, ACT_NORM, PREC)
+#define ADEC_TC(NT) \
+    ADEC_TC_FP32(NT, PREC_F16), ADEC_TC_FP32(NT, PREC_TF32), \
+    ADEC_TC1(NT, false, ACT_NONE, PREC_BF16), ADEC_TC1(NT, false, ACT_LRELU, PREC_BF16), ADEC_TC1(NT, false, ACT_NORM, PREC_BF16)
+const TcKernelCfg kTcKernels[] = {ADEC_TC(128), ADEC_TC(64), ADEC_TC(32)};
+int kTcMaxFuse = 128;    // residual units wider than this run as two launches on the tensor-core path (ADEC_TC_MAXFUSE)
 
-const TcfKernelCfg* find_tcf_kernel(int NT, bool fuse, int pre, int prec) {
-    for (const auto& k : kTcfKernels)
+const TcKernelCfg* find_tc_kernel(int NT, bool fuse, int pre, int prec) {
+    for (const auto& k : kTcKernels)
         if (k.NT == NT && k.fuse == fuse && k.pre == pre && k.prec == prec) return &k;
     return nullptr;
 }
@@ -223,8 +183,7 @@ struct Op {
     std::vector<float> hstate;  // initial state (P, st_C) or empty (zeros)
     // kernel config
     const ConvKernelCfg* kc = nullptr;
-    const TcKernelCfg* tc = nullptr;   // 3xTF32 tensor-core path; kc = FFMA path
-    const TcfKernelCfg* tcf = nullptr; // kind::f16 tensor-core path (default)
+    const TcKernelCfg* tc = nullptr;   // tensor-core path; kc = FFMA path
     float w_scale = 1.f, w2_scale = 1.f;
     int n_pieces = 1, n_co_tiles = 1;
     // device
@@ -257,17 +216,13 @@ struct adec_handle {
     std::vector<Op> enc_ops, dec_ops;
     int n_streams = 1;
     int st_cap = 1;        // streams the state buffers were allocated for
-    int engine = 2;               // ADEC_CONV_PATH: 2 = f16 (tcgen05 kind::f16, default), 1 = tf32 (round-1 3xTF32), 0 = ffma (CUDA cores)
+    int engine = 2;               // ADEC_CONV_PATH: 2 = f16 (fp16-split wgmma, default), 1 = tf32 (3xTF32 wgmma), 0 = ffma (CUDA cores)
     bool use_tc = true;           // any tensor-core engine
     bool bf16 = false;            // cfg.compute_dtype == 1: bf16 operands (HiFi-GAN vocoder, f16 engine only)
-    int plain_teams = 2;          // ADEC_PLAIN_TEAMS=1: one producer team on the un-fused launches (A/B)
-    int gspan = 0;                // ADEC_GSPAN: accumulation span of the f16 engine (ConvArgs::gspan)
-    int dbg_flags = 0;
-    int dbg_wdiv = 0;             // ADEC_DBG_WDIV (timing experiments, wrong results)
     bool stack_rows = true;       // ADEC_STACK_ROWS=0: never stack several streams' rows into one tile (A/B)
     unsigned long long* d_ktrace = nullptr;   // ADEC_KTRACE=1: per-launch {start ns, end ns, SM cycles} records (diagnostics)
     int ktrace_n = 0;
-    int n_sms = 148;
+    int n_sms = 132;
     DevBuf ws[3];
     std::vector<void*> owned;     // device allocations freed in destroy
     // rvq
@@ -466,20 +421,20 @@ int pick_piece_width(const Op& op) {
     return 0;
 }
 
-// choose the kernel instantiation, pack + upload weights, allocate state
+// 3xTF32 engine: choose the kernel instantiation, pack + upload weights
 int finalize_op_tc(adec_handle* h, Op* op) {
     int NT = op->Cout % 128 == 0 ? 128 : op->Cout % 64 == 0 ? 64 : 32;
     // 96 outputs (transposed conv 64 -> 3*32): one zero-padded 128-wide tile beats three 32-wide tiles that each rebuild the
-    // same activation window and are smem-operand bound (persistent kernel only: its epilogue masks per 32-column piece)
+    // same activation window (the epilogue masks per column pair)
     const bool pad_tile = !op->fuse && NT == 32 && op->Cout > 64 && op->Cout < 128;
     if (pad_tile) NT = 128;
-    op->tc = find_tc_kernel(NT, op->fuse, op->pre_act);
+    op->tc = find_tc_kernel(NT, op->fuse, op->pre_act, PREC_TF32);
     if (!op->tc || (op->fuse && (NT != op->Cout || op->mid_act != op->pre_act))) return h->fail(op->name + ": no tensor-core kernel");
-    const int KS = op->tc->KS, CP = TC_CP;
+    const int KS = TC_CP, CP = TC_CP;
     op->n_pieces = op->Cin_eff / CP;
     op->n_co_tiles = pad_tile ? 1 : op->Cout / NT;
     op->w_tile_floats = (long long)op->Ktaps * op->Cin_eff * NT * 2;
-    // stage c = ((piece*Ktaps + tap)*(CP/KS) + ks): [hi: (KS/4)][NT][4] | [lo: same]   (UMMA K-major, no swizzle)
+    // one (piece, tap): [hi: (KS/4) K blocks][NT][4] | [lo: same]   (K-major, no swizzle)
     auto pack = [&](const float* weff, int G, int ntiles, int pieces, int taps, int cin_eff, int cout, std::vector<float>* out) {
         out->assign((size_t)G * ntiles * taps * cin_eff * NT * 2, 0.f);
         size_t o = 0;
@@ -516,20 +471,20 @@ int finalize_op_tc(adec_handle* h, Op* op) {
     return 0;
 }
 
-// kind::f16 engine: weights as fp16 (hi | lo | hi * 2^-11) of w * 2^p, or one bf16 plane, in UMMA K-major no-swizzle blocks:
+// fp16-split / bf16 engine: weights as fp16 (hi | lo | hi * 2^-11) of w * 2^p, or one bf16 plane, in K-major no-swizzle blocks:
 //   [group g][co tile][piece][tap][plane][kb = 8-channel block][NT rows][8 x 16 bit]
-// one (piece, tap) = TAP_BYTES; the kernel's weight producer copies one or two consecutive taps per stage (tc_f16.cuh).
+// one (piece, tap) = TAP_BYTES; the kernel's weight producer copies one or two consecutive taps per stage (wg_conv.cuh).
 int finalize_op_f16(adec_handle* h, Op* op) {
     int NT = op->Cout % 128 == 0 ? 128 : op->Cout % 64 == 0 ? 64 : 32;
     const bool pad_tile = !op->fuse && NT == 32 && op->Cout > 64 && op->Cout < 128;     // e.g. transposed conv 64 -> 3*32: one padded 128-wide tile
     if (pad_tile) NT = 128;
-    const int prec = (h->bf16 && !op->fuse) ? 1 : 3;
-    op->tcf = find_tcf_kernel(NT, op->fuse, op->pre_act, prec);
-    if (!op->tcf || (op->fuse && (NT != op->Cout || op->mid_act != op->pre_act))) return h->fail(op->name + ": no tensor-core kernel");
-    const int CP = TC_CP, KB = F16_KB, npl = prec == 3 ? 3 : 1;
+    const int prec = (h->bf16 && !op->fuse) ? PREC_BF16 : PREC_F16;
+    op->tc = find_tc_kernel(NT, op->fuse, op->pre_act, prec);
+    if (!op->tc || (op->fuse && (NT != op->Cout || op->mid_act != op->pre_act))) return h->fail(op->name + ": no tensor-core kernel");
+    const int CP = TC_CP, KB = TC_CP / 8, npl = prec == PREC_F16 ? 3 : 1;
     op->n_pieces = op->Cin_eff / CP;
     op->n_co_tiles = pad_tile ? 1 : op->Cout / NT;
-    const size_t tap_bytes = (size_t)op->tcf->tap_bytes;
+    const size_t tap_bytes = (size_t)op->tc->tap_bytes;
     op->w_tile_floats = (long long)((size_t)op->n_pieces * op->Ktaps * tap_bytes / 4);
     auto pow2_scale = [](const std::vector<float>& w, int* p_out) {
         float wmax = 0.f;
@@ -554,7 +509,7 @@ int finalize_op_f16(adec_handle* h, Op* op) {
                                     const int k = pc * CP + kb * 8 + e;
                                     const float w = nt * NT + n < cout ? weff[(((size_t)g * taps + tap) * cin_eff + k) * cout + nt * NT + n] : 0.f;
                                     const size_t at = o + ((size_t)kb * NT + n) * 8 + e, plane = (size_t)KB * NT * 8;
-                                    if (prec == 3) {
+                                    if (prec == PREC_F16) {
                                         const float ws = std::ldexp(w, p2);
                                         const uint16_t hi = half_bits(ws);
                                         img[at] = hi;
@@ -570,7 +525,7 @@ int finalize_op_f16(adec_handle* h, Op* op) {
         memcpy(out->data(), img.data(), img.size() * 2);
     };
     int p1 = 0, p2 = 0;
-    if (prec == 3) pow2_scale(op->weff, &p1);
+    if (prec == PREC_F16) pow2_scale(op->weff, &p1);
     op->w_scale = std::ldexp(1.0f, -p1);
     std::vector<float> packed;
     pack(op->weff.data(), op->G, op->n_co_tiles, op->n_pieces, op->Ktaps, op->Cin_eff, op->Cout, p1, &packed);
@@ -730,34 +685,14 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
             a.y_bs = op.out_nct ? (long long)op.G * op.Cout * Tout : (long long)Tout * op.ldy;
             a.mid_act = op.mid_act;
             a.hist_rep = (rc.offline && op.up > 1) ? 1 : 0;
-            a.w_scale = op.w_scale; a.w2_scale = op.w2_scale; a.err = h->d_err; a.dbg_wdiv = h->dbg_wdiv; a.dbg_flags = h->dbg_flags;
-            a.teams = h->plain_teams;
-            // bf16-operand launches (the vocoder's reduced-precision mode) accumulate a whole 32-channel piece per TMEM partial: their groups
-            // are 4 MMAs, so the TMEM -> register round trip per group is what they wait for, and a 22-step accumulation chain's truncation
-            // (3e-7) is far below bf16 operand rounding (measured at batch 128: 43.9 -> 41.5 ms per step, blocks.3.convs2 2.06 -> 1.72 ms)
-            const bool bf16_span = op.tcf && op.tcf->prec == 1 && h->gspan == 0;
-            a.gspan = (bf16_span || h->gspan == 1 || (h->gspan == 2 && op.tcf && op.tcf->NT >= 128) || (h->gspan == 3 && op.tcf && op.tcf->NT >= 64)) ? 1 : 0;
-#ifdef ADEC_TIMELINE
-            // debug build: record CTA 1's event timeline of the op named by ADEC_TIMELINE_OP on its 4th launch, dump it to ADEC_TIMELINE_OUT
-            static unsigned int* tl_buf = nullptr;
-            static int tl_hits = 0;
-            if (const char* tlop = getenv("ADEC_TIMELINE_OP")) {
-                if (op.name == tlop && ++tl_hits == 4) {
-                    if (!tl_buf) cudaMalloc((void**)&tl_buf, (2 + 2 * 8192 * 6) * sizeof(unsigned int));
-                    cudaMemsetAsync(tl_buf, 0, (2 + 2 * 8192 * 6) * sizeof(unsigned int), rc.stream);
-                    a.tl = tl_buf;
-                    g_tl_last = tl_buf;
-                }
-            }
-#endif
+            a.w_scale = op.w_scale; a.w2_scale = op.w2_scale; a.err = h->d_err;
             if (h->d_ktrace && h->ktrace_n < 4096) a.dbg = h->d_ktrace + 3 * (size_t)(h->ktrace_n++);
-            if (op.tcf || op.tc) {
+            if (op.tc) {
                 // persistent tensor-core kernels: one CTA per SM loops over (time tile, channel tile, stream) tiles
                 const int wrows = TC_TT + (op.Ktaps - 1) * op.dil;
-                const int NT = op.tcf ? op.tcf->NT : op.tc->NT;
                 dim3 grid((Tout + TC_TT - 1) / TC_TT, op.G * op.n_co_tiles, rc.B);
                 a.n_streams = rc.B;
-                if (op.tcf && h->stack_rows) {
+                if (h->stack_rows) {
                     // fill the 128-row tiles across streams when that needs fewer tiles (short chunks: 256 streams x 5..25 rows per layer)
                     const long long L = (long long)Tout + (long long)(op.Ktaps - 1) * op.dil;
                     const long long stacked = (rc.B * L + TC_TT - 1) / TC_TT;
@@ -769,17 +704,10 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
                 }
                 const long long n_tiles = (long long)grid.x * grid.y * grid.z;
                 const int n_ctas = (int)std::min<long long>(n_tiles, h->n_sms);
-                size_t psmem;
-                if (op.tcf) {
-                    psmem = op.tcf->smem(wrows, op.fuse);
-                    a.n_wbuf = op.tcf->n_wbuf(wrows, op.fuse);
-                    if (a.n_wbuf < 2) return h->fail(fmt("%s: window of %d rows does not fit in shared memory", op.name.c_str(), wrows));
-                } else {
-                    const int wrp = std::max(wrows, 129) | 1;
-                    const int pst = TcpCfgStages(NT), pmb = NT == 128 ? TcpCfg<128>::MB : NT == 64 ? TcpCfg<64>::MB : TcpCfg<32>::MB;
-                    psmem = 512 + sizeof(float) * ((size_t)pst * 2 * op.tc->KS * NT + (size_t)4 * TC_CP * wrp + (op.fuse ? (size_t)pmb * 2 * TC_CP * TC_MIDP : 0));
-                }
-                e = (op.tcf ? op.tcf->pfn : op.tc->pfn)(a, (int)grid.x, (int)grid.y, (int)n_tiles, n_ctas, (int)psmem, rc.stream);
+                const size_t psmem = op.tc->smem(wrows, op.fuse);
+                a.n_wbuf = op.tc->n_wbuf(wrows, op.fuse);
+                if (a.n_wbuf < 1) return h->fail(fmt("%s: window of %d rows does not fit in shared memory", op.name.c_str(), wrows));
+                e = op.tc->pfn(a, (int)grid.x, (int)grid.y, (int)n_tiles, n_ctas, (int)psmem, rc.stream);
             } else {
                 const int TT = op.kc->TT;
                 dim3 grid((Tout + TT - 1) / TT, op.G * op.n_co_tiles, rc.B);
@@ -787,28 +715,6 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
             }
         }
         if (e != cudaSuccess) return h->fail(fmt("launch of %s failed: %s", op.name.c_str(), cudaGetErrorString(e)));
-#ifdef ADEC_TIMELINE
-        if (op.kind == OP_CONV && getenv("ADEC_TIMELINE_OP") && op.name == getenv("ADEC_TIMELINE_OP")) {
-            static bool dumped = false;
-            if (g_tl_last && !dumped) {
-                dumped = true;
-                cudaStreamSynchronize(rc.stream);
-                std::vector<unsigned int> hb(2 + 2 * 8192 * 6);
-                cudaMemcpy(hb.data(), g_tl_last, hb.size() * sizeof(unsigned int), cudaMemcpyDeviceToHost);
-                const char* outp = getenv("ADEC_TIMELINE_OUT");
-                if (FILE* f = fopen(outp ? outp : "timeline.txt", "w")) {
-                    fprintf(f, "# %s\n", op.name.c_str());
-                    for (unsigned r = 0; r < 6; ++r)
-                        for (unsigned i = 0; i < 8192; ++i) {
-                            const unsigned w0 = hb[2 + 2 * (8192 * r + i)], w1 = hb[3 + 2 * (8192 * r + i)];
-                            if (!w0 && !w1) break;
-                            fprintf(f, "%u %u %u\n", w0 >> 24, w0 & 0xffffffu, w1);
-                        }
-                    fclose(f);
-                }
-            }
-        }
-#endif
         ++h->launches;
         if (h->profiling) {
             cudaEventRecord(ev1, rc.stream);
@@ -1202,10 +1108,6 @@ int adec_create(const adec_config* cfg, int device, adec_handle** out) {
     }
     h->use_tc = h->engine != 0;
     if (const char* sr = getenv("ADEC_STACK_ROWS")) h->stack_rows = atoi(sr) != 0;
-    if (const char* gs = getenv("ADEC_GSPAN")) h->gspan = atoi(gs);
-    if (const char* pt = getenv("ADEC_PLAIN_TEAMS")) h->plain_teams = atoi(pt) == 1 ? 1 : 2;
-    if (const char* wd = getenv("ADEC_DBG_WDIV")) h->dbg_wdiv = atoi(wd);
-    if (const char* df = getenv("ADEC_DBG_FLAGS")) h->dbg_flags = atoi(df);
     if (const char* kt = getenv("ADEC_KTRACE")) {
         if (atoi(kt)) { DeviceGuard dgk(device); cudaMalloc((void**)&h->d_ktrace, 4096 * 3 * sizeof(unsigned long long)); }
     }
@@ -1492,7 +1394,6 @@ int adec_codec_host(adec_handle* enc, adec_handle* dec, const float* x_host, int
         int herr = 0;
         CK(enc, cudaMemcpy(&herr, hh->d_err, sizeof(int), cudaMemcpyDeviceToHost));
         if (herr) CK(enc, cudaMemset(hh->d_err, 0, sizeof(int)));
-        if (hh->dbg_flags || hh->dbg_wdiv) continue;      // timing experiments: results are wrong on purpose
         if (herr & 1) return enc->fail("lookup: index out of range");
         if (herr & 2) return enc->fail("an activation left the range of the fp16-split tensor-core engine (|a| >= 6e4); use ADEC_CONV_PATH=tf32");
         if (hh == dec) break;     // enc == dec
@@ -1556,17 +1457,27 @@ int adec_ktrace(adec_handle* h, unsigned long long* out, int max_records) {
     return n;
 }
 
-int adec_probe_mma_ex(int device, int kind, int NT, int n_groups, int a_off_rows, int a_pitch_rows, int tap_step_rows, int n_issuers, double* tflops, double* ms) {
-    if (!tflops || (kind != 0 && kind != 1) || NT < 16 || NT > 256 || NT % 16 || n_groups < 1 || a_off_rows < 0 || a_pitch_rows < 128 || a_pitch_rows > 256 || tap_step_rows < 0 || tap_step_rows > 16 || n_issuers < 1 || n_issuers > 4) { g_create_error = "probe_mma: bad argument"; return 1; }
+int adec_probe_mma(int device, int kind, int NT, int n_groups, double* tflops, double* ms) {
+    if (!tflops || (kind != 0 && kind != 1) || (NT != 32 && NT != 64 && NT != 128 && NT != 256) || n_groups < 1) { g_create_error = "probe_mma: bad argument"; return 1; }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) { g_create_error = "probe_mma: no usable CUDA device"; return 1; }
     DeviceGuard dg(device);
     int n_sms = 0;
     cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, device);
-    const int smem = ((8 * 2 * a_pitch_rows + a_off_rows + 8 * tap_step_rows + 8) * 16 & ~127) + 8 * 2 * NT * 16;
+    constexpr int a_pitch_rows = 136;          // a window pitch of the engine (128 rows + halo)
+    const int smem = 8 * 2 * a_pitch_rows * 16 + 8 * 2 * NT * 16;
     auto launch = [&](cudaStream_t s) {
-        if (kind == 0) { cudaFuncSetAttribute(mma_probe_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); mma_probe_kernel<0><<<n_sms, 128, smem, s>>>(NT, n_groups, a_off_rows, a_pitch_rows, tap_step_rows, n_issuers); }
-        else { cudaFuncSetAttribute(mma_probe_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); mma_probe_kernel<1><<<n_sms, 128, smem, s>>>(NT, n_groups, a_off_rows, a_pitch_rows, tap_step_rows, n_issuers); }
+        auto go = [&](auto kern) {
+            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+            kern<<<n_sms, 256, smem, s>>>(n_groups, a_pitch_rows);
+        };
+        if (kind == 0) {
+            if (NT == 32) go(mma_probe_kernel<32, PREC_TF32>); else if (NT == 64) go(mma_probe_kernel<64, PREC_TF32>);
+            else if (NT == 128) go(mma_probe_kernel<128, PREC_TF32>); else go(mma_probe_kernel<256, PREC_TF32>);
+        } else {
+            if (NT == 32) go(mma_probe_kernel<32, PREC_F16>); else if (NT == 64) go(mma_probe_kernel<64, PREC_F16>);
+            else if (NT == 128) go(mma_probe_kernel<128, PREC_F16>); else go(mma_probe_kernel<256, PREC_F16>);
+        }
     };
     cudaEvent_t e0, e1;
     cudaEventCreate(&e0); cudaEventCreate(&e1);
@@ -1583,10 +1494,6 @@ int adec_probe_mma_ex(int device, int kind, int NT, int n_groups, int a_off_rows
     *tflops = flops / (t * 1e-3) / 1e12;
     if (ms) *ms = t;
     return 0;
-}
-
-int adec_probe_mma(int device, int kind, int NT, int n_groups, double* tflops, double* ms) {
-    return adec_probe_mma_ex(device, kind, NT, n_groups, 0, 128, 0, 1, tflops, ms);
 }
 
 int adec_profile(adec_handle* h, int enable) {

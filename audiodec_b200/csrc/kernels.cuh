@@ -1,4 +1,4 @@
-// audiodec_b200 device kernels (sm_100a).
+// audiodec_b200 device kernels (sm_90a).
 //
 // Everything the reference does with torch.cat + nn.Conv1d / nn.ConvTranspose1d + separate
 // activation / add kernels (layers/conv_layer.py:153-156,194-197; residual_unit.py:78-81) is one
@@ -161,19 +161,14 @@ struct ConvArgs {
     int mid_act;         // FUSE: activation between the two GEMMs
     int hist_rep;        // non-streaming forward of a transposed conv: history rows = the FIRST input row (ReplicationPad1d,
                          // conv_layer.py:189-192) instead of the stored state
-    // tcgen05 kind::f16 engine (tc_f16.cuh): weights are stored times a power of two; the drain warps multiply the sums by these
+    // fp16-split tensor-core engine (wg_conv.cuh): weights are stored times a power of two; the epilogue multiplies the sums by these
     float w_scale, w2_scale;
-    int n_wbuf;          // window buffers in shared memory (2..4)
-    int teams;           // tc_f16, un-fused launches: 2 = the 8 producer warps build alternate window pieces as two teams of 4, 1 = one team
-    int gspan;           // tc_f16: 1 = one TMEM partial per 32-channel piece (all taps) instead of one per tap pair
+    int n_wbuf;          // window buffers in shared memory (1..4)
     // stacked rows: when a stream contributes fewer rows than a 128-row tile, the tiles run over ONE row space in which stream s owns
     // rows [s * stack_L, (s + 1) * stack_L), stack_L = Tout + (Ktaps - 1) * dil: local rows >= Tout are the receptive-field overlap into
     // the next stream and are computed but never stored.  0 = one row space per stream (blockIdx-style b dimension).
     int stack_L, n_streams;
     int* err;            // device flag word: bit 1 = an activation left the fp16-split range (|a| >= 6e4)
-    int dbg_flags;       // timing experiments only (ADEC_DBG_FLAGS): bit 0 = producers skip loads / activation / split of interior pieces
-    int dbg_wdiv;        // timing experiments only (ADEC_DBG_WDIV): 0/1 = normal, k > 1 = stream 1/k of every weight stage, -1 = none (results are WRONG)
-    unsigned int* tl;    // -DADEC_TIMELINE builds: event buffer of one CTA ({code << 24 | index, clock} pairs; word 0 = count), nullptr = off
     unsigned long long* dbg;   // ADEC_KTRACE: {globaltimer at start, at end, SM cycles} of CTA 0, one record per launch (nullptr = off)
 };
 

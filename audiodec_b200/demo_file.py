@@ -29,7 +29,7 @@ def run_file(audiodec, data: np.ndarray) -> np.ndarray:
 
 def _arguments(argv):
     """Same flags as the reference demo (demoFile.py:21-27)."""
-    ap = argparse.ArgumentParser(description="wav -> AudioDec codec on a B200 -> wav")
+    ap = argparse.ArgumentParser(description="wav -> AudioDec codec on an H100 -> wav")
     ap.add_argument("--model", default="libritts_v1", help="name from assign_model's table")
     ap.add_argument("-i", "--input", required=True, help="input wav (sample rate must match the model)")
     ap.add_argument("-o", "--output", required=True, help="output wav, written as PCM_16")

@@ -3,7 +3,7 @@
 The reference's ``AudioCodecStreamer`` (bin/stream.py:80-366) serves ONE stream: a sound-card callback puts a frame on
 ``encoder_queue``, an encoder thread and a decoder thread each run a batch-1 model call per frame
 (bin/stream.py:212-239), and ``_process`` (bin/stream.py:242-278) does the latency accounting and the frame-drop policy.
-On a B200 one batch-1 call uses a sliver of the GPU, so this server generalises the same loop to N concurrent streams
+On an H100 one batch-1 call uses a sliver of the GPU, so this server generalises the same loop to N concurrent streams
 that share every launch:
 
     submit(stream, frame)      <- what the sound-card callback does with ``indata``          (bin/stream.py:248-251)

@@ -16,7 +16,7 @@ NCCL is used only for the timing barrier and the max-over-ranks of the device ti
 `roofline`   : `frac` is the WHOLE STEP against the HBM roofline under SURVEY.md 8(d)'s per-conv-layer algorithmic
                byte model (9,323.2 B/sample for symAD fp32) and MEASURED_PEAKS.json's copy bandwidth; `kernel_frac`
                is the same for the dominant launch alone; `compute` is the step against the tensor-core ceiling
-               this process measured with the library's own tcgen05 probe (adec_probe_mma).
+               this process measured with the library's own wgmma probe (adec_probe_mma).
 `parity`     : after the timed region, utterances of the timed batch against the oracle (the oracle is the checker).
 `extra_workloads` (N=1): BASELINE configs[2] (AD v1, fp32 and bf16 vocoder), configs[3] (256 streams x 1500-sample
                chunks @ 24 kHz) and the B=1 per-chunk latency the reference publishes (figs/latency.jpg Table 4).
@@ -47,7 +47,7 @@ ALG_BYTES_PER_SAMPLE = {"symad": (ENC_B + RVQ_B + SYMDEC_B) / 300.0, "v1": (ENC_
 ALG_FLOP_PER_SAMPLE = {"symad": 549432.0, "v1": 2265247.0, "v1_bf16": 2265247.0}
 ALG_BYTES_PER_SAMPLE["stream_v1"] = ALG_BYTES_PER_SAMPLE["v1"]
 ALG_FLOP_PER_SAMPLE["stream_v1"] = ALG_FLOP_PER_SAMPLE["v1"]
-FFMA_PEAK_TFLOPS = 148 * 128 * 2 * 1.965e9 / 1e12     # not measured; informational
+FFMA_PEAK_TFLOPS = 132 * 128 * 2 * 1.98e9 / 1e12      # H100 SXM: 132 SMs x 128 FP32 lanes x 2 at 1.98 GHz; not measured, informational
 WORKLOAD_NAME = {"symad": "symAD_vctk_48000_hop300", "v1": "AudioDec_v1 (symAD encoder + HiFi-GAN v1 vocoder), fp32",
                  "v1_bf16": "AudioDec_v1 (symAD encoder fp32-grade + HiFi-GAN v1 vocoder with bf16 conv operands)",
                  "stream_v1": "libritts_v1 streaming: 256 streams x 1500-sample chunks @ 24 kHz (one chunk per step)"}
@@ -60,11 +60,11 @@ def measured_peaks():
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)", d
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)", {}
+    return 3350.0, "fallback (NVIDIA H100 SXM data sheet: 3.35 TB/s HBM3, not measured)", {}
 
 
 class ClockSampler:
-    """SM clock, power and throttle reasons DURING the timed region (B200_PROFILING.md recipe).  Default source is NVML in a
+    """SM clock, power and throttle reasons DURING the timed region (measured in-process).  Default source is NVML in a
     thread of this process (the library nvidia-smi itself reads; no subprocess, 20 ms period); ADEC_BENCH_SAMPLER=smi runs the
     recipe's `nvidia-smi -lms 100` loop instead, =off disables sampling."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
@@ -201,10 +201,11 @@ def workload_shape(workload):
 
 
 def codec_step(tx, rx, dec, x):
+    """One pass of the path; returns what its caller receives: waveform, code indices, latent z, quantized latent zq."""
     z = tx.encode(x)
     idx = tx.quantize(z)
     zq = rx.lookup(idx)
-    return dec.decode(zq), idx
+    return dec.decode(zq), idx, z, zq
 
 
 def parity_vs_oracle(workload, dev, x_batch, sel, chunks=1):
@@ -220,7 +221,7 @@ def parity_vs_oracle(workload, dev, x_batch, sel, chunks=1):
     ys, idxs, rys, ridxs, rzs = [], [], [], [], []
     for c in range(chunks):
         xc = xs[:, :, c * T:(c + 1) * T].contiguous()
-        y, idx = codec_step(tx, rx, dec, xc.to(dev))
+        y, idx = codec_step(tx, rx, dec, xc.to(dev))[:2]
         ys.append(y.cpu()), idxs.append(idx.cpu() if idx.dim() == 3 else idx.cpu().unsqueeze(1))
         with torch.no_grad():
             rz, ridx, _, ry = orc.run(xc[sel])
@@ -357,6 +358,15 @@ def measure_latency_b1(dev, chunks=60):
     return out
 
 
+def dump_outputs(out_dir, arrays):
+    """What the last timed step returned to its caller, as <name>.npy: float tensors as float32, integer ones as float64 (exact)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy()
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float32 if a.dtype.kind == "f" else np.float64))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -382,7 +392,7 @@ def run_ours(args):
     x_dev = [x.to(dev) for x in x_host]
 
     def step(i):
-        return codec_step(tx, rx, dec, x_dev[i % n_in])[0]
+        return codec_step(tx, rx, dec, x_dev[i % n_in])
 
     def barrier():
         if world > 1:
@@ -399,7 +409,7 @@ def run_ours(args):
     # pre-warm: clocks / power state settle over the first ~second of load; these steps are not counted in W.  The clock sampler
     # starts BEFORE the warm-up steps and nothing idles between warm-up and the timed region: a 250 ms pause there (round 1 slept to let
     # the sampler spin up) lets some boxes drop their power state, and the first timed steps then run at ramping clocks (measured with
-    # tools/ktrace.py: same kernels, 10.2 ms per step back to back, but 12.4 ms in a timed region entered after the pause).
+    # per-launch kernel traces: the same kernels ran ~20 % slower in a timed region entered after the pause).
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()
@@ -411,9 +421,8 @@ def run_ours(args):
         step(i)
     # The timed region - EXACTLY K steps between barrier + synchronize on both sides, device time by CUDA events, max over ranks - is
     # measured `--regions` R times back to back and the MEDIAN region is reported (all R values are on the line as
-    # `timed_regions_ms_per_step`).  Reason: on these power-capped boxes (sw_power_cap at ~1 kW) about one region in four runs 15-60 %
-    # slow for its ~100 ms (three of twelve single-region runs of the same build in round 2: 10.0 .. 10.3 ms vs 11.8 / 15.2 / 16.0),
-    # while the e2e loop and the per-launch event sums of the same process stay put; a single region is a coin flip, the median is not.
+    # `timed_regions_ms_per_step`).  Reason: on a shared, power-limited GPU an occasional region runs slow while the rest stay put;
+    # a single region is a coin flip, the median is not.
     regions = []
     for r in range(max(1, args.regions)):
         l0 = tx.launch_count + rx.launch_count + dec.launch_count
@@ -422,7 +431,7 @@ def run_ours(args):
         w0 = time.time()
         e0.record()
         for i in range(args.steps):
-            y = step(i)
+            y, idx, z, zq = step(i)
         e1.record()
         barrier()
         w1 = time.time()
@@ -441,9 +450,10 @@ def run_ours(args):
             per.append(a0.elapsed_time(a1))
         print(f"synced per-step ms: {[round(v, 3) for v in per]}; back-to-back mean {ms_total / args.steps:.3f}", file=sys.stderr)
     launches = (tx.launch_count + rx.launch_count + dec.launch_count - l0)
-    dbg_run = any(k.startswith("ADEC_DBG_") for k in os.environ)    # timing experiments with deliberately wrong results (tools/gpu_dbg.sh)
-    assert dbg_run or torch.isfinite(y).all()
-    if not dbg_run and (tx.range_error() or dec.range_error()):
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"waveform": y, "code_indices": idx, "z": z, "zq": zq})
+    assert torch.isfinite(y).all()
+    if tx.range_error() or dec.range_error():
         raise SystemExit("an activation left the fp16-split range of the conv engine: results invalid")
 
     # ---- e2e: host buffers through adec_codec_host (H2D + 4 calls + D2H inside the timed region)
@@ -498,24 +508,16 @@ def run_ours(args):
     per_gpu = value / world
     alg_b = ALG_BYTES_PER_SAMPLE[args.workload]
     achieved = alg_b * per_gpu / 1e9
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if prof and os.path.exists(tpath):
-        with open(tpath) as f:
-            tj = json.load(f)
-        for key, val in tj.items():
-            if key != "_comment" and key in prof["kernel"]:
-                traffic = val
     k_achieved = prof["alg_bytes_per_launch"] / (prof["launch_ms"] * 1e-3) / 1e9 if prof else achieved
     conv_path = os.environ.get("ADEC_CONV_PATH", "f16")
-    engine = {"f16": "tc_conv_f16_kernel (tcgen05 kind::f16, fp16-split operands x3 products)", "tc": "tc_conv_f16_kernel (tcgen05 kind::f16)",
-              "tf32": "tc_conv_persist_kernel (tcgen05 3xTF32)", "ffma": "conv_gemm_kernel (fp32 FFMA)"}.get(conv_path, conv_path)
+    engine = {"f16": "wg_conv_kernel (wgmma, fp16-split operands x3 products)", "tc": "wg_conv_kernel (wgmma, fp16-split operands x3 products)",
+              "tf32": "wg_conv_kernel (wgmma 3xTF32)", "ffma": "conv_gemm_kernel (fp32 FFMA)"}.get(conv_path, conv_path)
     # compute ceiling: measured here with the library's own MMA-only probe; the tensor-core engines issue 3 MMAs per fp32-grade MAC
     probe = probe_compute(local)
     useful_tflops = ALG_FLOP_PER_SAMPLE[args.workload] * per_gpu / 1e12
     mma_per_mac = {"f16": 3.0, "tc": 3.0, "tf32": 3.0, "ffma": None}.get(conv_path)
     pk = probe.get("tf32_n256_tflops" if conv_path == "tf32" else "f16_n256_tflops")
-    compute = {"probe": "adec_probe_mma: every SM streams tcgen05.mma M=128 x N from shared-memory operands, nothing else",
+    compute = {"probe": "adec_probe_mma: every SM streams wgmma (2 warpgroups x M=64, N in 64-column slices) from shared-memory operands, nothing else",
                "measured_tflops": probe, "useful_tflops": useful_tflops, "tensor_products_per_useful_mac": mma_per_mac,
                "issued_tflops": useful_tflops * mma_per_mac if mma_per_mac else None,
                "peak_tflops": pk, "frac": (useful_tflops * mma_per_mac / pk) if (mma_per_mac and pk) else None,
@@ -531,16 +533,13 @@ def run_ours(args):
         "data": "synthetic (0.1*randn waveforms, seeded synthetic checkpoint; the reference ships no weights)",
         "config": {"workload": WORKLOAD_NAME[args.workload] + f" batch={B}x{T} per GPU (BASELINE configs[{WORKLOAD_CFG[args.workload]}])",
                    "utterances_per_gpu": B, "samples_per_utterance": T, "parallelism": f"independent utterance shards x{world}, no collective",
-                   "l2": "per-step activation working set ~3 GB per GPU >> 126 MB L2; inputs rotate over 4 distinct resident batches",
+                   "l2": "per-step activation working set ~3 GB per GPU >> 50 MB L2; inputs rotate over 4 distinct resident batches",
                    "realtime_factor_per_gpu": per_gpu / sr},
         "gpu_launches": int(launches),
         "e2e": {"value": e2e_value, "unit": "samples/s", "h2d_bytes_per_step": B * T * 4,
                 "d2h_bytes_per_step": B * F * hop * 4 + 8 * B * F * 8, "ms_per_step": ms_e2e / args.steps,
                 "api": "audiodec_b200.codec.codec_host -> adec_codec_host (pinned host buffers, per GPU)"},
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": traffic,
-                     "traffic_source": ("stored constant from profiles/traffic.json (ncu --set full capture of the dominant kernel), not re-measured "
-                                        "in this run") if traffic else None,
                      "peak_source": peak_src,
                      "model": f"whole step: {alg_b:.1f} algorithmic B/sample (SURVEY.md 8(d) per-conv-layer model) x samples/s per GPU",
                      "kernel": engine + " launch of " + (prof["kernel"] if prof else "?"),
@@ -728,7 +727,7 @@ def run_reference(args):
         "config": {"workload": WORKLOAD_NAME[args.workload] + f" batch={B}x{T} per GPU (BASELINE configs[{WORKLOAD_CFG[args.workload]}]); "
                                "each step a bounded sample of it",
                    "note": "reference = pure-Python torch-CPU path; timed via the oracle port (identical torch ops/order) because "
-                           "/root/reference does not exist on the GPU box; rank 0 only; value = best of one process (median over steps) and "
+                           "the reference is not installed where the benchmark runs; rank 0 only; value = best of one process (median over steps) and "
                            "all-cores multi-process"},
         "cpu_baseline": dict(last, value=value, one_process=one_proc, all_cores=allc, cores=allc.get("cores", last["cores"])),
         "e2e": {"value": value, "unit": "samples/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
@@ -754,7 +753,14 @@ def main():
     ap.add_argument("--ref-utts", type=int, default=16, help="--impl reference: utterances per step (each step time-bounded at 15 s)")
     ap.add_argument("--regions", type=int, default=5, help="timed K-step regions measured back to back; the median is reported, all are listed")
     ap.add_argument("--breakdown", action="store_true", help="print per-launch CUDA-event times to stderr")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="--impl ours: write the last timed step's outputs to DIR/<name>.npy - waveform (B,1,T), z (B,D,F) and zq (B,F,D) "
+                         "as float32, code_indices (Nq,B,F) as float64")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs applies to --impl ours only")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.impl == "reference":
         run_reference(args)

@@ -1,5 +1,5 @@
 /*
- * audiodec_b200 - C ABI of the B200-native AudioDec streaming forward path.
+ * audiodec_b200 - C ABI of the H100-native AudioDec streaming forward path.
  *
  * This is the drop-in boundary (SURVEY.md section 8(b)).  The reference has no FFI: its
  * plug points are the two abstract hooks AudioCodec._load_encoder / _load_decoder
@@ -141,7 +141,7 @@ int adec_lookup_packed(adec_handle *h, const uint8_t *packed, int B, int F, floa
  * out-of-range index since the last call (the reference's F.embedding would have raised, vq_module.py:160), -1 on error */
 int adec_index_error(adec_handle *h, void *stream);
 /* same protocol for the conv engine's range flag: 1 if an activation reached |a| >= 6e4 since the last call.  The default engine
- * multiplies fp16 pieces of the fp32 activations (tc_f16.cuh); the reference's fp32 convs (layers/conv_layer.py:55-64) have no such
+ * multiplies fp16 pieces of the fp32 activations (wg_conv.cuh); the reference's fp32 convs (layers/conv_layer.py:55-64) have no such
  * bound, so a model that gets there must run with ADEC_CONV_PATH=tf32.  adec_codec_host checks both flags itself. */
 int adec_range_error(adec_handle *h, void *stream);
 
@@ -153,15 +153,10 @@ int64_t adec_launch_count(const adec_handle *h);
  * number of records or -1.  Used to measure the effective SM clock and the gaps between back-to-back launches. */
 int adec_ktrace(adec_handle *h, unsigned long long *out, int max_records);
 
-/* Measured compute ceiling of the conv engine for bench.py's roofline: every SM streams `n_groups` x 12 tcgen05.mma (M = 128, N = NT,
- * kind 0 = tf32 / 1 = f16) from shared-memory operands in the engine's layout, nothing else; *tflops = dense TFLOP/s, *ms = duration
- * (may be NULL).  No handle needed. */
+/* Measured compute ceiling of the conv engine for bench.py's roofline: every SM streams `n_groups` x 12 wgmma per 64-column slice
+ * (M = 2 x 64, N = NT in {32, 64, 128, 256}, kind 0 = tf32 / 1 = f16) from shared-memory operands in the engine's layout, nothing else;
+ * *tflops = dense TFLOP/s, *ms = duration (may be NULL).  No handle needed. */
 int adec_probe_mma(int device, int kind, int NT, int n_groups, double *tflops, double *ms);
-/* Same with the A operand placed like a conv window: first row a_off_rows, a_pitch_rows rows per 16-byte K block (LBO), and MMA k of a
- * group reading rows shifted by (k % 7) * tap_step_rows - measures what a tap's row-shifted, non-128-byte-aligned start address costs; n_issuers (1..4) warps issue the
- * groups round robin, each group on its own TMEM accumulator, without ordering between the warps. */
-int adec_probe_mma_ex(int device, int kind, int NT, int n_groups, int a_off_rows, int a_pitch_rows, int tap_step_rows, int n_issuers,
-                      double *tflops, double *ms);
 
 /* Per-launch CUDA-event timing on the handle's stream (bench.py's roofline leg).  adec_profile(h,1) starts
  * recording around every kernel launch, adec_profile(h,0) stops and clears.  adec_profile_report writes one line

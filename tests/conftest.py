@@ -10,12 +10,12 @@ GOLDEN = os.path.join(REPO, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
     """`pytest tests` on a machine without a CUDA device (or without the built library) skips the gpu-marked tests instead of
-    failing them; `-m gpu` on the B200 box runs them."""
+    failing them; `-m gpu` on an H100 runs them."""
     import torch
     lib = os.path.join(REPO, "audiodec_b200", "lib", "libaudiodec_b200.so")
     reason = None
@@ -49,7 +49,7 @@ def hifigan_sd():
 
 @pytest.fixture(params=["f16", "tf32", "ffma"])
 def conv_path(request, monkeypatch):
-    """The conv engines behind the same C ABI: tcgen05 kind::f16 with fp16-split operands (default), the round-1 tcgen05 3xTF32
-    kernels and the CUDA-core FFMA kernels.  The library reads ADEC_CONV_PATH when a handle is created."""
+    """The conv engines behind the same C ABI: wgmma with fp16-split operands (default), wgmma 3xTF32 and the CUDA-core FFMA
+    kernels.  The library reads ADEC_CONV_PATH when a handle is created."""
     monkeypatch.setenv("ADEC_CONV_PATH", request.param)
     return request.param
