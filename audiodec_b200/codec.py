@@ -15,6 +15,9 @@ Differences from the reference, all extensions:
     ``ResidualVQ.forward_index`` yields before its ``squeeze(1)``, vq_module.py:148-149) and ``lookup``
     returns (B,F,D).
   * there is no CPU path: ``.to('cpu')`` raises.
+  * ``HiFiGANStreamGenerator.set_activation_dtype(torch.bfloat16)`` keeps every activation, the causal state and the decode
+    input / output in bf16 (the data layout and dtype contract of the reference's ``decoder.to(torch.bfloat16)``); plain
+    ``.to(torch.bfloat16)`` rounds only the conv operands and keeps fp32 activations and fp32 I/O.
 """
 from __future__ import annotations
 
@@ -49,6 +52,8 @@ class _StreamGeneratorBase:
         self._sd = None
         self._h = None
         self._device = None
+        self._operand_mode = 0        # what .to(dtype) selected: 0 = fp32, 1 = bf16 conv operands
+        self._act_bf16 = False        # HiFi-GAN only (set_activation_dtype): bf16 activations, state and decode I/O = compute_dtype 2
 
     # -- torch.nn.Module look-alikes ------------------------------------------------------------
     def load_state_dict(self, state_dict, strict=True):
@@ -93,10 +98,16 @@ class _StreamGeneratorBase:
             want = 1
         else:
             raise NotImplementedError(f"{type(self).__name__} has no {dtype} mode (fp32 everywhere; bf16 for the HiFi-GAN vocoder only)")
-        if self._h is not None and want != self._cfg.compute_dtype:
+        mode = 2 if self._act_bf16 else want
+        if self._h is not None and mode != self._cfg.compute_dtype:
             raise RuntimeError("set the compute dtype before .to(device): the weights are packed when the handle is created")
-        self._cfg.compute_dtype = want
+        self._operand_mode = want
+        self._cfg.compute_dtype = mode
         return self
+
+    def set_activation_dtype(self, dtype):
+        raise NotImplementedError(f"{type(self).__name__} keeps fp32 activations: the encoder, projector and RVQ must stay fp32-grade "
+                                  "for bit-identical indices (bf16 activations are built for the HiFi-GAN vocoder only)")
 
     def bfloat16(self):
         return self._set_dtype(torch.bfloat16)
@@ -371,11 +382,13 @@ class SymADStreamGenerator(_StreamGeneratorBase):
 def _decode_offline(gen, zq):
     gen._ready()
     gen._want(zq, "decode_offline / forward", 1, getattr(gen, "code_dim", None) or gen.in_channels)
-    zq = gen._in(zq)
+    dtype = torch.bfloat16 if gen._act_bf16 else torch.float32
+    zq = gen._in(zq, dtype)
     b, _, f = zq.shape
     zq_cl = zq.transpose(1, 2).contiguous()                       # the kernels' native channels-last (B,F,D)
-    y = torch.empty(b, 1, f * gen._lib.adec_hop_length(gen._h), device=gen._device, dtype=torch.float32)
-    _check(gen._lib.adec_decode_offline(gen._h, _ptr(zq_cl), b, f, _ptr(y), gen._stream()), gen._h)
+    y = torch.empty(b, 1, f * gen._lib.adec_hop_length(gen._h), device=gen._device, dtype=dtype)
+    fn = gen._lib.adec_decode_offline_bf16 if gen._act_bf16 else gen._lib.adec_decode_offline
+    _check(fn(gen._h, _ptr(zq_cl), b, f, _ptr(y), gen._stream()), gen._h)
     return y
 
 
@@ -414,18 +427,36 @@ class HiFiGANStreamGenerator(_StreamGeneratorBase):
         c.has_stats = int(stats is not None)       # mean/scale themselves come from the state dict (HiFiGAN.py:206-219)
         self.in_channels = in_channels
 
+    def set_activation_dtype(self, dtype):
+        """torch.bfloat16: every activation, the causal state, and decode's zq input and y output are bf16 (conv operands bf16, fp32
+        accumulation, one rounding per stored value) - what the reference's `decoder.to(torch.bfloat16)` stores and returns.
+        torch.float32: back to fp32 activations with the operand precision `.to(dtype)` chose.  Call before `.to(device)`; returns
+        self, so `d.set_activation_dtype(torch.bfloat16).to(dev)` chains."""
+        if dtype not in (torch.float32, torch.bfloat16):
+            raise NotImplementedError(f"HiFiGANStreamGenerator has no {dtype} activation mode (float32 or bfloat16)")
+        if self._h is not None:
+            raise RuntimeError("set the activation dtype before .to(device): the state and workspaces are laid out when the handle is created")
+        self._act_bf16 = dtype == torch.bfloat16
+        self._cfg.compute_dtype = 2 if self._act_bf16 else self._operand_mode
+        return self
+
     def initial_decoder(self, c):
         self.decode(c)                                                                # HiFiGAN.py:264-265
 
     def decode(self, c):
-        """zq (B,F,in_channels) channels-last -> y (B,1,F*prod(scales)) in (-1,1)   (HiFiGAN.py:268-296)"""
+        """zq (B,F,in_channels) channels-last -> y (B,1,F*prod(scales)) in (-1,1)   (HiFiGAN.py:268-296).  With bf16 activations
+        zq may be bf16 or fp32 (cast on the device) and y is bf16."""
         self._ready()
         self._want(c, "decode", 2, self.in_channels)
-        c = self._in(c)
+        dtype = torch.bfloat16 if self._act_bf16 else torch.float32
+        c = self._in(c, dtype)
+        if self._act_bf16 and c.data_ptr() % 16:
+            c = c.clone()                  # the bf16 kernels read zq as 16-byte vectors: realign an offset view
         b, f, _ = c.shape
         self._batch(b)
-        y = torch.empty(b, 1, f * self._lib.adec_hop_length(self._h), device=self._device, dtype=torch.float32)
-        _check(self._lib.adec_decode(self._h, _ptr(c), b, f, _ptr(y), self._stream()), self._h)
+        y = torch.empty(b, 1, f * self._lib.adec_hop_length(self._h), device=self._device, dtype=dtype)
+        fn = self._lib.adec_decode_bf16 if self._act_bf16 else self._lib.adec_decode
+        _check(fn(self._h, _ptr(c), b, f, _ptr(y), self._stream()), self._h)
         return y
 
     def forward(self, c):

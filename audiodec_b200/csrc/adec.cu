@@ -93,15 +93,15 @@ const ConvKernelCfg* find_conv_kernel(int CW, int CO, bool fuse) {
 }
 
 // tensor-core engine (wg_conv.cuh): PREC_F16 = two fp16 pieces per operand, three products (fp32-grade, default); PREC_TF32 = 3xTF32
-// (ADEC_CONV_PATH=tf32); PREC_BF16 = bf16 operands, one product (the vocoder's bf16 mode).  Persistent: one CTA per SM loops over
-// (time tile, channel tile, stream) tiles.
+// (ADEC_CONV_PATH=tf32); PREC_BF16 = bf16 operands, one product (the vocoder's bf16 modes; BST = bf16 activations in HBM as well).
+// Persistent: one CTA per SM loops over (time tile, channel tile, stream) tiles.
 typedef cudaError_t (*TcPersistFn)(const ConvArgs&, int, int, int, int, int, cudaStream_t);
-template <int NT, bool F, int PRE, int PREC>
+template <int NT, bool F, int PRE, int PREC, bool BST>
 cudaError_t launch_wg(const ConvArgs& a, int n_xtiles, int n_ytiles, int n_tiles, int n_ctas, int smem_bytes, cudaStream_t s) {
     static bool configured[64] = {false};
     int dev = 0;
     cudaGetDevice(&dev);
-    auto kern = wg_conv_kernel<NT, F, PRE, PREC>;
+    auto kern = wg_conv_kernel<NT, F, PRE, PREC, BST>;
     constexpr int kMaxDyn = 227 * 1024;
     if (dev < 64 && !configured[dev]) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn);
@@ -127,21 +127,21 @@ cudaError_t launch_wg(const ConvArgs& a, int n_xtiles, int n_ytiles, int n_tiles
 }
 typedef size_t (*TcSmemFn)(int, bool);
 typedef int (*TcWbufFn)(int, bool);
-struct TcKernelCfg { int NT; bool fuse; int pre, prec, tap_bytes; TcPersistFn pfn; TcSmemFn smem; TcWbufFn n_wbuf; };
-#define ADEC_TC1(NT, F, PRE, PREC) \
-    {NT, F, PRE, PREC, WgCfg<NT, PREC>::TAP_BYTES, launch_wg<NT, F, PRE, PREC>, WgCfg<NT, PREC>::smem_bytes, WgCfg<NT, PREC>::n_wbuf}
+struct TcKernelCfg { int NT; bool fuse; int pre, prec; bool bst; int tap_bytes; TcPersistFn pfn; TcSmemFn smem; TcWbufFn n_wbuf; };
+#define ADEC_TC1(NT, F, PRE, PREC, BST) \
+    {NT, F, PRE, PREC, BST, WgCfg<NT, PREC>::TAP_BYTES, launch_wg<NT, F, PRE, PREC, BST>, WgCfg<NT, PREC>::smem_bytes, WgCfg<NT, PREC>::n_wbuf}
 #define ADEC_TC_FP32(NT, PREC) \
-    ADEC_TC1(NT, true, ACT_ELU, PREC), ADEC_TC1(NT, false, ACT_NONE, PREC), ADEC_TC1(NT, false, ACT_ELU, PREC), ADEC_TC1(NT, false, ACT_LRELU, PREC), \
-    ADEC_TC1(NT, false, ACT_NORM, PREC)
-#define ADEC_TC(NT) \
-    ADEC_TC_FP32(NT, PREC_F16), ADEC_TC_FP32(NT, PREC_TF32), \
-    ADEC_TC1(NT, false, ACT_NONE, PREC_BF16), ADEC_TC1(NT, false, ACT_LRELU, PREC_BF16), ADEC_TC1(NT, false, ACT_NORM, PREC_BF16)
+    ADEC_TC1(NT, true, ACT_ELU, PREC, false), ADEC_TC1(NT, false, ACT_NONE, PREC, false), ADEC_TC1(NT, false, ACT_ELU, PREC, false), \
+    ADEC_TC1(NT, false, ACT_LRELU, PREC, false), ADEC_TC1(NT, false, ACT_NORM, PREC, false)
+#define ADEC_TC_BF16(NT, BST) \
+    ADEC_TC1(NT, false, ACT_NONE, PREC_BF16, BST), ADEC_TC1(NT, false, ACT_LRELU, PREC_BF16, BST), ADEC_TC1(NT, false, ACT_NORM, PREC_BF16, BST)
+#define ADEC_TC(NT) ADEC_TC_FP32(NT, PREC_F16), ADEC_TC_FP32(NT, PREC_TF32), ADEC_TC_BF16(NT, false), ADEC_TC_BF16(NT, true)
 const TcKernelCfg kTcKernels[] = {ADEC_TC(128), ADEC_TC(64), ADEC_TC(32)};
 int kTcMaxFuse = 128;    // residual units wider than this run as two launches on the tensor-core path (ADEC_TC_MAXFUSE)
 
-const TcKernelCfg* find_tc_kernel(int NT, bool fuse, int pre, int prec) {
+const TcKernelCfg* find_tc_kernel(int NT, bool fuse, int pre, int prec, bool bst) {
     for (const auto& k : kTcKernels)
-        if (k.NT == NT && k.fuse == fuse && k.pre == pre && k.prec == prec) return &k;
+        if (k.NT == NT && k.fuse == fuse && k.pre == pre && k.prec == prec && k.bst == bst) return &k;
     return nullptr;
 }
 
@@ -218,7 +218,9 @@ struct adec_handle {
     int st_cap = 1;        // streams the state buffers were allocated for
     int engine = 2;               // ADEC_CONV_PATH: 2 = f16 (fp16-split wgmma, default), 1 = tf32 (3xTF32 wgmma), 0 = ffma (CUDA cores)
     bool use_tc = true;           // any tensor-core engine
-    bool bf16 = false;            // cfg.compute_dtype == 1: bf16 operands (HiFi-GAN vocoder, f16 engine only)
+    bool bf16 = false;            // cfg.compute_dtype >= 1: bf16 operands (HiFi-GAN vocoder, f16 engine only)
+    bool act_bf16 = false;        // cfg.compute_dtype == 2: bf16 activations, causal state and decode I/O as well
+    int act_bytes() const { return act_bf16 ? 2 : 4; }   // bytes per stored activation / state element
     bool stack_rows = true;       // ADEC_STACK_ROWS=0: never stack several streams' rows into one tile (A/B)
     unsigned long long* d_ktrace = nullptr;   // ADEC_KTRACE=1: per-launch {start ns, end ns, SM cycles} records (diagnostics)
     int ktrace_n = 0;
@@ -428,7 +430,7 @@ int finalize_op_tc(adec_handle* h, Op* op) {
     // same activation window (the epilogue masks per column pair)
     const bool pad_tile = !op->fuse && NT == 32 && op->Cout > 64 && op->Cout < 128;
     if (pad_tile) NT = 128;
-    op->tc = find_tc_kernel(NT, op->fuse, op->pre_act, PREC_TF32);
+    op->tc = find_tc_kernel(NT, op->fuse, op->pre_act, PREC_TF32, false);
     if (!op->tc || (op->fuse && (NT != op->Cout || op->mid_act != op->pre_act))) return h->fail(op->name + ": no tensor-core kernel");
     const int KS = TC_CP, CP = TC_CP;
     op->n_pieces = op->Cin_eff / CP;
@@ -479,7 +481,8 @@ int finalize_op_f16(adec_handle* h, Op* op) {
     const bool pad_tile = !op->fuse && NT == 32 && op->Cout > 64 && op->Cout < 128;     // e.g. transposed conv 64 -> 3*32: one padded 128-wide tile
     if (pad_tile) NT = 128;
     const int prec = (h->bf16 && !op->fuse) ? PREC_BF16 : PREC_F16;
-    op->tc = find_tc_kernel(NT, op->fuse, op->pre_act, prec);
+    if (h->act_bf16 && op->RG > 1) return h->fail(op->name + ": bf16 activations are built for stride-1 and transposed convs only");
+    op->tc = find_tc_kernel(NT, op->fuse, op->pre_act, prec, h->act_bf16);
     if (!op->tc || (op->fuse && (NT != op->Cout || op->mid_act != op->pre_act))) return h->fail(op->name + ": no tensor-core kernel");
     const int CP = TC_CP, KB = TC_CP / 8, npl = prec == PREC_F16 ? 3 : 1;
     op->n_pieces = op->Cin_eff / CP;
@@ -583,16 +586,19 @@ int finalize_op(adec_handle* h, Op* op) {
 }
 
 int alloc_state(adec_handle* h, Op* op, int n_streams) {
-    const size_t per = (size_t)op->P * op->st_C;
+    const size_t per = (size_t)op->P * op->st_C, eb = h->act_bytes();
     if (per == 0) return 0;
     for (int i = 0; i < 2; ++i) {
-        CK(h, cudaMalloc((void**)&op->st[i], per * n_streams * sizeof(float)));     // owned by the op: freed on resize / destroy
-        CK(h, cudaMemset(op->st[i], 0, per * n_streams * sizeof(float)));
+        CK(h, cudaMalloc((void**)&op->st[i], per * n_streams * eb));     // owned by the op: freed on resize / destroy
+        CK(h, cudaMemset(op->st[i], 0, per * n_streams * eb));
     }
     op->cur = 0;
     if (!op->hstate.empty()) {
+        std::vector<uint16_t> hb;       // bf16 activations: the checkpoint's pad_buffer rounded once, like `.to(torch.bfloat16)`
+        if (h->act_bf16) for (float v : op->hstate) hb.push_back(bf16_bits(v));
+        const void* src = h->act_bf16 ? (const void*)hb.data() : (const void*)op->hstate.data();
         for (int s = 0; s < n_streams; ++s)
-            CK(h, cudaMemcpy(op->st[0] + s * per, op->hstate.data(), per * sizeof(float), cudaMemcpyHostToDevice));
+            CK(h, cudaMemcpy((char*)op->st[0] + s * per * eb, src, per * eb, cudaMemcpyHostToDevice));
     }
     return 0;
 }
@@ -638,8 +644,8 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
             T = Tout * op.up;
         }
     }
-    for (int i = 0; i < 3; ++i)
-        if (need[i] && ensure(h, h->ws[i], need[i])) return 1;
+    for (int i = 0; i < 3; ++i)     // need[] counts elements; the buffers are sized in floats
+        if (need[i] && ensure(h, h->ws[i], (need[i] * h->act_bytes() + 3) / 4)) return 1;
     if (rc.B != h->n_streams) return h->fail(fmt("batch %d != n_streams %d (call adec_set_streams)", rc.B, h->n_streams));
 
     int T = T_in;
@@ -668,7 +674,8 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
             a.w = op.w; a.bias = op.head_bias; a.pre_act = op.pre_act; a.slope = op.slope; a.post_tanh = op.post_tanh;
             a.y = yout; a.y_bs = T;
             dim3 grid((T + 255) / 256, rc.B);
-            head_kernel<32, 7><<<grid, 256, 0, rc.stream>>>(a);
+            if (h->act_bf16) head_kernel<32, 7, true><<<grid, 256, 0, rc.stream>>>(a);
+            else head_kernel<32, 7, false><<<grid, 256, 0, rc.stream>>>(a);
             e = cudaGetLastError();
         } else {
             ConvArgs a{};
@@ -720,12 +727,14 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
             cudaEventRecord(ev1, rc.stream);
             h->prof_events.emplace_back(ev0, ev1);
             h->prof_names.push_back(op.name);
-            // algorithmic bytes: 4*(Cin*Tin + Cout*Tout [+ Cout*Tout residual]) per stream (fused unit: its two convs + skip)
+            // algorithmic bytes: eb*(Cin*Tin + Cout*Tout [+ Cout*Tout residual]) per stream (fused unit: its two convs + skip), eb = 4 for
+            // fp32 activations, 2 for bf16
             const double cin = op.kind == OP_STEM ? 1 : (double)op.G * op.Cin_eff / std::max(1, op.RG) * (op.shared_in ? 1.0 / op.G : 1.0);
             const double cout = op.kind == OP_HEAD ? 1 : (double)op.G * op.Cout;
-            double bytes = 4.0 * rc.B * (cin * T + cout * Tout);
-            if (op.fuse) bytes += 4.0 * rc.B * (3.0 * cout * Tout);      // mid write+read (1x1 conv in/out) and the skip read
-            else if (op.res_buf >= 0) bytes += 4.0 * rc.B * cout * Tout;
+            const double eb = h->act_bytes();
+            double bytes = eb * rc.B * (cin * T + cout * Tout);
+            if (op.fuse) bytes += eb * rc.B * (3.0 * cout * Tout);      // mid write+read (1x1 conv in/out) and the skip read
+            else if (op.res_buf >= 0) bytes += eb * rc.B * cout * Tout;
             h->prof_bytes.push_back(bytes);
         }
         if (op.P > 0) op.cur ^= 1;
@@ -1111,11 +1120,21 @@ int adec_create(const adec_config* cfg, int device, adec_handle** out) {
     if (const char* kt = getenv("ADEC_KTRACE")) {
         if (atoi(kt)) { DeviceGuard dgk(device); cudaMalloc((void**)&h->d_ktrace, 4096 * 3 * sizeof(unsigned long long)); }
     }
-    h->bf16 = cfg->compute_dtype == 1;
-    if (cfg->compute_dtype != 0 && cfg->compute_dtype != 1) { g_create_error = "compute_dtype must be 0 (fp32) or 1 (bf16)"; delete h; return 1; }
+    h->bf16 = cfg->compute_dtype == 1 || cfg->compute_dtype == 2;
+    h->act_bf16 = cfg->compute_dtype == 2;
+    if (cfg->compute_dtype < 0 || cfg->compute_dtype > 2) {
+        g_create_error = "compute_dtype must be 0 (fp32), 1 (bf16 operands) or 2 (bf16 operands and activations)";
+        delete h;
+        return 1;
+    }
     if (h->bf16 && (cfg->model_type != ADEC_MODEL_HIFIGAN || h->engine != 2)) {
         g_create_error = "compute_dtype = bf16 is built for the HiFi-GAN vocoder on the f16 tensor-core engine only (the encoder, projector and RVQ "
                          "must stay fp32-grade for bit-identical indices)";
+        delete h;
+        return 1;
+    }
+    if (h->act_bf16 && cfg->in_channels % 8) {      // a bf16 zq row must be whole 16-byte vectors
+        g_create_error = "compute_dtype = 2 needs in_channels to be a multiple of 8";
         delete h;
         return 1;
     }
@@ -1189,7 +1208,8 @@ static int resize_state(adec_handle* h, int n, bool replicate) {
     CK(h, cudaDeviceSynchronize());
     for (auto* ops : {&h->enc_ops, &h->dec_ops})
         for (Op& op : *ops) {
-            const size_t per = (size_t)op.P * op.st_C;
+            // per-stream state in 4-byte words (bf16 state: st_C is a multiple of 32, so a stream's rows are whole words)
+            const size_t per = (size_t)op.P * op.st_C * h->act_bytes() / 4;
             if (!per) continue;
             if (n > h->st_cap) {
                 float* nb[2] = {nullptr, nullptr};
@@ -1237,7 +1257,7 @@ int adec_reset(adec_handle* h, void* stream) {
         for (Op& op : *ops) {
             const size_t per = (size_t)op.P * op.st_C;
             if (!per) continue;
-            for (int i = 0; i < 2; ++i) CK(h, cudaMemsetAsync(op.st[i], 0, per * h->n_streams * sizeof(float), (cudaStream_t)stream));
+            for (int i = 0; i < 2; ++i) CK(h, cudaMemsetAsync(op.st[i], 0, per * h->n_streams * h->act_bytes(), (cudaStream_t)stream));
         }
     return 0;
 }
@@ -1260,12 +1280,30 @@ int adec_encode(adec_handle* h, const float* x, int B, int T, float* z, void* st
     return run_ops(h, h->enc_ops, rc, T, nullptr);
 }
 
-int adec_decode(adec_handle* h, const float* zq, int B, int F, float* y, void* stream) {
+// decode / decode_offline in either activation dtype: the entry point's I/O dtype must be the handle's (compute_dtype 2 = bf16)
+static int decode_common(adec_handle* h, const void* zq, int B, int F, void* y, void* stream, bool offline, bool bf16_io) {
     if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    if (B < 1 || F < 1) return h->fail("decode: empty input");
+    const char* name = offline ? (bf16_io ? "decode_offline_bf16" : "decode_offline") : (bf16_io ? "decode_bf16" : "decode");
+    if (h->act_bf16 && !bf16_io)
+        return h->fail(fmt("%s: this handle has bf16 activations (compute_dtype 2); call adec_%s_bf16 with bf16 zq / y", name,
+                           offline ? "decode_offline" : "decode"));
+    if (!h->act_bf16 && bf16_io)
+        return h->fail(fmt("%s: this handle has fp32 activations (compute_dtype %d); call adec_%s with fp32 zq / y", name, h->cfg.compute_dtype,
+                           offline ? "decode_offline" : "decode"));
+    if (bf16_io && (((uintptr_t)zq | (uintptr_t)y) & 15)) return h->fail(fmt("%s: zq and y must be 16-byte aligned", name));
+    if (B < 1 || F < 1) return h->fail(fmt("%s: empty input", name));
     DeviceGuard dg(h->device);
-    RunCtx rc{B, zq, y, (cudaStream_t)stream};
+    if (offline && offline_state(h, B, (cudaStream_t)stream)) return 1;
+    RunCtx rc{B, (const float*)zq, (float*)y, (cudaStream_t)stream, offline};
     return run_ops(h, h->dec_ops, rc, F, nullptr);
+}
+
+int adec_decode(adec_handle* h, const float* zq, int B, int F, float* y, void* stream) {
+    return decode_common(h, zq, B, F, y, stream, false, false);
+}
+
+int adec_decode_bf16(adec_handle* h, const uint16_t* zq, int B, int F, uint16_t* y, void* stream) {
+    return decode_common(h, zq, B, F, y, stream, false, true);
 }
 
 int adec_encode_offline(adec_handle* h, const float* x, int B, int T, float* z, void* stream) {
@@ -1279,12 +1317,11 @@ int adec_encode_offline(adec_handle* h, const float* x, int B, int T, float* z, 
 }
 
 int adec_decode_offline(adec_handle* h, const float* zq, int B, int F, float* y, void* stream) {
-    if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    if (B < 1 || F < 1) return h->fail("decode_offline: empty input");
-    DeviceGuard dg(h->device);
-    if (offline_state(h, B, (cudaStream_t)stream)) return 1;
-    RunCtx rc{B, zq, y, (cudaStream_t)stream, true};
-    return run_ops(h, h->dec_ops, rc, F, nullptr);
+    return decode_common(h, zq, B, F, y, stream, true, false);
+}
+
+int adec_decode_offline_bf16(adec_handle* h, const uint16_t* zq, int B, int F, uint16_t* y, void* stream) {
+    return decode_common(h, zq, B, F, y, stream, true, true);
 }
 
 static int index_bits(int n) { int b = 1; while ((1 << b) < n) ++b; return b; }
@@ -1368,6 +1405,8 @@ int adec_codec_host(adec_handle* enc, adec_handle* dec, const float* x_host, int
                     float* y_host, void* stream) {
     if (!enc || !dec) return 1;
     if (enc->device != dec->device) return enc->fail("codec_host: handles on different devices");
+    if (dec->act_bf16) return enc->fail("codec_host: the decoder has bf16 activations (compute_dtype 2), which the host path does not carry; "
+                                        "use compute_dtype 0 or 1, or adec_decode_bf16 on device buffers");
     DeviceGuard dg(enc->device);
     cudaStream_t s = (cudaStream_t)stream;
     const int F = adec_frames_for(enc, T);

@@ -20,9 +20,12 @@
 //                       first-index arg-min by warp shuffles, int64 flat indices.
 //   lookup_kernel     - codebook gather-sum.
 #pragma once
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+
+#include <type_traits>
 
 namespace adec {
 
@@ -119,6 +122,41 @@ __device__ __forceinline__ float4 apply_act(float4 v, int act, float slope) {
     }
     return v;
 }
+
+// Activation storage in HBM (x, causal state, residual, y): fp32, or bf16 (compute_dtype 2, the vocoder's bf16-activation mode).  bf16
+// values are widened to fp32 on load; arithmetic stays fp32 and every stored value is rounded to nearest once.
+__device__ __forceinline__ float bf_lo(uint32_t w) { return __uint_as_float(w << 16); }
+__device__ __forceinline__ float bf_hi(uint32_t w) { return __uint_as_float(w & 0xFFFF0000u); }
+__device__ __forceinline__ uint32_t bf2_bits(float x, float y) { const __nv_bfloat162 h = __floats2bfloat162_rn(x, y); return *reinterpret_cast<const uint32_t*>(&h); }
+__device__ __forceinline__ float4 bf4_f4(uint2 r) { return make_float4(bf_lo(r.x), bf_hi(r.x), bf_lo(r.y), bf_hi(r.y)); }
+__device__ __forceinline__ uint2 f4_bf4(float4 v) { return make_uint2(bf2_bits(v.x, v.y), bf2_bits(v.z, v.w)); }
+// 8 consecutive channels: 32 B of fp32 or one 16-byte vector of bf16
+__device__ __forceinline__ void ldg8(const float* p, float4& u, float4& v) {
+    u = __ldg(reinterpret_cast<const float4*>(p));
+    v = __ldg(reinterpret_cast<const float4*>(p) + 1);
+}
+__device__ __forceinline__ void ldg8(const __nv_bfloat16* p, float4& u, float4& v) {
+    const uint4 r = __ldg(reinterpret_cast<const uint4*>(p));
+    u = bf4_f4(make_uint2(r.x, r.y));
+    v = bf4_f4(make_uint2(r.z, r.w));
+}
+// 4 consecutive channels
+__device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+__device__ __forceinline__ float4 ldg4(const __nv_bfloat16* p) { return bf4_f4(__ldg(reinterpret_cast<const uint2*>(p))); }
+__device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
+__device__ __forceinline__ float4 ld4(const __nv_bfloat16* p) { return bf4_f4(*reinterpret_cast<const uint2*>(p)); }
+__device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
+__device__ __forceinline__ void st4(__nv_bfloat16* p, float4 v) { *reinterpret_cast<uint2*>(p) = f4_bf4(v); }
+// 2 consecutive channels, 1 value
+__device__ __forceinline__ float2 ldg2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
+__device__ __forceinline__ float2 ldg2(const __nv_bfloat16* p) { const uint32_t w = __ldg(reinterpret_cast<const unsigned int*>(p)); return make_float2(bf_lo(w), bf_hi(w)); }
+__device__ __forceinline__ void st2(float* p, float x, float y) { *reinterpret_cast<float2*>(p) = make_float2(x, y); }
+__device__ __forceinline__ void st2(__nv_bfloat16* p, float x, float y) { *reinterpret_cast<uint32_t*>(p) = bf2_bits(x, y); }
+__device__ __forceinline__ void st1(float* p, float x) { *p = x; }
+__device__ __forceinline__ void st1(__nv_bfloat16* p, float x) { *p = __float2bfloat16_rn(x); }
+// the value a store of type T keeps (bf16 storage: what the causal state holds, so that a window row read from the chunk matches it)
+template <bool BST> __device__ __forceinline__ float4 stored4(float4 v) { return BST ? bf4_f4(f4_bf4(v)) : v; }
+
 
 // ------------------------------------------------------------------------------------------------
 // conv_gemm_kernel
@@ -475,15 +513,17 @@ struct HeadArgs {
 // is read 14/8 times from L1), applies the pre-activation in registers and accumulates its 4-channel share of the R dot products with
 // the K x 4 weights it keeps in registers; three xor-shuffles add the eight shares and lane j stores output j.  The layer moves
 // 128 B per output row and does 2*K*CIN flops on it: memory-bound once the LDS traffic of the round-1 version (112 LDS.128 per output)
-// is gone.
-template <int CIN, int K>
+// is gone.  BST: bf16 input, state and output (the vocoder's bf16-activation mode); a chunk row enters the window as the bf16 value the
+// state keeps of it, so that a streamed chunk and a one-shot call see the same window.
+template <int CIN, int K, bool BST>
 __global__ void __launch_bounds__(256) head_kernel(const HeadArgs a) {
     static_assert(CIN == 32, "eight lanes x four channels");
+    using XT = typename std::conditional<BST, __nv_bfloat16, float>::type;
     constexpr int R = 8, P = K - 1, TT = 256;
     const int b = blockIdx.y, tid = threadIdx.x, c4 = tid & 7;
     const int t0 = blockIdx.x * TT + (tid >> 3) * R;               // first output of this lane group
-    const float* xg = a.x + (long long)b * a.x_bs;
-    const float* sg = a.st_in + (long long)b * P * CIN;
+    const XT* xg = reinterpret_cast<const XT*>(a.x) + (long long)b * a.x_bs;
+    const XT* sg = reinterpret_cast<const XT*>(a.st_in) + (long long)b * P * CIN;
     float4 w[K];
 #pragma unroll
     for (int k = 0; k < K; ++k) w[k] = __ldg(reinterpret_cast<const float4*>(a.w + k * CIN) + c4);
@@ -496,8 +536,8 @@ __global__ void __launch_bounds__(256) head_kernel(const HeadArgs a) {
         for (int r = 0; r < R + P; ++r) {
             const long long i = (long long)t0 + r;                  // x~ row = history(P) || chunk
             xv[r] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (i < P) xv[r] = __ldg(reinterpret_cast<const float4*>(sg + i * CIN) + c4);            // state rows are stored post-activation
-            else if (i - P < a.T) xv[r] = apply_act(__ldg(reinterpret_cast<const float4*>(xg + (i - P) * a.ldx) + c4), a.pre_act, a.slope);
+            if (i < P) xv[r] = ldg4(sg + i * CIN + 4 * c4);          // state rows are stored post-activation
+            else if (i - P < a.T) xv[r] = stored4<BST>(apply_act(ldg4(xg + (i - P) * a.ldx + 4 * c4), a.pre_act, a.slope));
         }
 #pragma unroll
         for (int j = 0; j < R; ++j)
@@ -519,17 +559,17 @@ __global__ void __launch_bounds__(256) head_kernel(const HeadArgs a) {
     if (t0 + c4 < a.T) {
         mine += a.bias;
         if (a.post_tanh) mine = tanhf(mine);
-        a.y[(long long)b * a.y_bs + t0 + c4] = mine;
+        st1(reinterpret_cast<XT*>(a.y) + (long long)b * a.y_bs + t0 + c4, mine);
     }
     if (blockIdx.x == gridDim.x - 1) {
-        float* so = a.st_out + (long long)b * P * CIN;
+        XT* so = reinterpret_cast<XT*>(a.st_out) + (long long)b * P * CIN;
         for (int idx = tid; idx < P * (CIN / 4); idx += 256) {
             const int r = idx / (CIN / 4), ci = (idx - r * (CIN / 4)) * 4;
             const long long i = (long long)a.T + r;
             float4 v;
-            if (i < P) v = *reinterpret_cast<const float4*>(sg + i * CIN + ci);
-            else v = apply_act(__ldg(reinterpret_cast<const float4*>(xg + (i - P) * a.ldx + ci)), a.pre_act, a.slope);
-            *reinterpret_cast<float4*>(so + r * CIN + ci) = v;
+            if (i < P) v = ld4(sg + i * CIN + ci);
+            else v = apply_act(ldg4(xg + (i - P) * a.ldx + ci), a.pre_act, a.slope);
+            st4(so + r * CIN + ci, v);
         }
     }
 }

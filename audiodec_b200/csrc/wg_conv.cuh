@@ -241,9 +241,12 @@ __device__ __forceinline__ void wg_group(float (&d)[WgCfg<NT, PREC>::PW / 2], ui
     wg_fence_regs(d);
 }
 
-template <int NT, bool FUSE, int PRE, int PREC>
+// BST: activations, causal state, residual and output stored as bf16 in HBM (bf16 operands only; no 4-channel strided convs)
+template <int NT, bool FUSE, int PRE, int PREC, bool BST>
 __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(const ConvArgs a, int n_xtiles, int n_ytiles, int n_tiles) {
+    static_assert(!BST || (PREC == PREC_BF16 && !FUSE), "bf16 storage is built for the non-fused bf16-operand kernels");
     using Cfg = WgCfg<NT, PREC>;
+    using XT = typename std::conditional<BST, __nv_bfloat16, float>::type;
     constexpr int S = Cfg::stages(FUSE), CP = TC_CP, TT = TC_TT, KBB = Cfg::KBB, EB = Cfg::EB, TPG = Cfg::TPG, PW = Cfg::PW;
     constexpr int NPROD = Cfg::NPROD, WWARP = (256 + NPROD) / 32;         // weight producer warp
     constexpr int STAGE_BYTES = Cfg::STAGE_BYTES, TAP_BYTES = Cfg::TAP_BYTES;
@@ -301,7 +304,8 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
             }
         }
     } else if (warp >= 8) {
-        // ------------------------------------------------ activation producers: one item = 8 channels (32 B of global) of one window row.
+        // ------------------------------------------------ activation producers: one item = 8 channels (32 B of fp32 / 16 B of bf16) of one
+        // window row.
         // The loads of a piece are issued BEFORE the wait for a free window buffer, so global latency overlaps the MMAs that still read
         // the buffer; a.n_wbuf (2..4) buffers let the producers run several pieces ahead.
         const int pt = tid - 256;
@@ -317,8 +321,8 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
             int g = 0, co_tile = y;
             if (a.n_co_tiles != n_ytiles) { g = y / a.n_co_tiles; co_tile = y - g * a.n_co_tiles; }
             const int j0 = xt * TT;
-            const float* xg = a.x + (long long)b * a.x_bs + g * a.x_goff;
-            const float* sg = a.st_in + (long long)b * a.P * a.st_ld + g * a.st_goff;
+            const XT* xg = reinterpret_cast<const XT*>(a.x) + (long long)b * a.x_bs + g * a.x_goff;
+            const XT* sg = reinterpret_cast<const XT*>(a.st_in) + (long long)b * a.P * a.st_ld + g * a.st_goff;
             for (int p = 0; p < a.n_pieces; ++p) {
                 const int buf = wb;
                 const uint32_t wpar = (uint32_t)(wround - 1) & 1u;
@@ -333,16 +337,13 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                 const long long i_last = (long long)(j0 + wrows - 1) * a.RG + r;
                 if (i_first >= a.P && i_last - a.P < a.T && PRE != ACT_NORM && !halves && !a.stack_L) {
                     // interior piece: every row comes from the chunk
-                    const float* xp = xg + ci + (i_first - a.P + (long long)m0 * a.RG) * a.ldx;
+                    const XT* xp = xg + ci + (i_first - a.P + (long long)m0 * a.RG) * a.ldx;
                     const long long xstep = (long long)RPP * a.RG * a.ldx;
                     for (int mb = m0; mb < wrows; mb += RPP * UNR, xp += xstep * UNR) {
                         float4 u[UNR], v[UNR];
 #pragma unroll
                         for (int k = 0; k < UNR; ++k)
-                            if (mb + k * RPP < wrows) {
-                                u[k] = __ldg(reinterpret_cast<const float4*>(xp + k * xstep));
-                                v[k] = __ldg(reinterpret_cast<const float4*>(xp + k * xstep) + 1);
-                            }
+                            if (mb + k * RPP < wrows) ldg8(xp + k * xstep, u[k], v[k]);
                         if (!waited) { mbar_wait(&w_empty[buf], wpar, 500); waited = true; }
 #pragma unroll
                         for (int k = 0; k < UNR; ++k) {
@@ -363,8 +364,8 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                             if (m < wrows) {
                                 // stacked rows: window row j0 + m of the stack is local row `ml` of stream `sm`
                                 int ml = j0 + m;
-                                const float* xs = xg;
-                                const float* ss = sg;
+                                const XT* xs = xg;
+                                const XT* ss = sg;
                                 bool live = true;
                                 if (a.stack_L) {
                                     const int sm = ml / a.stack_L;
@@ -373,19 +374,30 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                                     xs = xg + (long long)sm * a.x_bs;
                                     ss = sg + (long long)sm * a.P * a.st_ld;
                                 }
-#pragma unroll
-                                for (int hf = 0; hf < 2; ++hf) {
-                                    int rr = r, cc = ci + 4 * hf;
-                                    if (halves) { rr = (q + 4 * hf) >> a.lgCin; cc = (q + 4 * hf) & (a.Cin - 1); if (hf) ci2 = cc; }
-                                    const long long i = (long long)ml * a.RG + rr;
+                                if constexpr (BST) {
+                                    // both halves are one 16-byte vector of the same x~ row (bf16 storage has no 4-channel strided convs)
+                                    const long long i = (long long)ml * a.RG + r;
                                     long long ti = i - a.P;
-                                    if (a.hist_rep && ti < 0) ti = 0;              // non-streaming transposed conv: replicate the first input row
-                                    float4 w4 = make_float4(0.f, 0.f, 0.f, 0.f);
+                                    if (a.hist_rep && ti < 0) ti = 0;
                                     if (live) {
-                                        if (ti < 0) w4 = __ldg(reinterpret_cast<const float4*>(ss + i * a.st_ld + cc));
-                                        else if (ti < a.T) { w4 = __ldg(reinterpret_cast<const float4*>(xs + ti * a.ldx + cc)); act |= 1u << (2 * k + hf); }
+                                        if (ti < 0) ldg8(ss + i * a.st_ld + ci, u[k], v[k]);
+                                        else if (ti < a.T) { ldg8(xs + ti * a.ldx + ci, u[k], v[k]); act |= 3u << (2 * k); }
                                     }
-                                    if (hf) v[k] = w4; else u[k] = w4;
+                                } else {
+#pragma unroll
+                                    for (int hf = 0; hf < 2; ++hf) {
+                                        int rr = r, cc = ci + 4 * hf;
+                                        if (halves) { rr = (q + 4 * hf) >> a.lgCin; cc = (q + 4 * hf) & (a.Cin - 1); if (hf) ci2 = cc; }
+                                        const long long i = (long long)ml * a.RG + rr;
+                                        long long ti = i - a.P;
+                                        if (a.hist_rep && ti < 0) ti = 0;              // non-streaming transposed conv: replicate the first input row
+                                        float4 w4 = make_float4(0.f, 0.f, 0.f, 0.f);
+                                        if (live) {
+                                            if (ti < 0) w4 = __ldg(reinterpret_cast<const float4*>(ss + i * a.st_ld + cc));
+                                            else if (ti < a.T) { w4 = __ldg(reinterpret_cast<const float4*>(xs + ti * a.ldx + cc)); act |= 1u << (2 * k + hf); }
+                                        }
+                                        if (hf) v[k] = w4; else u[k] = w4;
+                                    }
                                 }
                             }
                         }
@@ -419,9 +431,9 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                     s_hi = b;
                 }
                 for (int sm = s_lo; sm <= s_hi; ++sm) {
-                    const float* xs = a.x + (long long)sm * a.x_bs + g * a.x_goff;
-                    const float* ss = a.st_in + (long long)sm * a.P * a.st_ld + g * a.st_goff;
-                    float* so = a.st_out + (long long)sm * a.P * a.st_ld + g * a.st_goff;
+                    const XT* xs = reinterpret_cast<const XT*>(a.x) + (long long)sm * a.x_bs + g * a.x_goff;
+                    const XT* ss = reinterpret_cast<const XT*>(a.st_in) + (long long)sm * a.P * a.st_ld + g * a.st_goff;
+                    XT* so = reinterpret_cast<XT*>(a.st_out) + (long long)sm * a.P * a.st_ld + g * a.st_goff;
                     const int nvec = a.P * (a.Cin / 4);
                     for (int idx = pt; idx < nvec; idx += NPROD) {
                         const int r = idx / (a.Cin / 4);
@@ -429,13 +441,13 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                         const long long i = (long long)a.T + r;
                         float4 w4;
                         if (i < a.P) {
-                            w4 = *reinterpret_cast<const float4*>(ss + i * a.st_ld + cc);
+                            w4 = ld4(ss + i * a.st_ld + cc);
                         } else {
-                            w4 = __ldg(reinterpret_cast<const float4*>(xs + (i - a.P) * a.ldx + cc));
+                            w4 = ldg4(xs + (i - a.P) * a.ldx + cc);
                             if (PRE == ACT_NORM) w4 = norm4(w4, a.mean + cc, a.scale + cc);
                             else w4 = apply_act_t<PRE>(w4, a.slope);
                         }
-                        *reinterpret_cast<float4*>(so + (long long)r * a.st_ld + cc) = w4;
+                        st4(so + (long long)r * a.st_ld + cc, w4);
                     }
                 }
             }
@@ -538,16 +550,16 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                         v0 += b2.x; v1 += b2.y;
                     }
                     if (a.res) {
-                        const float2 r2 = __ldg(reinterpret_cast<const float2*>(a.res + (long long)bo * a.res_bs + (long long)t * a.ldr + g * a.r_goff + co_l));
+                        const float2 r2 = ldg2(reinterpret_cast<const XT*>(a.res) + (long long)bo * a.res_bs + (long long)t * a.ldr + g * a.r_goff + co_l);
                         v0 = r2.x + v0; v1 = r2.y + v1;
                     }
                     vmax = fmaxf(vmax, fmaxf(fabsf(v0), fabsf(v1)));
                     if (a.out_nct) {
-                        float* yp = a.y + (long long)bo * a.y_bs + (long long)(g * a.y_goff + co_l) * a.Tout + t;
-                        yp[0] = v0;
-                        yp[a.Tout] = v1;
+                        XT* yp = reinterpret_cast<XT*>(a.y) + (long long)bo * a.y_bs + (long long)(g * a.y_goff + co_l) * a.Tout + t;
+                        st1(yp, v0);
+                        st1(yp + a.Tout, v1);
                     } else {
-                        *reinterpret_cast<float2*>(a.y + (long long)bo * a.y_bs + (long long)t * a.ldy + g * a.y_goff + co_l) = make_float2(v0, v1);
+                        st2(reinterpret_cast<XT*>(a.y) + (long long)bo * a.y_bs + (long long)t * a.ldy + g * a.y_goff + co_l, v0, v1);
                     }
                 }
             }

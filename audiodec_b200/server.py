@@ -152,6 +152,8 @@ class MultiStreamCodecServer:
             else:
                 y_host = y
         now = self._clock()
+        if y_host.dtype == torch.bfloat16:
+            y_host = y_host.float()             # a bf16-activation decoder: half the D2H bytes, widened here; frames out stay float32
         y_all = y_host.numpy().reshape(self.n_streams, -1)[:, :self.frame_size].copy()    # one copy; the queues hold row views of it
         with self._lock:
             for s in range(self.n_streams):

@@ -14,7 +14,8 @@
  *     (adec_last_error() gives the message).  Nothing throws, nothing falls back to CPU.
  *   - all data pointers of the *_dev entry points are DEVICE pointers on the handle's GPU;
  *     `stream` is a cudaStream_t passed as void* (NULL = legacy default stream).
- *   - activations are fp32.  Layouts at the boundary are the reference's own
+ *   - activations are fp32, except on HiFi-GAN handles with compute_dtype 2 (the *_bf16 decode entry points).  Layouts at
+ *     the boundary are the reference's own
  *     (SURVEY.md A.3):  x (B,1,T)   z (B,64,F) channels-first   idx (Nq,B,F) int64 flat
  *     (+1024*i already added)   zq (B,F,64) channels-last   y (B,1,F*hop).
  *   - a handle owns its weights and its per-stream causal state (the reference's
@@ -63,7 +64,10 @@ typedef struct adec_config {
     int n_resblocks;  int resblock_kernel_sizes[ADEC_MAX_STAGES];   /* AD v0: MultiReceptiveField, one residual block per kernel size */
     /* appended in round 2 */
     int compute_dtype;                                     /* 0 = fp32-grade (default); 1 = bf16 conv operands with fp32 accumulation, HiFi-GAN vocoder
-                                                              only: what `decoder.to(torch.bfloat16)` asks of the reference (BASELINE configs[2]) */
+                                                              only: what `decoder.to(torch.bfloat16)` asks of the reference (BASELINE configs[2]);
+                                                              2 = as 1, and every activation, the causal state and the decode input / output are
+                                                              bf16 in memory (the reference's bf16 data layout and dtype contract): decode with
+                                                              adec_decode_bf16 / adec_decode_offline_bf16.  1 and 2 need the f16 engine. */
 } adec_config;
 
 /* -- lifetime ---------------------------------------------------------------- */
@@ -106,6 +110,10 @@ int adec_lookup(adec_handle *h, const int64_t *idx, int B, int F, float *zq, voi
 /* StreamGenerator.decode (AudioDec.py:246-247 / HiFiGAN.py:268-273): zq (B,F,code_dim) -> y (B,1,F*hop). */
 int adec_decode(adec_handle *h, const float *zq, int B, int F, float *y, void *stream);
 
+/* Same, for a HiFi-GAN handle with compute_dtype 2: zq (B,F,in_channels) and y (B,1,F*hop) are bf16 (raw 16-bit words), both
+ * 16-byte aligned.  adec_decode on such a handle fails, and so does adec_decode_bf16 on any other handle. */
+int adec_decode_bf16(adec_handle *h, const uint16_t *zq, int B, int F, uint16_t *y, void *stream);
+
 /* -- the non-streaming batch forward (SURVEY.md 8(f) rank 4; codecTest.py:78-95, codecStatistic.py:92-98) ---------- */
 /* Encoder.forward + Projector.forward (models/autoencoder/modules/encoder.py:131, projector.py:49-50): every causal
  * conv zero-pads on the left (layers/conv_layer.py:148-151) = no history; any batch size.  x (B,1,T) -> z (B,code_dim,F).
@@ -114,6 +122,8 @@ int adec_encode_offline(adec_handle *h, const float *x, int B, int T, float *z, 
 /* Decoder.forward (decoder.py:135-140) / HiFi-GAN Generator.forward (HiFiGAN.py:140-160): as above, and every transposed conv
  * pads with its FIRST input frame (ReplicationPad1d, conv_layer.py:189-192).  zq (B,F,code_dim) channels-last -> y (B,1,F*hop). */
 int adec_decode_offline(adec_handle *h, const float *zq, int B, int F, float *y, void *stream);
+/* adec_decode_offline for a compute_dtype 2 handle: bf16 zq (B,F,in_channels) channels-last -> bf16 y (B,1,F*hop), 16-byte aligned. */
+int adec_decode_offline_bf16(adec_handle *h, const uint16_t *zq, int B, int F, uint16_t *y, void *stream);
 
 /* output frames of encode for T input samples: floor((T-1)/s)+1 applied per stride (conv_layer.py:153-156) */
 int adec_frames_for(const adec_handle *h, int T);
@@ -123,7 +133,7 @@ int adec_hop_length(const adec_handle *h);
 /* -- whole path with HOST buffers (what demoFile.py:55-62 does around the four calls) ------- */
 /* x_host (B,1,T) -> idx_host (Nq,B,F) (may be NULL) and y_host (B,1,F*hop).  Copies H2D, runs
  * enc.encode -> enc.quantize -> enc.lookup -> dec.decode on `stream`, copies D2H and synchronises.
- * `enc` must be a symAD handle; `dec` a symAD or HiFi-GAN handle (may equal enc). */
+ * `enc` must be a symAD handle; `dec` a symAD or HiFi-GAN handle (may equal enc) with fp32 activations (compute_dtype 0 or 1). */
 int adec_codec_host(adec_handle *enc, adec_handle *dec, const float *x_host, int B, int T,
                     int64_t *idx_host, float *y_host, void *stream);
 
