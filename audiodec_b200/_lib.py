@@ -62,6 +62,9 @@ SYMBOLS = {
     "adec_decode_offline": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "adec_decode_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "adec_decode_offline_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "adec_encode_offline_varlen": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),
+    "adec_decode_offline_varlen": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),
+    "adec_decode_offline_varlen_bf16": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),
     "adec_frames_for": (c_int, [c_void_p, c_int]),
     "adec_hop_length": (c_int, [c_void_p]),
     "adec_codec_host": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),

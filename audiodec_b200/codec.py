@@ -42,6 +42,25 @@ def _fill(arr, values):
         arr[i] = int(v)
 
 
+def varlen_layout(lengths, strides):
+    """Frame counts and column offsets of a varlen batch: F_b = frames_for(T_b) (floor((t - 1) / s) + 1 per stride, conv_layer.py:153-156)
+    and offsets[b] = sum_{i<b} F_i, B + 1 entries.  Utterance b's frames are columns [offsets[b], offsets[b + 1]) of the varlen z / zq;
+    times the hop, the same offsets place its samples in the decoded waveform."""
+    frames, offsets = [], [0]
+    for t in lengths:
+        t = int(t)
+        for s in strides:
+            t = (t - 1) // s + 1
+        frames.append(t)
+        offsets.append(offsets[-1] + t)
+    return frames, offsets
+
+
+def _int_array(values):
+    values = [int(v) for v in values]
+    return (ctypes.c_int * max(1, len(values)))(*values), len(values)
+
+
 class _StreamGeneratorBase:
     """Common plumbing: deferred handle creation (weights arrive before the device is known, exactly
     like ``Generator(**params)`` -> ``load_state_dict`` -> ``.to(device)`` in the reference)."""
@@ -215,6 +234,7 @@ class SymADStreamGenerator(_StreamGeneratorBase):
         c.codec_activate = int(codec == "activate_audiodec")
         self.input_channels = input_channels
         self.code_dim, self.codebook_num = code_dim, codebook_num
+        self.enc_strides = tuple(enc_strides)
 
     # -- streaming API ---------------------------------------------------------------------------------
     def initial_encoder(self, receptive_length, device):
@@ -309,6 +329,27 @@ class SymADStreamGenerator(_StreamGeneratorBase):
         _check(self._lib.adec_encode_offline(self._h, _ptr(x), b, t, _ptr(z), self._stream()), self._h)
         return z
 
+    def encode_offline_varlen(self, xs):
+        """Utterances of different lengths in one launch sequence: xs is a list of 1-D (T_b,) or (1, T_b) tensors.  Returns
+        (z (1, code_dim, sum F_b), [F_b]); utterance b's frames are columns [sum_{i<b} F_i, +F_b) and equal encode_offline of that
+        utterance alone.  z is quantize_offline's B = 1 layout, so one quantize_offline call quantizes the whole batch."""
+        self._ready()
+        flat = []
+        for x in xs:
+            x = x[0] if x.dim() == 2 and x.size(0) == 1 else x
+            if x.dim() != 1:
+                raise RuntimeError(f"audiodec_b200: encode_offline_varlen: expected 1-D (T,) or (1, T) utterances, got {tuple(x.shape)}")
+            flat.append(self._in(x))
+        if not flat:
+            raise RuntimeError("audiodec_b200: encode_offline_varlen: no utterances")
+        lengths = [x.numel() for x in flat]
+        frames, offsets = varlen_layout(lengths, self.enc_strides)
+        x = torch.cat(flat)
+        z = torch.empty(1, self.code_dim, offsets[-1], device=self._device, dtype=torch.float32)
+        arr, b = _int_array(lengths)
+        _check(self._lib.adec_encode_offline_varlen(self._h, _ptr(x), arr, b, _ptr(z), self._stream()), self._h)
+        return z, frames
+
     def quantize_offline(self, z):
         """z (B,code_dim,F) -> (zq (B,code_dim,F) channels-first like Quantizer.forward (quantizer.py:31-34), idx (Nq,B,F))."""
         self._ready()
@@ -325,6 +366,12 @@ class SymADStreamGenerator(_StreamGeneratorBase):
         """zq (B,code_dim,F) channels-first (what Decoder.forward takes, decoder.py:135-140) -> y (B,1,F*hop); transposed convs
         replicate their first input frame (conv_layer.py:189-192)."""
         return _decode_offline(self, zq)
+
+    def decode_offline_varlen(self, zq, frames):
+        """zq (1, code_dim, sum F_b) channels-first holding utterances of `frames` frames each (what encode_offline_varlen +
+        quantize_offline give) -> list of B waveforms (1, 1, F_b * hop), views of one output buffer, each equal to decode_offline of
+        that utterance alone."""
+        return _decode_offline_varlen(self, zq, frames)
 
     # ---- index bitstream (SURVEY.md 8(f) rank 2; the reference queues the raw int64 tensor, bin/stream.py:224)
     def packed_frame_bytes(self):
@@ -390,6 +437,29 @@ def _decode_offline(gen, zq):
     fn = gen._lib.adec_decode_offline_bf16 if gen._act_bf16 else gen._lib.adec_decode_offline
     _check(fn(gen._h, _ptr(zq_cl), b, f, _ptr(y), gen._stream()), gen._h)
     return y
+
+
+def _decode_offline_varlen(gen, zq, frames):
+    gen._ready()
+    gen._want(zq, "decode_offline_varlen / forward_varlen", 1, getattr(gen, "code_dim", None) or gen.in_channels)
+    frames = [int(f) for f in frames]
+    if zq.size(0) != 1 or zq.size(2) != sum(frames):
+        raise RuntimeError(f"audiodec_b200: decode_offline_varlen / forward_varlen: expected (1, D, {sum(frames)}) for frames summing to "
+                           f"{sum(frames)}, got {tuple(zq.shape)}")
+    dtype = torch.bfloat16 if gen._act_bf16 else torch.float32
+    zq_cl = gen._in(zq, dtype)[0].transpose(0, 1).contiguous()     # the kernels' native channels-last (sum F, D)
+    if gen._act_bf16 and zq_cl.data_ptr() % 16:
+        zq_cl = zq_cl.clone()                                       # the bf16 kernels read zq as 16-byte vectors
+    hop = gen._lib.adec_hop_length(gen._h)
+    y = torch.empty(sum(frames) * hop, device=gen._device, dtype=dtype)
+    arr, b = _int_array(frames)
+    fn = gen._lib.adec_decode_offline_varlen_bf16 if gen._act_bf16 else gen._lib.adec_decode_offline_varlen
+    _check(fn(gen._h, _ptr(zq_cl), arr, b, _ptr(y), gen._stream()), gen._h)
+    out, o = [], 0
+    for f in frames:
+        out.append(y[o * hop:(o + f) * hop].view(1, 1, f * hop))
+        o += f
+    return out
 
 
 class HiFiGANStreamGenerator(_StreamGeneratorBase):
@@ -466,6 +536,12 @@ class HiFiGANStreamGenerator(_StreamGeneratorBase):
 
     __call__ = forward
 
+    def forward_varlen(self, c, frames):
+        """Generator.forward over utterances of different lengths in one launch sequence: c (1, in_channels, sum F_b) channels-first,
+        utterance b at columns [sum_{i<b} F_i, +F_b) -> list of B waveforms (1, 1, F_b * hop), views of one output buffer (bf16 with
+        bf16 activations), each equal to forward of that utterance alone."""
+        return _decode_offline_varlen(self, c, frames)
+
 
 class OfflineCodec:
     """Mirror of codecTest.py's TestMain.encode / decode (codecTest.py:78-95): the non-streaming batch path.
@@ -487,6 +563,39 @@ class OfflineCodec:
 
     def decode(self, zq):
         return self.decoder.forward(zq) if isinstance(self.decoder, HiFiGANStreamGenerator) else self.decoder.decode_offline(zq)
+
+    def encode_many(self, audios):
+        """encode() of every (T_i, C_i) array in `audios` through ONE varlen encode and quantize: each audio channel is an utterance.
+        Returns [zq_i (C_i, code_dim, F_i)], equal to [encode(a) for a in audios]."""
+        if self.multi_channel:
+            raise NotImplementedError("encode_many runs one utterance per audio channel (multi_channel=False)")
+        dev = self.encoder._device
+        arrs = [torch.as_tensor(a, dtype=torch.float32) for a in audios]
+        chans = [x.shape[1] for x in arrs]
+        rows = torch.cat([x.transpose(1, 0).reshape(-1) for x in arrs]).to(dev)      # channel-major: one utterance per (file, channel)
+        lengths = [x.shape[0] for x, c in zip(arrs, chans) for _ in range(c)]
+        z, frames = self.encoder.encode_offline_varlen(list(torch.split(rows, lengths)))
+        zq, _ = self.encoder.quantize_offline(z)                                       # (1, code_dim, sum F)
+        cols = list(torch.split(zq[0], frames, dim=1))
+        out, k = [], 0
+        for c in chans:
+            out.append(torch.stack(cols[k:k + c]))
+            k += c
+        return out
+
+    def decode_many(self, zqs):
+        """decode() of every zq_i (C_i, code_dim, F_i) through ONE varlen decode.  Returns [y_i (C_i, 1, F_i * hop)], equal to
+        [decode(zq) for zq in zqs]."""
+        chans = [zq.size(0) for zq in zqs]
+        frames = [zq.size(2) for zq in zqs for _ in range(zq.size(0))]
+        c = torch.cat([zq[i] for zq in zqs for i in range(zq.size(0))], dim=1).unsqueeze(0)
+        fn = self.decoder.forward_varlen if isinstance(self.decoder, HiFiGANStreamGenerator) else self.decoder.decode_offline_varlen
+        ys = fn(c, frames)
+        out, k = [], 0
+        for n in chans:
+            out.append(torch.cat(ys[k:k + n]))
+            k += n
+        return out
 
 
 def codec_host(encoder: SymADStreamGenerator, decoder, x_host: torch.Tensor, want_idx=True, reuse_buffers=False):

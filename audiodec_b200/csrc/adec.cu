@@ -96,12 +96,12 @@ const ConvKernelCfg* find_conv_kernel(int CW, int CO, bool fuse) {
 // (ADEC_CONV_PATH=tf32); PREC_BF16 = bf16 operands, one product (the vocoder's bf16 modes; BST = bf16 activations in HBM as well).
 // Persistent: one CTA per SM loops over (time tile, channel tile, stream) tiles.
 typedef cudaError_t (*TcPersistFn)(const ConvArgs&, int, int, int, int, int, cudaStream_t);
-template <int NT, bool F, int PRE, int PREC, bool BST>
+template <int NT, bool F, int PRE, int PREC, bool BST, bool VL>
 cudaError_t launch_wg(const ConvArgs& a, int n_xtiles, int n_ytiles, int n_tiles, int n_ctas, int smem_bytes, cudaStream_t s) {
     static bool configured[64] = {false};
     int dev = 0;
     cudaGetDevice(&dev);
-    auto kern = wg_conv_kernel<NT, F, PRE, PREC, BST>;
+    auto kern = wg_conv_kernel<NT, F, PRE, PREC, BST, VL>;
     constexpr int kMaxDyn = 227 * 1024;
     if (dev < 64 && !configured[dev]) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn);
@@ -127,9 +127,11 @@ cudaError_t launch_wg(const ConvArgs& a, int n_xtiles, int n_ytiles, int n_tiles
 }
 typedef size_t (*TcSmemFn)(int, bool);
 typedef int (*TcWbufFn)(int, bool);
-struct TcKernelCfg { int NT; bool fuse; int pre, prec; bool bst; int tap_bytes; TcPersistFn pfn; TcSmemFn smem; TcWbufFn n_wbuf; };
+// pfn_vl: the varlen instantiation (adec_*_offline_varlen)
+struct TcKernelCfg { int NT; bool fuse; int pre, prec; bool bst; int tap_bytes; TcPersistFn pfn, pfn_vl; TcSmemFn smem; TcWbufFn n_wbuf; };
 #define ADEC_TC1(NT, F, PRE, PREC, BST) \
-    {NT, F, PRE, PREC, BST, WgCfg<NT, PREC>::TAP_BYTES, launch_wg<NT, F, PRE, PREC, BST>, WgCfg<NT, PREC>::smem_bytes, WgCfg<NT, PREC>::n_wbuf}
+    {NT, F, PRE, PREC, BST, WgCfg<NT, PREC>::TAP_BYTES, launch_wg<NT, F, PRE, PREC, BST, false>, launch_wg<NT, F, PRE, PREC, BST, true>, \
+     WgCfg<NT, PREC>::smem_bytes, WgCfg<NT, PREC>::n_wbuf}
 #define ADEC_TC_FP32(NT, PREC) \
     ADEC_TC1(NT, true, ACT_ELU, PREC, false), ADEC_TC1(NT, false, ACT_NONE, PREC, false), ADEC_TC1(NT, false, ACT_ELU, PREC, false), \
     ADEC_TC1(NT, false, ACT_LRELU, PREC, false), ADEC_TC1(NT, false, ACT_NORM, PREC, false)
@@ -238,6 +240,7 @@ struct adec_handle {
     std::vector<double> prof_bytes;   // algorithmic bytes of each recorded launch (SURVEY 8(d) per-layer model)
     // host-path scratch
     DevBuf hx, hz, hzq, hy;
+    DevBuf vl_tab;                // varlen row tables of the last call (ints)
     long long* hidx = nullptr;
     size_t hidx_cap = 0;
 
@@ -631,26 +634,88 @@ struct RunCtx {
     float* ext_out;
     cudaStream_t stream;
     bool offline = false;   // non-streaming forward: transposed convs replicate their first input row instead of reading state
+    const int* vl_len = nullptr;   // varlen: HOST lengths of the B utterances, concatenated along time in ext_in / ext_out (offline only)
+    const char* what = "";         // entry point, for messages
 };
 
+// varlen row spaces must stay inside the kernels' 32-bit row indices, with room for a tile and its halo past the end
+constexpr long long kVlMaxRows = (1ll << 31) - 4096;
+
+// Per-op row tables of a varlen call: utterance b's input rows [in[b], in[b + 1]) and output rows [out[b], out[b + 1]) of every op,
+// the arithmetic of the uniform path (Tout = (T - 1) / down + 1, then T = Tout * up) applied per utterance.  Fails on a row space
+// that does not fit the kernels' 32-bit row indices.
+struct VlPlan {
+    std::vector<int> tab;                 // per op: in (B + 1) | out (B + 1)
+    std::vector<long long> T, Tout;       // per op: total input / output rows
+};
+int plan_varlen(adec_handle* h, const std::vector<Op>& ops, const RunCtx& rc, VlPlan* pl) {
+    const int B = rc.B;
+    std::vector<long long> len(rc.vl_len, rc.vl_len + B);
+    pl->tab.assign(ops.size() * 2 * (B + 1), 0);
+    for (size_t k = 0; k < ops.size(); ++k) {
+        const Op& op = ops[k];
+        const long long halo = op.kind == OP_CONV ? (long long)(op.Ktaps - 1) * op.dil : 0;
+        int* in = pl->tab.data() + k * 2 * (B + 1);
+        int* out = in + B + 1;
+        long long si = 0, so = 0;
+        for (int b = 0; b < B; ++b) {
+            const long long tout = (len[b] - 1) / op.down + 1;
+            si += len[b];
+            so += tout;
+            if (si > kVlMaxRows || so * op.up > kVlMaxRows || so + (b + 1) * halo > kVlMaxRows)
+                return h->fail(fmt("%s: the batch needs more than %lld rows at %s, beyond the kernels' 32-bit row indexing; split it",
+                                   rc.what, kVlMaxRows, op.name.c_str()));
+            in[b + 1] = (int)si;
+            out[b + 1] = (int)so;
+            len[b] = tout * op.up;
+        }
+        pl->T.push_back(si);
+        pl->Tout.push_back(so);
+    }
+    return 0;
+}
+
 int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, int* T_out_final) {
-    // pass 1: workspace sizes
+    // pass 1: workspace sizes (varlen: the row tables, uploaded in one copy on the call's stream)
+    const bool vl = rc.vl_len != nullptr;
+    VlPlan pl;
+    if (vl) {
+        if (plan_varlen(h, ops, rc, &pl)) return 1;
+        for (const Op& op : ops)
+            if (op.kind == OP_CONV && !op.tc)
+                return h->fail(fmt("%s: the FFMA engine (ADEC_CONV_PATH=ffma) has no varlen kernels; use the f16 or tf32 tensor-core engine",
+                                   rc.what));
+    }
     size_t need[3] = {0, 0, 0};
     {
         int T = T_in;
-        for (const Op& op : ops) {
+        for (size_t k = 0; k < ops.size(); ++k) {
+            const Op& op = ops[k];
             const int Tout = (T - 1) / op.down + 1;
-            if (op.out_buf >= 0) need[op.out_buf] = std::max(need[op.out_buf], (size_t)rc.B * Tout * op.ldy);
+            const size_t rows = vl ? (size_t)pl.Tout[k] : (size_t)rc.B * Tout;
+            if (op.out_buf >= 0) need[op.out_buf] = std::max(need[op.out_buf], rows * op.ldy);
             T = Tout * op.up;
         }
     }
     for (int i = 0; i < 3; ++i)     // need[] counts elements; the buffers are sized in floats
         if (need[i] && ensure(h, h->ws[i], (need[i] * h->act_bytes() + 3) / 4)) return 1;
-    if (rc.B != h->n_streams) return h->fail(fmt("batch %d != n_streams %d (call adec_set_streams)", rc.B, h->n_streams));
+    if (!vl && rc.B != h->n_streams) return h->fail(fmt("batch %d != n_streams %d (call adec_set_streams)", rc.B, h->n_streams));
+    const int* vl_tab = nullptr;
+    if (vl) {
+        if (adec_reset(h, (void*)rc.stream)) return 1;      // discards the streaming state, as the uniform offline calls do
+        if (ensure(h, h->vl_tab, pl.tab.size())) return 1;
+        CK(h, cudaMemcpyAsync(h->vl_tab.p, pl.tab.data(), pl.tab.size() * sizeof(int), cudaMemcpyHostToDevice, rc.stream));
+        vl_tab = reinterpret_cast<const int*>(h->vl_tab.p);
+    }
 
     int T = T_in;
-    for (Op& op : ops) {
-        const int Tout = (T - 1) / op.down + 1;
+    for (size_t k = 0; k < ops.size(); ++k) {
+        Op& op = ops[k];
+        int Tout = (T - 1) / op.down + 1;
+        const int* vl_in = vl ? vl_tab + k * 2 * (rc.B + 1) : nullptr;
+        const int* vl_out = vl ? vl_in + rc.B + 1 : nullptr;
+        if (vl) { T = (int)pl.T[k]; Tout = (int)pl.Tout[k]; }
+        const int nb = vl ? 1 : rc.B;                        // varlen: one row space of concatenated utterances
         const float* xin = op.in_buf == BUF_EXT_IN ? rc.ext_in : h->ws[op.in_buf].p;
         float* yout = op.out_buf == BUF_EXT_OUT ? rc.ext_out : h->ws[op.out_buf].p;
         const float* st_in = op.st[op.cur];
@@ -665,16 +730,21 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
             StemArgs a{};
             a.x = xin; a.x_bs = T; a.st_in = st_in; a.st_out = st_out; a.T = T;
             a.w = op.w; a.bias = op.bias; a.y = yout; a.y_bs = (long long)T * op.ldy;
-            dim3 grid((T + 1023) / 1024, rc.B);
-            stem_kernel<32, 7><<<grid, 256, 0, rc.stream>>>(a);
+            a.vl_off = vl_in; a.vl_B = rc.B;
+            dim3 grid((T + 1023) / 1024, nb);
+            if (vl) stem_kernel<32, 7, true><<<grid, 256, 0, rc.stream>>>(a);
+            else stem_kernel<32, 7><<<grid, 256, 0, rc.stream>>>(a);
             e = cudaGetLastError();
         } else if (op.kind == OP_HEAD) {
             HeadArgs a{};
             a.x = xin; a.x_bs = (long long)T * op.ldx; a.ldx = op.ldx; a.st_in = st_in; a.st_out = st_out; a.T = T;
             a.w = op.w; a.bias = op.head_bias; a.pre_act = op.pre_act; a.slope = op.slope; a.post_tanh = op.post_tanh;
             a.y = yout; a.y_bs = T;
-            dim3 grid((T + 255) / 256, rc.B);
-            if (h->act_bf16) head_kernel<32, 7, true><<<grid, 256, 0, rc.stream>>>(a);
+            a.vl_off = vl_in; a.vl_B = rc.B;
+            dim3 grid((T + 255) / 256, nb);
+            if (vl && h->act_bf16) head_kernel<32, 7, true, true><<<grid, 256, 0, rc.stream>>>(a);
+            else if (vl) head_kernel<32, 7, false, true><<<grid, 256, 0, rc.stream>>>(a);
+            else if (h->act_bf16) head_kernel<32, 7, true><<<grid, 256, 0, rc.stream>>>(a);
             else head_kernel<32, 7, false><<<grid, 256, 0, rc.stream>>>(a);
             e = cudaGetLastError();
         } else {
@@ -699,7 +769,13 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
                 const int wrows = TC_TT + (op.Ktaps - 1) * op.dil;
                 dim3 grid((Tout + TC_TT - 1) / TC_TT, op.G * op.n_co_tiles, rc.B);
                 a.n_streams = rc.B;
-                if (h->stack_rows) {
+                if (vl) {
+                    // one stacked row space: utterance b owns Tout_b + halo rows (ConvArgs::vl_in / vl_out)
+                    const long long rows = (long long)Tout + (long long)rc.B * (op.Ktaps - 1) * op.dil;
+                    grid = dim3((unsigned)((rows + TC_TT - 1) / TC_TT), grid.y, 1);
+                    a.n_streams = 1;
+                    a.vl_in = vl_in; a.vl_out = vl_out; a.vl_B = rc.B;
+                } else if (h->stack_rows) {
                     // fill the 128-row tiles across streams when that needs fewer tiles (short chunks: 256 streams x 5..25 rows per layer)
                     const long long L = (long long)Tout + (long long)(op.Ktaps - 1) * op.dil;
                     const long long stacked = (rc.B * L + TC_TT - 1) / TC_TT;
@@ -714,7 +790,7 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
                 const size_t psmem = op.tc->smem(wrows, op.fuse);
                 a.n_wbuf = op.tc->n_wbuf(wrows, op.fuse);
                 if (a.n_wbuf < 1) return h->fail(fmt("%s: window of %d rows does not fit in shared memory", op.name.c_str(), wrows));
-                e = op.tc->pfn(a, (int)grid.x, (int)grid.y, (int)n_tiles, n_ctas, (int)psmem, rc.stream);
+                e = (vl ? op.tc->pfn_vl : op.tc->pfn)(a, (int)grid.x, (int)grid.y, (int)n_tiles, n_ctas, (int)psmem, rc.stream);
             } else {
                 const int TT = op.kc->TT;
                 dim3 grid((Tout + TT - 1) / TT, op.G * op.n_co_tiles, rc.B);
@@ -732,12 +808,12 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
             const double cin = op.kind == OP_STEM ? 1 : (double)op.G * op.Cin_eff / std::max(1, op.RG) * (op.shared_in ? 1.0 / op.G : 1.0);
             const double cout = op.kind == OP_HEAD ? 1 : (double)op.G * op.Cout;
             const double eb = h->act_bytes();
-            double bytes = eb * rc.B * (cin * T + cout * Tout);
-            if (op.fuse) bytes += eb * rc.B * (3.0 * cout * Tout);      // mid write+read (1x1 conv in/out) and the skip read
-            else if (op.res_buf >= 0) bytes += eb * rc.B * cout * Tout;
+            double bytes = eb * nb * (cin * T + cout * Tout);
+            if (op.fuse) bytes += eb * nb * (3.0 * cout * Tout);      // mid write+read (1x1 conv in/out) and the skip read
+            else if (op.res_buf >= 0) bytes += eb * nb * cout * Tout;
             h->prof_bytes.push_back(bytes);
         }
-        if (op.P > 0) op.cur ^= 1;
+        if (op.P > 0 && !vl) op.cur ^= 1;       // varlen calls neither read nor write the causal state
         T = Tout * op.up;
     }
     if (T_out_final) *T_out_final = T;
@@ -1158,7 +1234,7 @@ void adec_destroy(adec_handle* h) {
         for (Op& op : *ops)
             for (int i = 0; i < 2; ++i) if (op.st[i]) cudaFree(op.st[i]);
     for (auto& b : h->ws) if (b.p) cudaFree(b.p);
-    for (DevBuf* b : {&h->hx, &h->hz, &h->hzq, &h->hy}) if (b->p) cudaFree(b->p);
+    for (DevBuf* b : {&h->hx, &h->hz, &h->hzq, &h->hy, &h->vl_tab}) if (b->p) cudaFree(b->p);
     if (h->hidx) cudaFree(h->hidx);
     if (h->d_err) cudaFree(h->d_err);
     if (h->d_ktrace) cudaFree(h->d_ktrace);
@@ -1280,22 +1356,37 @@ int adec_encode(adec_handle* h, const float* x, int B, int T, float* z, void* st
     return run_ops(h, h->enc_ops, rc, T, nullptr);
 }
 
-// decode / decode_offline in either activation dtype: the entry point's I/O dtype must be the handle's (compute_dtype 2 = bf16)
-static int decode_common(adec_handle* h, const void* zq, int B, int F, void* y, void* stream, bool offline, bool bf16_io) {
+// the host arguments of a varlen offline call: B >= 1 utterances of >= 1 samples / frames each
+static int varlen_args(adec_handle* h, const char* name, const int* lengths, int B) {
+    if (B < 1) return h->fail(fmt("%s: B must be >= 1, got %d", name, B));
+    if (!lengths) return h->fail(fmt("%s: lengths is NULL", name));
+    for (int b = 0; b < B; ++b)
+        if (lengths[b] < 1) return h->fail(fmt("%s: utterance %d has length %d; every length must be >= 1", name, b, lengths[b]));
+    return 0;
+}
+
+// decode / decode_offline / decode_offline_varlen in either activation dtype: the entry point's I/O dtype must be the handle's
+// (compute_dtype 2 = bf16).  vl: a varlen call, vl_frames the HOST frame counts of its B utterances (F unused).
+static int decode_common(adec_handle* h, const void* zq, int B, int F, void* y, void* stream, bool offline, bool bf16_io,
+                         bool vl = false, const int* vl_frames = nullptr) {
     if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    const char* name = offline ? (bf16_io ? "decode_offline_bf16" : "decode_offline") : (bf16_io ? "decode_bf16" : "decode");
+    const char* base = vl ? "decode_offline_varlen" : offline ? "decode_offline" : "decode";
+    const std::string name = std::string(base) + (bf16_io ? "_bf16" : "");
     if (h->act_bf16 && !bf16_io)
-        return h->fail(fmt("%s: this handle has bf16 activations (compute_dtype 2); call adec_%s_bf16 with bf16 zq / y", name,
-                           offline ? "decode_offline" : "decode"));
+        return h->fail(fmt("%s: this handle has bf16 activations (compute_dtype 2); call adec_%s_bf16 with bf16 zq / y", name.c_str(), base));
     if (!h->act_bf16 && bf16_io)
-        return h->fail(fmt("%s: this handle has fp32 activations (compute_dtype %d); call adec_%s with fp32 zq / y", name, h->cfg.compute_dtype,
-                           offline ? "decode_offline" : "decode"));
-    if (bf16_io && (((uintptr_t)zq | (uintptr_t)y) & 15)) return h->fail(fmt("%s: zq and y must be 16-byte aligned", name));
-    if (B < 1 || F < 1) return h->fail(fmt("%s: empty input", name));
+        return h->fail(fmt("%s: this handle has fp32 activations (compute_dtype %d); call adec_%s with fp32 zq / y", name.c_str(),
+                           h->cfg.compute_dtype, base));
+    if (bf16_io && (((uintptr_t)zq | (uintptr_t)y) & 15)) return h->fail(fmt("%s: zq and y must be 16-byte aligned", name.c_str()));
+    if (vl) {
+        if (varlen_args(h, name.c_str(), vl_frames, B)) return 1;
+    } else if (B < 1 || F < 1) {
+        return h->fail(fmt("%s: empty input", name.c_str()));
+    }
     DeviceGuard dg(h->device);
-    if (offline && offline_state(h, B, (cudaStream_t)stream)) return 1;
-    RunCtx rc{B, (const float*)zq, (float*)y, (cudaStream_t)stream, offline};
-    return run_ops(h, h->dec_ops, rc, F, nullptr);
+    if (offline && !vl && offline_state(h, B, (cudaStream_t)stream)) return 1;
+    RunCtx rc{B, (const float*)zq, (float*)y, (cudaStream_t)stream, offline, vl ? vl_frames : nullptr, name.c_str()};
+    return run_ops(h, h->dec_ops, rc, vl ? 1 : F, nullptr);
 }
 
 int adec_decode(adec_handle* h, const float* zq, int B, int F, float* y, void* stream) {
@@ -1322,6 +1413,23 @@ int adec_decode_offline(adec_handle* h, const float* zq, int B, int F, float* y,
 
 int adec_decode_offline_bf16(adec_handle* h, const uint16_t* zq, int B, int F, uint16_t* y, void* stream) {
     return decode_common(h, zq, B, F, y, stream, true, true);
+}
+
+int adec_encode_offline_varlen(adec_handle* h, const float* x, const int* lengths, int B, float* z, void* stream) {
+    if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
+    if (h->cfg.model_type != ADEC_MODEL_SYMAD) return h->fail("encode_offline_varlen: not a symAD handle");
+    if (varlen_args(h, "encode_offline_varlen", lengths, B)) return 1;
+    DeviceGuard dg(h->device);
+    RunCtx rc{B, x, z, (cudaStream_t)stream, true, lengths, "encode_offline_varlen"};
+    return run_ops(h, h->enc_ops, rc, 1, nullptr);
+}
+
+int adec_decode_offline_varlen(adec_handle* h, const float* zq, const int* frames, int B, float* y, void* stream) {
+    return decode_common(h, zq, B, 0, y, stream, true, false, true, frames);
+}
+
+int adec_decode_offline_varlen_bf16(adec_handle* h, const uint16_t* zq, const int* frames, int B, uint16_t* y, void* stream) {
+    return decode_common(h, zq, B, 0, y, stream, true, true, true, frames);
 }
 
 static int index_bits(int n) { int b = 1; while ((1 << b) < n) ++b; return b; }

@@ -208,7 +208,26 @@ struct ConvArgs {
     int stack_L, n_streams;
     int* err;            // device flag word: bit 1 = an activation left the fp16-split range (|a| >= 6e4)
     unsigned long long* dbg;   // ADEC_KTRACE: {globaltimer at start, at end, SM cycles} of CTA 0, one record per launch (nullptr = off)
+    // varlen (the VL kernels): vl_B utterances of different lengths, concatenated along time in x, res and y.  Utterance u's input rows
+    // are [vl_in[u], vl_in[u + 1]) and its output rows [vl_out[u], vl_out[u + 1]) (B + 1 entries each); in the tiles' row space it owns
+    // the stacked rows [vl_row(u), vl_row(u + 1)), vl_row(u) = vl_out[u] + u * (Ktaps - 1) * dil, as stack_L does for equal lengths.
+    // Every utterance starts from zero history; T and Tout are the totals.
+    const int* vl_in;
+    const int* vl_out;
+    int vl_B;
 };
+
+// varlen row spaces: utterance u owns rows [off[u] + u * halo, off[u + 1] + (u + 1) * halo); off has B + 1 ascending entries
+__device__ __forceinline__ int vl_row(const int* off, int halo, int u) { return __ldg(off + u) + u * halo; }
+// the utterance that owns row j (the last one for rows past the end)
+__device__ __forceinline__ int vl_find(const int* off, int halo, int B, int j) {
+    int lo = 0, hi = B - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (vl_row(off, halo, mid) <= j) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
 
 constexpr int CONV_STAGES = 4;
 
@@ -451,9 +470,11 @@ struct StemArgs {
     const float* w;                      // [K][COUT]
     const float* bias;                   // [COUT] or nullptr
     float* y; long long y_bs;
+    const int* vl_off; int vl_B;         // VL: utterance u is rows [vl_off[u], vl_off[u + 1]) of x and y (B = 1, T = the total)
 };
 
-template <int COUT, int K>
+// VL: one row space of concatenated utterances, each with a zero left pad; no state is read or written
+template <int COUT, int K, bool VL = false>
 __global__ void __launch_bounds__(256) stem_kernel(const StemArgs a) {
     constexpr int TT = 1024, P = K - 1, Q = COUT / 4;
     __shared__ float xw[TT + P];
@@ -464,7 +485,7 @@ __global__ void __launch_bounds__(256) stem_kernel(const StemArgs a) {
     for (int i = tid; i < TT + P; i += 256) {
         const long long r = (long long)j0 + i;       // x~ row
         float v = 0.f;
-        if (r < P) v = a.st_in[b * P + r];
+        if (r < P) { if (!VL) v = a.st_in[b * P + r]; }
         else if (r - P < a.T) v = __ldg(xg + r - P);
         xw[i] = v;
     }
@@ -474,12 +495,19 @@ __global__ void __launch_bounds__(256) stem_kernel(const StemArgs a) {
     const int q = tid % Q, tl = tid / Q;
     constexpr int TSTEP = 256 / Q;
     float* yg = a.y + (long long)b * a.y_bs;
+    int u = 0, u_start = 0, u_next = 0;              // VL: the utterance of row j0 + t, its first row, the next one's first row
+    if (VL && j0 + tl < a.T) {
+        u = vl_find(a.vl_off, 0, a.vl_B, j0 + tl);
+        u_start = __ldg(a.vl_off + u);
+        u_next = __ldg(a.vl_off + u + 1);
+    }
     for (int t = tl; t < TT; t += TSTEP) {
         if (j0 + t >= a.T) break;
+        if (VL) while (j0 + t >= u_next) { ++u; u_start = u_next; u_next = __ldg(a.vl_off + u + 1); }
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
         for (int k = 0; k < K; ++k) {
-            const float xv = xw[t + k];
+            const float xv = (!VL || j0 + t + k - P >= u_start) ? xw[t + k] : 0.f;   // taps before the utterance: its zero pad
             const float4 w4 = *reinterpret_cast<const float4*>(sw + k * COUT + q * 4);
             acc.x = fmaf(xv, w4.x, acc.x); acc.y = fmaf(xv, w4.y, acc.y);
             acc.z = fmaf(xv, w4.z, acc.z); acc.w = fmaf(xv, w4.w, acc.w);
@@ -488,7 +516,7 @@ __global__ void __launch_bounds__(256) stem_kernel(const StemArgs a) {
         acc.x += b4.x; acc.y += b4.y; acc.z += b4.z; acc.w += b4.w;
         *reinterpret_cast<float4*>(yg + (long long)(j0 + t) * COUT + q * 4) = acc;
     }
-    if (blockIdx.x == gridDim.x - 1) {
+    if (!VL && blockIdx.x == gridDim.x - 1) {
         for (int r = tid; r < P; r += 256) {
             const long long i = (long long)a.T + r;
             a.st_out[b * P + r] = (i < P) ? a.st_in[b * P + i] : xg[i - P];
@@ -506,6 +534,7 @@ struct HeadArgs {
     const float* w;                      // [K][CIN]
     float bias; int pre_act; float slope; int post_tanh;
     float* y; long long y_bs;
+    const int* vl_off; int vl_B;         // VL: utterance u is rows [vl_off[u], vl_off[u + 1]) of x and y (B = 1, T = the total)
 };
 
 // Eight lanes share one run of R = 8 consecutive outputs: lane c4 owns channels 4*c4..4*c4+3, loads the R + K - 1 window rows of its
@@ -514,8 +543,9 @@ struct HeadArgs {
 // the K x 4 weights it keeps in registers; three xor-shuffles add the eight shares and lane j stores output j.  The layer moves
 // 128 B per output row and does 2*K*CIN flops on it: memory-bound once the LDS traffic of the round-1 version (112 LDS.128 per output)
 // is gone.  BST: bf16 input, state and output (the vocoder's bf16-activation mode); a chunk row enters the window as the bf16 value the
-// state keeps of it, so that a streamed chunk and a one-shot call see the same window.
-template <int CIN, int K, bool BST>
+// state keeps of it, so that a streamed chunk and a one-shot call see the same window.  VL: concatenated utterances, each with a zero
+// left pad (a run of eight outputs may span several of them, so each output masks the taps that fall before its utterance).
+template <int CIN, int K, bool BST, bool VL = false>
 __global__ void __launch_bounds__(256) head_kernel(const HeadArgs a) {
     static_assert(CIN == 32, "eight lanes x four channels");
     using XT = typename std::conditional<BST, __nv_bfloat16, float>::type;
@@ -536,16 +566,26 @@ __global__ void __launch_bounds__(256) head_kernel(const HeadArgs a) {
         for (int r = 0; r < R + P; ++r) {
             const long long i = (long long)t0 + r;                  // x~ row = history(P) || chunk
             xv[r] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (i < P) xv[r] = ldg4(sg + i * CIN + 4 * c4);          // state rows are stored post-activation
+            if (i < P) { if (!VL) xv[r] = ldg4(sg + i * CIN + 4 * c4); }   // state rows are stored post-activation
             else if (i - P < a.T) xv[r] = stored4<BST>(apply_act(ldg4(xg + (i - P) * a.ldx + 4 * c4), a.pre_act, a.slope));
         }
+        int u = 0, u_start = 0, u_next = 0;
+        if (VL) {
+            u = vl_find(a.vl_off, 0, a.vl_B, t0);
+            u_start = __ldg(a.vl_off + u);
+            u_next = __ldg(a.vl_off + u + 1);
+        }
 #pragma unroll
-        for (int j = 0; j < R; ++j)
+        for (int j = 0; j < R; ++j) {
+            if (VL) while (u + 1 < a.vl_B && t0 + j >= u_next) { ++u; u_start = u_next; u_next = __ldg(a.vl_off + u + 1); }
 #pragma unroll
             for (int k = 0; k < K; ++k) {
-                acc[j] = fmaf(xv[j + k].x, w[k].x, acc[j]); acc[j] = fmaf(xv[j + k].y, w[k].y, acc[j]);
-                acc[j] = fmaf(xv[j + k].z, w[k].z, acc[j]); acc[j] = fmaf(xv[j + k].w, w[k].w, acc[j]);
+                float4 x = xv[j + k];
+                if (VL && t0 + j + k - P < u_start) x = make_float4(0.f, 0.f, 0.f, 0.f);
+                acc[j] = fmaf(x.x, w[k].x, acc[j]); acc[j] = fmaf(x.y, w[k].y, acc[j]);
+                acc[j] = fmaf(x.z, w[k].z, acc[j]); acc[j] = fmaf(x.w, w[k].w, acc[j]);
             }
+        }
     }
     float mine = 0.f;
 #pragma unroll
@@ -561,7 +601,7 @@ __global__ void __launch_bounds__(256) head_kernel(const HeadArgs a) {
         if (a.post_tanh) mine = tanhf(mine);
         st1(reinterpret_cast<XT*>(a.y) + (long long)b * a.y_bs + t0 + c4, mine);
     }
-    if (blockIdx.x == gridDim.x - 1) {
+    if (!VL && blockIdx.x == gridDim.x - 1) {
         XT* so = reinterpret_cast<XT*>(a.st_out) + (long long)b * P * CIN;
         for (int idx = tid; idx < P * (CIN / 4); idx += 256) {
             const int r = idx / (CIN / 4), ci = (idx - r * (CIN / 4)) * 4;

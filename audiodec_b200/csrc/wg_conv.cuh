@@ -242,7 +242,9 @@ __device__ __forceinline__ void wg_group(float (&d)[WgCfg<NT, PREC>::PW / 2], ui
 }
 
 // BST: activations, causal state, residual and output stored as bf16 in HBM (bf16 operands only; no 4-channel strided convs)
-template <int NT, bool FUSE, int PRE, int PREC, bool BST>
+// VL: utterances of different lengths in one stacked row space (ConvArgs::vl_in / vl_out), zero history, no state written; a separate
+// instantiation, so that the uniform kernels keep their code
+template <int NT, bool FUSE, int PRE, int PREC, bool BST, bool VL = false>
 __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(const ConvArgs a, int n_xtiles, int n_ytiles, int n_tiles) {
     static_assert(!BST || (PREC == PREC_BF16 && !FUSE), "bf16 storage is built for the non-fused bf16-operand kernels");
     using Cfg = WgCfg<NT, PREC>;
@@ -323,6 +325,18 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
             const int j0 = xt * TT;
             const XT* xg = reinterpret_cast<const XT*>(a.x) + (long long)b * a.x_bs + g * a.x_goff;
             const XT* sg = reinterpret_cast<const XT*>(a.st_in) + (long long)b * a.P * a.st_ld + g * a.st_goff;
+            // VL: the utterance u0 that owns row j0, the first rows of it and of the next one, its input rows and length
+            const int halo = (a.Ktaps - 1) * a.dil;
+            int u0 = 0, u0_start = 0, u0_next = 0, u0_T = 0;
+            const XT* xu0 = xg;
+            if constexpr (VL) {
+                u0 = vl_find(a.vl_out, halo, a.vl_B, j0);
+                u0_start = vl_row(a.vl_out, halo, u0);
+                u0_next = vl_row(a.vl_out, halo, u0 + 1);
+                const int i0 = __ldg(a.vl_in + u0);
+                u0_T = __ldg(a.vl_in + u0 + 1) - i0;
+                xu0 = xg + (long long)i0 * a.ldx;
+            }
             for (int p = 0; p < a.n_pieces; ++p) {
                 const int buf = wb;
                 const uint32_t wpar = (uint32_t)(wround - 1) & 1u;
@@ -333,11 +347,21 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                 const int q = p * CP + c8 * 8;
                 int r = 0, ci = q;
                 if (a.RG > 1) { r = q >> a.lgCin; ci = q & (a.Cin - 1); }
-                const long long i_first = (long long)j0 * a.RG + r;
-                const long long i_last = (long long)(j0 + wrows - 1) * a.RG + r;
-                if (i_first >= a.P && i_last - a.P < a.T && PRE != ACT_NORM && !halves && !a.stack_L) {
-                    // interior piece: every row comes from the chunk
-                    const XT* xp = xg + ci + (i_first - a.P + (long long)m0 * a.RG) * a.ldx;
+                long long i_first = (long long)j0 * a.RG + r;
+                long long i_last = (long long)(j0 + wrows - 1) * a.RG + r;
+                const XT* xb = xg;
+                int Tb = a.T;
+                bool one_utt = true;
+                if constexpr (VL) {
+                    i_first = (long long)(j0 - u0_start) * a.RG + r;
+                    i_last = (long long)(j0 - u0_start + wrows - 1) * a.RG + r;
+                    xb = xu0;
+                    Tb = u0_T;
+                    one_utt = j0 + wrows <= u0_next;
+                }
+                if (i_first >= a.P && i_last - a.P < Tb && one_utt && PRE != ACT_NORM && !halves && !a.stack_L) {
+                    // interior piece: every row comes from the chunk (VL: from one utterance)
+                    const XT* xp = xb + ci + (i_first - a.P + (long long)m0 * a.RG) * a.ldx;
                     const long long xstep = (long long)RPP * a.RG * a.ldx;
                     for (int mb = m0; mb < wrows; mb += RPP * UNR, xp += xstep * UNR) {
                         float4 u[UNR], v[UNR];
@@ -354,6 +378,9 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                 } else {
                     // edge piece: rows from the causal state (stored post-activation), the chunk, or beyond its end (zeros)
                     int ci2 = ci + 4;
+                    // VL: this thread's rows ascend, so the utterance of each is found by stepping forward from u0
+                    int vu = u0, vu_start = u0_start, vu_next = u0_next, vu_T = u0_T;
+                    const XT* xvu = xu0;
                     for (int mb = m0; mb < wrows; mb += RPP * UNR_E) {
                         float4 u[UNR_E], v[UNR_E];
                         unsigned act = 0u;
@@ -367,7 +394,18 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                                 const XT* xs = xg;
                                 const XT* ss = sg;
                                 bool live = true;
-                                if (a.stack_L) {
+                                if constexpr (VL) {
+                                    while (vu + 1 < a.vl_B && ml >= vu_next) {
+                                        ++vu;
+                                        vu_start = vu_next;
+                                        vu_next = vl_row(a.vl_out, halo, vu + 1);
+                                        const int i0 = __ldg(a.vl_in + vu);
+                                        vu_T = __ldg(a.vl_in + vu + 1) - i0;
+                                        xvu = xg + (long long)i0 * a.ldx;
+                                    }
+                                    ml -= vu_start;
+                                    xs = xvu;
+                                } else if (a.stack_L) {
                                     const int sm = ml / a.stack_L;
                                     ml -= sm * a.stack_L;
                                     live = sm < a.n_streams;
@@ -380,8 +418,8 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                                     long long ti = i - a.P;
                                     if (a.hist_rep && ti < 0) ti = 0;
                                     if (live) {
-                                        if (ti < 0) ldg8(ss + i * a.st_ld + ci, u[k], v[k]);
-                                        else if (ti < a.T) { ldg8(xs + ti * a.ldx + ci, u[k], v[k]); act |= 3u << (2 * k); }
+                                        if (ti < 0) { if (!VL) ldg8(ss + i * a.st_ld + ci, u[k], v[k]); }   // VL: zero history
+                                        else if (ti < (VL ? vu_T : a.T)) { ldg8(xs + ti * a.ldx + ci, u[k], v[k]); act |= 3u << (2 * k); }
                                     }
                                 } else {
 #pragma unroll
@@ -393,8 +431,8 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                                         if (a.hist_rep && ti < 0) ti = 0;              // non-streaming transposed conv: replicate the first input row
                                         float4 w4 = make_float4(0.f, 0.f, 0.f, 0.f);
                                         if (live) {
-                                            if (ti < 0) w4 = __ldg(reinterpret_cast<const float4*>(ss + i * a.st_ld + cc));
-                                            else if (ti < a.T) { w4 = __ldg(reinterpret_cast<const float4*>(xs + ti * a.ldx + cc)); act |= 1u << (2 * k + hf); }
+                                            if (ti < 0) { if (!VL) w4 = __ldg(reinterpret_cast<const float4*>(ss + i * a.st_ld + cc)); }
+                                            else if (ti < (VL ? vu_T : a.T)) { w4 = __ldg(reinterpret_cast<const float4*>(xs + ti * a.ldx + cc)); act |= 1u << (2 * k + hf); }
                                         }
                                         if (hf) v[k] = w4; else u[k] = w4;
                                     }
@@ -418,7 +456,7 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                 mbar_arrive(&w_full[buf]);
             }
             // ---- new causal state (conv_layer.py:155): written by the CTA whose tile holds the stream's last output row
-            if (co_tile == 0 && g < a.st_groups && a.P > 0) {
+            if (!VL && co_tile == 0 && g < a.st_groups && a.P > 0) {
                 int s_lo = b, s_hi = b - 1;
                 if (a.stack_L) {
                     // streams whose last valid row sm * L + Tout - 1 lies in [j0, j0 + TT)
@@ -534,11 +572,27 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
             }
             // ---- epilogue: rows wrow and wrow + 8 of the tile, column pairs of this thread's fragment
             const float oscale = FUSE ? a.w2_scale : a.w_scale;
+            // VL: the utterance of row j0 + wrow (then of row + 8) and where its stacked rows start and end
+            int vu = 0, vu_start = 0, vu_next = 0;
+            const int halo = (a.Ktaps - 1) * a.dil;
+            if constexpr (VL) {
+                vu = vl_find(a.vl_out, halo, a.vl_B, j0 + wrow);
+                vu_start = vl_row(a.vl_out, halo, vu);
+                vu_next = vl_row(a.vl_out, halo, vu + 1);
+            }
 #pragma unroll
             for (int hr = 0; hr < 2; ++hr) {
                 int bo = b, t = j0 + wrow + 8 * hr;
-                if (a.stack_L) { bo = t / a.stack_L; t -= bo * a.stack_L; }
-                if (!(t < a.Tout && bo < a.n_streams)) continue;
+                if constexpr (VL) {
+                    // local row t - vu_start of the utterance; rows past its Tout are the receptive-field overlap, computed and dropped
+                    while (vu + 1 < a.vl_B && t >= vu_next) { ++vu; vu_start = vu_next; vu_next = vl_row(a.vl_out, halo, vu + 1); }
+                    const int o0 = __ldg(a.vl_out + vu), ml = t - vu_start;
+                    if (ml >= __ldg(a.vl_out + vu + 1) - o0) continue;
+                    t = o0 + ml;
+                } else {
+                    if (a.stack_L) { bo = t / a.stack_L; t -= bo * a.stack_L; }
+                    if (!(t < a.Tout && bo < a.n_streams)) continue;
+                }
 #pragma unroll
                 for (int i = 2 * hr; i < NACC; i += 4) {
                     const int h = i / (PW / 2), fi = i % (PW / 2);

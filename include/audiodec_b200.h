@@ -125,6 +125,20 @@ int adec_decode_offline(adec_handle *h, const float *zq, int B, int F, float *y,
 /* adec_decode_offline for a compute_dtype 2 handle: bf16 zq (B,F,in_channels) channels-last -> bf16 y (B,1,F*hop), 16-byte aligned. */
 int adec_decode_offline_bf16(adec_handle *h, const uint16_t *zq, int B, int F, uint16_t *y, void *stream);
 
+/* The same forwards over B utterances of DIFFERENT lengths in one launch sequence (codecTest.py transcodes a folder of them):
+ * utterance b gives exactly what a uniform offline call of its own length gives, and no padded rows are computed.
+ * Encoder.forward + Projector.forward: x is the utterances' samples concatenated, (sum T_b) device floats.  lengths: HOST array of B
+ * sample counts (>= 1).  z: (code_dim, sum F_b) channels-first, utterance b's frames at columns [sum_{i<b} F_i, +F_b),
+ * F_b = adec_frames_for(h, T_b).  This is the uniform layout with B = 1, F = sum F_b, so adec_quantize* and adec_lookup* take it
+ * unchanged.  Discards the streaming state, as adec_encode_offline does.  Every row count of the batch must fit in 31 bits. */
+int adec_encode_offline_varlen(adec_handle *h, const float *x, const int *lengths, int B, float *z, void *stream);
+/* Decoder.forward / HiFi-GAN Generator.forward over B utterances.  zq: (sum F_b, code_dim) channels-last.  frames: HOST array of B
+ * frame counts (>= 1).  y: (sum F_b * hop) device floats, utterance b at [hop * sum_{i<b} F_i, +hop * F_b). */
+int adec_decode_offline_varlen(adec_handle *h, const float *zq, const int *frames, int B, float *y, void *stream);
+/* adec_decode_offline_varlen for a compute_dtype 2 handle: bf16 zq and y, 16-byte aligned. */
+int adec_decode_offline_varlen_bf16(adec_handle *h, const uint16_t *zq, const int *frames, int B, uint16_t *y, void *stream);
+/* The varlen entry points need a tensor-core engine (f16 or tf32); the FFMA engine (ADEC_CONV_PATH=ffma) refuses them. */
+
 /* output frames of encode for T input samples: floor((T-1)/s)+1 applied per stride (conv_layer.py:153-156) */
 int adec_frames_for(const adec_handle *h, int T);
 /* product of the strides (utils/audiodec.py:58-62) */
