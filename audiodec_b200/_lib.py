@@ -65,6 +65,10 @@ SYMBOLS = {
     "adec_encode_offline_varlen": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),
     "adec_decode_offline_varlen": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),
     "adec_decode_offline_varlen_bf16": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),
+    "adec_encode_streams": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),
+    "adec_decode_streams": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),
+    "adec_decode_streams_bf16": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),
+    "adec_copy_stream_state": (c_int, [c_void_p, c_int, ctypes.POINTER(c_int), c_int, c_void_p]),
     "adec_frames_for": (c_int, [c_void_p, c_int]),
     "adec_hop_length": (c_int, [c_void_p]),
     "adec_codec_host": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),

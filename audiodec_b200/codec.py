@@ -204,6 +204,19 @@ class _StreamGeneratorBase:
         self._ready()
         _check(self._lib.adec_reset(self._h, self._stream()), self._h)
 
+    # ---- stream slots: every stream of the handle (n_streams, see set_streams) is a slot with its own causal state
+    def set_streams(self, n):
+        """Resize the handle to n stream slots.  Existing streams keep their state; growing from one stream replicates its state."""
+        self._ready()
+        self._batch(int(n))
+
+    def copy_stream_state(self, src, dst):
+        """Copy stream `src`'s current causal state into stream(s) `dst` (an int or a list): a joining stream starts warm."""
+        self._ready()
+        dst = [dst] if isinstance(dst, int) else list(dst)
+        arr, n = _int_array(dst)
+        _check(self._lib.adec_copy_stream_state(self._h, int(src), arr, n, self._stream()), self._h)
+
 
 class SymADStreamGenerator(_StreamGeneratorBase):
     """models/autoencoder/AudioDec.py:166-256."""
@@ -350,6 +363,34 @@ class SymADStreamGenerator(_StreamGeneratorBase):
         _check(self._lib.adec_encode_offline_varlen(self._h, _ptr(x), arr, b, _ptr(z), self._stream()), self._h)
         return z, frames
 
+    def encode_streams(self, chunks, streams):
+        """Advance streams[b] by chunks[b] (1-D (T_b,) or (1, T_b); lengths may differ) in one launch sequence.  Returns
+        (z (1, code_dim, sum F_b), [F_b]) laid out like encode_offline_varlen; stream b's frames equal a B = 1 streaming encode of its
+        chunk.  Streams not listed keep their state untouched."""
+        self._ready()
+        flat = []
+        for x in chunks:
+            x = x[0] if x.dim() == 2 and x.size(0) == 1 else x
+            if x.dim() != 1:
+                raise RuntimeError(f"audiodec_b200: encode_streams: expected 1-D (T,) or (1, T) chunks, got {tuple(x.shape)}")
+            flat.append(self._in(x))
+        if len(flat) != len(streams):
+            raise RuntimeError(f"audiodec_b200: encode_streams: {len(flat)} chunks for {len(streams)} streams")
+        lengths = [x.numel() for x in flat]
+        frames, offsets = varlen_layout(lengths, self.enc_strides)
+        x = torch.cat(flat) if flat else torch.empty(0, device=self._device)
+        z = torch.empty(1, self.code_dim, offsets[-1], device=self._device, dtype=torch.float32)
+        arr, b = _int_array(lengths)
+        sarr, _ = _int_array(streams)
+        _check(self._lib.adec_encode_streams(self._h, _ptr(x), arr, sarr, b, _ptr(z), self._stream()), self._h)
+        return z, frames
+
+    def decode_streams(self, zq, frames, streams):
+        """Advance streams[b] by frames[b] frames of zq ((1, sum F_b, code_dim) or (sum F_b, code_dim) channels-last, as lookup
+        returns it) in one launch sequence -> list of B waveforms (1, 1, F_b * hop), views of one output buffer, each equal to a
+        B = 1 streaming decode of those frames.  Streams not listed keep their state untouched."""
+        return _decode_streams(self, zq, frames, streams)
+
     def quantize_offline(self, z):
         """z (B,code_dim,F) -> (zq (B,code_dim,F) channels-first like Quantizer.forward (quantizer.py:31-34), idx (Nq,B,F))."""
         self._ready()
@@ -462,6 +503,34 @@ def _decode_offline_varlen(gen, zq, frames):
     return out
 
 
+def _decode_streams(gen, zq, frames, streams):
+    gen._ready()
+    d = getattr(gen, "code_dim", None) or gen.in_channels
+    frames = [int(f) for f in frames]
+    if zq.dim() == 3 and zq.size(0) == 1:
+        zq = zq[0]
+    if zq.dim() != 2 or zq.size(0) != sum(frames) or zq.size(1) != d:
+        raise RuntimeError(f"audiodec_b200: decode_streams: expected (1, {sum(frames)}, {d}) channels-last for frames summing to "
+                           f"{sum(frames)}, got {tuple(zq.shape)}")
+    if len(frames) != len(streams):
+        raise RuntimeError(f"audiodec_b200: decode_streams: {len(frames)} frame counts for {len(streams)} streams")
+    dtype = torch.bfloat16 if gen._act_bf16 else torch.float32
+    zq = gen._in(zq, dtype)
+    if gen._act_bf16 and zq.data_ptr() % 16:
+        zq = zq.clone()                                             # the bf16 kernels read zq as 16-byte vectors
+    hop = gen._lib.adec_hop_length(gen._h)
+    y = torch.empty(sum(frames) * hop, device=gen._device, dtype=dtype)
+    arr, b = _int_array(frames)
+    sarr, _ = _int_array(streams)
+    fn = gen._lib.adec_decode_streams_bf16 if gen._act_bf16 else gen._lib.adec_decode_streams
+    _check(fn(gen._h, _ptr(zq), arr, sarr, b, _ptr(y), gen._stream()), gen._h)
+    out, o = [], 0
+    for f in frames:
+        out.append(y[o * hop:(o + f) * hop].view(1, 1, f * hop))
+        o += f
+    return out
+
+
 class HiFiGANStreamGenerator(_StreamGeneratorBase):
     """models/vocoder/HiFiGAN.py:222-305 (AD v1: groups>1 and a single resblock kernel -> MultiGroupConv1d)."""
 
@@ -541,6 +610,12 @@ class HiFiGANStreamGenerator(_StreamGeneratorBase):
         utterance b at columns [sum_{i<b} F_i, +F_b) -> list of B waveforms (1, 1, F_b * hop), views of one output buffer (bf16 with
         bf16 activations), each equal to forward of that utterance alone."""
         return _decode_offline_varlen(self, c, frames)
+
+    def decode_streams(self, c, frames, streams):
+        """Advance streams[b] by frames[b] frames of c ((1, sum F_b, in_channels) or (sum F_b, in_channels) channels-last) in one
+        launch sequence -> list of B waveforms (1, 1, F_b * hop), views of one output buffer (bf16 with bf16 activations), each equal to
+        a B = 1 streaming decode of those frames.  Streams not listed keep their state untouched."""
+        return _decode_streams(self, c, frames, streams)
 
 
 class OfflineCodec:

@@ -206,6 +206,15 @@ struct DevBuf {
     size_t cap = 0;
 };
 
+// Stream slots of one op list (encoder or decoder): bit[s] = 1 when stream s's current state is in st[cur ^ 1] of every stateful op
+// of the list rather than st[cur].  Slot calls advance a subset of streams without flipping op.cur: they flip the bits of the streams
+// they advance instead.  Calls that know nothing of slots (uniform encode / decode, adec_set_streams) first copy the flipped streams
+// back into st[cur] (only when a slot call has happened since the last time: `dirty`).
+struct SlotBits {
+    std::vector<uint8_t> bit;
+    bool dirty = false;
+};
+
 }  // namespace
 
 struct adec_handle {
@@ -241,6 +250,8 @@ struct adec_handle {
     // host-path scratch
     DevBuf hx, hz, hzq, hy;
     DevBuf vl_tab;                // varlen row tables of the last call (ints)
+    SlotBits enc_slots, dec_slots;
+    DevBuf slot_tab;              // stream pairs of the last state copy (ints)
     long long* hidx = nullptr;
     size_t hidx_cap = 0;
 
@@ -634,9 +645,47 @@ struct RunCtx {
     float* ext_out;
     cudaStream_t stream;
     bool offline = false;   // non-streaming forward: transposed convs replicate their first input row instead of reading state
-    const int* vl_len = nullptr;   // varlen: HOST lengths of the B utterances, concatenated along time in ext_in / ext_out (offline only)
+    const int* vl_len = nullptr;   // varlen: HOST lengths of the B utterances, concatenated along time in ext_in / ext_out
     const char* what = "";         // entry point, for messages
+    const int* slots = nullptr;    // varlen streaming (adec_*_streams): HOST stream slot of each utterance; nullptr = offline varlen
 };
+
+SlotBits* slot_bits(adec_handle* h, const std::vector<Op>& ops) {
+    return &ops == &h->enc_ops ? &h->enc_slots : &ops == &h->dec_ops ? &h->dec_slots : nullptr;
+}
+
+// Copy per-stream state rows of every stateful op of `ops`: pair j copies stream pairs[2j] of st[cur ^ src_sel] to stream pairs[2j + 1]
+// of st[cur ^ dst_sel].  The pairs go up in one copy on `stream`.
+int slot_copy(adec_handle* h, std::vector<Op>& ops, const std::vector<int>& pairs, int src_sel, int dst_sel, cudaStream_t stream) {
+    const int n = (int)pairs.size() / 2;
+    if (n == 0) return 0;
+    if (ensure(h, h->slot_tab, pairs.size())) return 1;
+    CK(h, cudaMemcpyAsync(h->slot_tab.p, pairs.data(), pairs.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
+    for (Op& op : ops) {
+        const long long per = (long long)op.P * op.st_C * h->act_bytes() / 4;     // words per stream (see resize_state)
+        if (!per) continue;
+        const long long tot = per * n;
+        slot_copy_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(op.st[op.cur ^ dst_sel], op.st[op.cur ^ src_sel], per,
+                                                                          reinterpret_cast<const int*>(h->slot_tab.p), n);
+        CK(h, cudaGetLastError());
+        ++h->launches;
+    }
+    return 0;
+}
+
+// Put every stream's current state back into st[cur] (the layout the uniform calls and adec_set_streams know): one copy of the streams
+// whose bit is set, and only if a slot call has happened since the last time.
+int slot_fixup(adec_handle* h, std::vector<Op>& ops, cudaStream_t stream) {
+    SlotBits* sb = slot_bits(h, ops);
+    if (!sb || !sb->dirty) return 0;
+    std::vector<int> pairs;
+    for (int s = 0; s < (int)sb->bit.size(); ++s)
+        if (sb->bit[s]) { pairs.push_back(s); pairs.push_back(s); }
+    if (slot_copy(h, ops, pairs, 1, 0, stream)) return 1;
+    std::fill(sb->bit.begin(), sb->bit.end(), 0);
+    sb->dirty = false;
+    return 0;
+}
 
 // varlen row spaces must stay inside the kernels' 32-bit row indices, with room for a tile and its halo past the end
 constexpr long long kVlMaxRows = (1ll << 31) - 4096;
@@ -701,11 +750,27 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
         if (need[i] && ensure(h, h->ws[i], (need[i] * h->act_bytes() + 3) / 4)) return 1;
     if (!vl && rc.B != h->n_streams) return h->fail(fmt("batch %d != n_streams %d (call adec_set_streams)", rc.B, h->n_streams));
     const int* vl_tab = nullptr;
-    if (vl) {
+    const int* vl_slot = nullptr;
+    SlotBits* sb = slot_bits(h, ops);
+    if (vl && rc.slots) {
+        // streaming varlen: the slot table (2 * slot + bit per utterance, the same for every op) follows the row tables in the one copy
+        for (const Op& op : ops)      // the conv kernels address a slot's history rows with 32-bit element offsets
+            if ((long long)h->n_streams * op.P * op.st_C >= (1ll << 31))
+                return h->fail(fmt("%s: %d streams of %s state exceed 2^31 elements per buffer; use fewer streams per handle", rc.what,
+                                   h->n_streams, op.name.c_str()));
+        const size_t at = pl.tab.size();
+        for (int b = 0; b < rc.B; ++b) pl.tab.push_back(2 * rc.slots[b] + sb->bit[rc.slots[b]]);
+        if (ensure(h, h->vl_tab, pl.tab.size())) return 1;
+        CK(h, cudaMemcpyAsync(h->vl_tab.p, pl.tab.data(), pl.tab.size() * sizeof(int), cudaMemcpyHostToDevice, rc.stream));
+        vl_tab = reinterpret_cast<const int*>(h->vl_tab.p);
+        vl_slot = vl_tab + at;
+    } else if (vl) {
         if (adec_reset(h, (void*)rc.stream)) return 1;      // discards the streaming state, as the uniform offline calls do
         if (ensure(h, h->vl_tab, pl.tab.size())) return 1;
         CK(h, cudaMemcpyAsync(h->vl_tab.p, pl.tab.data(), pl.tab.size() * sizeof(int), cudaMemcpyHostToDevice, rc.stream));
         vl_tab = reinterpret_cast<const int*>(h->vl_tab.p);
+    } else if (slot_fixup(h, ops, rc.stream)) {
+        return 1;
     }
 
     int T = T_in;
@@ -730,7 +795,7 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
             StemArgs a{};
             a.x = xin; a.x_bs = T; a.st_in = st_in; a.st_out = st_out; a.T = T;
             a.w = op.w; a.bias = op.bias; a.y = yout; a.y_bs = (long long)T * op.ldy;
-            a.vl_off = vl_in; a.vl_B = rc.B;
+            a.vl_off = vl_in; a.vl_B = rc.B; a.vl_slot = vl_slot;
             dim3 grid((T + 1023) / 1024, nb);
             if (vl) stem_kernel<32, 7, true><<<grid, 256, 0, rc.stream>>>(a);
             else stem_kernel<32, 7><<<grid, 256, 0, rc.stream>>>(a);
@@ -740,7 +805,7 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
             a.x = xin; a.x_bs = (long long)T * op.ldx; a.ldx = op.ldx; a.st_in = st_in; a.st_out = st_out; a.T = T;
             a.w = op.w; a.bias = op.head_bias; a.pre_act = op.pre_act; a.slope = op.slope; a.post_tanh = op.post_tanh;
             a.y = yout; a.y_bs = T;
-            a.vl_off = vl_in; a.vl_B = rc.B;
+            a.vl_off = vl_in; a.vl_B = rc.B; a.vl_slot = vl_slot;
             dim3 grid((T + 255) / 256, nb);
             if (vl && h->act_bf16) head_kernel<32, 7, true, true><<<grid, 256, 0, rc.stream>>>(a);
             else if (vl) head_kernel<32, 7, false, true><<<grid, 256, 0, rc.stream>>>(a);
@@ -774,7 +839,7 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
                     const long long rows = (long long)Tout + (long long)rc.B * (op.Ktaps - 1) * op.dil;
                     grid = dim3((unsigned)((rows + TC_TT - 1) / TC_TT), grid.y, 1);
                     a.n_streams = 1;
-                    a.vl_in = vl_in; a.vl_out = vl_out; a.vl_B = rc.B;
+                    a.vl_in = vl_in; a.vl_out = vl_out; a.vl_B = rc.B; a.vl_slot = vl_slot;
                 } else if (h->stack_rows) {
                     // fill the 128-row tiles across streams when that needs fewer tiles (short chunks: 256 streams x 5..25 rows per layer)
                     const long long L = (long long)Tout + (long long)(op.Ktaps - 1) * op.dil;
@@ -813,8 +878,12 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
             else if (op.res_buf >= 0) bytes += eb * nb * cout * Tout;
             h->prof_bytes.push_back(bytes);
         }
-        if (op.P > 0 && !vl) op.cur ^= 1;       // varlen calls neither read nor write the causal state
+        if (op.P > 0 && !vl) op.cur ^= 1;       // offline varlen calls neither read nor write the causal state; slot calls flip bits below
         T = Tout * op.up;
+    }
+    if (vl_slot) {
+        for (int b = 0; b < rc.B; ++b) sb->bit[rc.slots[b]] ^= 1;
+        sb->dirty = true;
     }
     if (T_out_final) *T_out_final = T;
     return 0;
@@ -1234,7 +1303,7 @@ void adec_destroy(adec_handle* h) {
         for (Op& op : *ops)
             for (int i = 0; i < 2; ++i) if (op.st[i]) cudaFree(op.st[i]);
     for (auto& b : h->ws) if (b.p) cudaFree(b.p);
-    for (DevBuf* b : {&h->hx, &h->hz, &h->hzq, &h->hy, &h->vl_tab}) if (b->p) cudaFree(b->p);
+    for (DevBuf* b : {&h->hx, &h->hz, &h->hzq, &h->hy, &h->vl_tab, &h->slot_tab}) if (b->p) cudaFree(b->p);
     if (h->hidx) cudaFree(h->hidx);
     if (h->d_err) cudaFree(h->d_err);
     if (h->d_ktrace) cudaFree(h->d_ktrace);
@@ -1269,6 +1338,8 @@ int adec_finalize(adec_handle* h) {
             if (alloc_state(h, &op, 1)) return 1;
         }
     h->n_streams = 1;
+    h->enc_slots.bit.assign(1, 0);
+    h->dec_slots.bit.assign(1, 0);
     h->tensors.clear();
     h->finalized = true;
     return 0;
@@ -1281,6 +1352,10 @@ int adec_n_streams(const adec_handle* h) { return h ? h->n_streams : 0; }
 // demand and the replaced ones are freed.
 static int resize_state(adec_handle* h, int n, bool replicate) {
     const int keep = std::min(n, h->n_streams);
+    // every call in flight, on whatever stream (torch side streams do not synchronise with stream 0), has finished before the state
+    // is touched; then every stream's latest state goes into st[cur]
+    CK(h, cudaDeviceSynchronize());
+    if (slot_fixup(h, h->enc_ops, 0) || slot_fixup(h, h->dec_ops, 0)) return 1;
     CK(h, cudaDeviceSynchronize());
     for (auto* ops : {&h->enc_ops, &h->dec_ops})
         for (Op& op : *ops) {
@@ -1308,6 +1383,8 @@ static int resize_state(adec_handle* h, int n, bool replicate) {
     CK(h, cudaDeviceSynchronize());
     h->st_cap = std::max(h->st_cap, n);
     h->n_streams = n;
+    h->enc_slots.bit.assign(n, 0);
+    h->dec_slots.bit.assign(n, 0);
     return 0;
 }
 
@@ -1335,6 +1412,10 @@ int adec_reset(adec_handle* h, void* stream) {
             if (!per) continue;
             for (int i = 0; i < 2; ++i) CK(h, cudaMemsetAsync(op.st[i], 0, per * h->n_streams * h->act_bytes(), (cudaStream_t)stream));
         }
+    for (SlotBits* sb : {&h->enc_slots, &h->dec_slots}) {     // both buffers are zero: every stream's state is in st[cur] again
+        std::fill(sb->bit.begin(), sb->bit.end(), 0);
+        sb->dirty = false;
+    }
     return 0;
 }
 
@@ -1365,12 +1446,27 @@ static int varlen_args(adec_handle* h, const char* name, const int* lengths, int
     return 0;
 }
 
-// decode / decode_offline / decode_offline_varlen in either activation dtype: the entry point's I/O dtype must be the handle's
-// (compute_dtype 2 = bf16).  vl: a varlen call, vl_frames the HOST frame counts of its B utterances (F unused).
+// the stream slots of a slot call: B distinct streams of the handle
+static int stream_args(adec_handle* h, const char* name, const int* streams, int B) {
+    if (!streams) return h->fail(fmt("%s: streams is NULL", name));
+    std::vector<char> seen(h->n_streams, 0);
+    for (int b = 0; b < B; ++b) {
+        const int s = streams[b];
+        if (s < 0 || s >= h->n_streams)
+            return h->fail(fmt("%s: stream %d (entry %d) is out of range [0, %d) (call adec_set_streams)", name, s, b, h->n_streams));
+        if (seen[s]) return h->fail(fmt("%s: stream %d is listed twice; each stream advances by one chunk per call", name, s));
+        seen[s] = 1;
+    }
+    return 0;
+}
+
+// decode / decode_offline / decode_offline_varlen / decode_streams in either activation dtype: the entry point's I/O dtype must be the
+// handle's (compute_dtype 2 = bf16).  vl: a varlen call, vl_frames the HOST frame counts of its B utterances (F unused); slots: a
+// streaming varlen call (adec_decode_streams), the HOST stream of each utterance.
 static int decode_common(adec_handle* h, const void* zq, int B, int F, void* y, void* stream, bool offline, bool bf16_io,
-                         bool vl = false, const int* vl_frames = nullptr) {
+                         bool vl = false, const int* vl_frames = nullptr, const int* slots = nullptr, bool slot_call = false) {
     if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    const char* base = vl ? "decode_offline_varlen" : offline ? "decode_offline" : "decode";
+    const char* base = slot_call ? "decode_streams" : vl ? "decode_offline_varlen" : offline ? "decode_offline" : "decode";
     const std::string name = std::string(base) + (bf16_io ? "_bf16" : "");
     if (h->act_bf16 && !bf16_io)
         return h->fail(fmt("%s: this handle has bf16 activations (compute_dtype 2); call adec_%s_bf16 with bf16 zq / y", name.c_str(), base));
@@ -1380,12 +1476,13 @@ static int decode_common(adec_handle* h, const void* zq, int B, int F, void* y, 
     if (bf16_io && (((uintptr_t)zq | (uintptr_t)y) & 15)) return h->fail(fmt("%s: zq and y must be 16-byte aligned", name.c_str()));
     if (vl) {
         if (varlen_args(h, name.c_str(), vl_frames, B)) return 1;
+        if (slot_call && stream_args(h, name.c_str(), slots, B)) return 1;
     } else if (B < 1 || F < 1) {
         return h->fail(fmt("%s: empty input", name.c_str()));
     }
     DeviceGuard dg(h->device);
     if (offline && !vl && offline_state(h, B, (cudaStream_t)stream)) return 1;
-    RunCtx rc{B, (const float*)zq, (float*)y, (cudaStream_t)stream, offline, vl ? vl_frames : nullptr, name.c_str()};
+    RunCtx rc{B, (const float*)zq, (float*)y, (cudaStream_t)stream, offline, vl ? vl_frames : nullptr, name.c_str(), slots};
     return run_ops(h, h->dec_ops, rc, vl ? 1 : F, nullptr);
 }
 
@@ -1430,6 +1527,47 @@ int adec_decode_offline_varlen(adec_handle* h, const float* zq, const int* frame
 
 int adec_decode_offline_varlen_bf16(adec_handle* h, const uint16_t* zq, const int* frames, int B, uint16_t* y, void* stream) {
     return decode_common(h, zq, B, 0, y, stream, true, true, true, frames);
+}
+
+// Stream slots: advance B distinct streams of the handle by one chunk each, every chunk with its own length, in one launch sequence.
+// The varlen row space with each utterance's history read from, and its new state written to, its stream's slot (ConvArgs::vl_slot).
+int adec_encode_streams(adec_handle* h, const float* x, const int* lengths, const int* streams, int B, float* z, void* stream) {
+    if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
+    if (h->cfg.model_type != ADEC_MODEL_SYMAD) return h->fail("encode_streams: not a symAD handle");
+    if (varlen_args(h, "encode_streams", lengths, B) || stream_args(h, "encode_streams", streams, B)) return 1;
+    DeviceGuard dg(h->device);
+    RunCtx rc{B, x, z, (cudaStream_t)stream, false, lengths, "encode_streams", streams};
+    return run_ops(h, h->enc_ops, rc, 1, nullptr);
+}
+
+int adec_decode_streams(adec_handle* h, const float* zq, const int* frames, const int* streams, int B, float* y, void* stream) {
+    return decode_common(h, zq, B, 0, y, stream, false, false, true, frames, streams, true);
+}
+
+int adec_decode_streams_bf16(adec_handle* h, const uint16_t* zq, const int* frames, const int* streams, int B, uint16_t* y, void* stream) {
+    return decode_common(h, zq, B, 0, y, stream, false, true, true, frames, streams, true);
+}
+
+int adec_copy_stream_state(adec_handle* h, int src, const int* dst, int n, void* stream) {
+    if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
+    if (src < 0 || src >= h->n_streams) return h->fail(fmt("copy_stream_state: src %d is out of range [0, %d)", src, h->n_streams));
+    if (n < 0 || (n > 0 && !dst)) return h->fail("copy_stream_state: bad dst list");
+    for (int i = 0; i < n; ++i)
+        if (dst[i] < 0 || dst[i] >= h->n_streams)
+            return h->fail(fmt("copy_stream_state: dst %d (entry %d) is out of range [0, %d)", dst[i], i, h->n_streams));
+    DeviceGuard dg(h->device);
+    for (auto* ops : {&h->enc_ops, &h->dec_ops}) {
+        SlotBits* sb = slot_bits(h, *ops);
+        const int sel = sb->bit[src];
+        std::vector<int> pairs;
+        for (int i = 0; i < n; ++i)
+            if (dst[i] != src) { pairs.push_back(src); pairs.push_back(dst[i]); }
+        // into the buffer src's state is in, which becomes the destination's current buffer
+        if (slot_copy(h, *ops, pairs, sel, sel, (cudaStream_t)stream)) return 1;
+        for (int i = 0; i < n; ++i) sb->bit[dst[i]] = (uint8_t)sel;
+        if (sel) sb->dirty = true;
+    }
+    return 0;
 }
 
 static int index_bits(int n) { int b = 1; while ((1 << b) < n) ++b; return b; }

@@ -215,7 +215,19 @@ struct ConvArgs {
     const int* vl_in;
     const int* vl_out;
     int vl_B;
+    // streaming varlen (stream slots): nullptr = offline (zero history, no state).  Otherwise utterance u is a chunk of stream slot
+    // vl_slot[u] >> 1: its history rows come from that slot's rows of buffer (vl_slot[u] & 1 ? st_out : st_in) and its new state goes
+    // to the same rows of the other buffer, so each slot keeps its own ping-pong phase and slots not in the call are not touched.
+    const int* vl_slot;
 };
+
+// stream slots: the state rows of utterance u's slot that the call reads (rd = true) or writes; base = st_in / st_out of the args
+template <typename T>
+__device__ __forceinline__ T* slot_rows(const int* vl_slot, int u, const T* st_in, const T* st_out, long long per_slot, bool rd) {
+    const int e = __ldg(vl_slot + u);
+    const T* base = ((e & 1) != 0) == rd ? st_out : st_in;
+    return const_cast<T*>(base) + (long long)(e >> 1) * per_slot;
+}
 
 // varlen row spaces: utterance u owns rows [off[u] + u * halo, off[u + 1] + (u + 1) * halo); off has B + 1 ascending entries
 __device__ __forceinline__ int vl_row(const int* off, int halo, int u) { return __ldg(off + u) + u * halo; }
@@ -471,9 +483,11 @@ struct StemArgs {
     const float* bias;                   // [COUT] or nullptr
     float* y; long long y_bs;
     const int* vl_off; int vl_B;         // VL: utterance u is rows [vl_off[u], vl_off[u + 1]) of x and y (B = 1, T = the total)
+    const int* vl_slot;                  // VL: stream slots (ConvArgs::vl_slot), or nullptr
 };
 
-// VL: one row space of concatenated utterances, each with a zero left pad; no state is read or written
+// VL: one row space of concatenated utterances, each with a zero left pad and no state written; with vl_slot, each with its slot's
+// history, and the slot's new state written by the block that holds the utterance's last row
 template <int COUT, int K, bool VL = false>
 __global__ void __launch_bounds__(256) stem_kernel(const StemArgs a) {
     constexpr int TT = 1024, P = K - 1, Q = COUT / 4;
@@ -505,12 +519,18 @@ __global__ void __launch_bounds__(256) stem_kernel(const StemArgs a) {
         if (j0 + t >= a.T) break;
         if (VL) while (j0 + t >= u_next) { ++u; u_start = u_next; u_next = __ldg(a.vl_off + u + 1); }
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-        for (int k = 0; k < K; ++k) {
-            const float xv = (!VL || j0 + t + k - P >= u_start) ? xw[t + k] : 0.f;   // taps before the utterance: its zero pad
+        auto tap = [&](int k, float xv) {
             const float4 w4 = *reinterpret_cast<const float4*>(sw + k * COUT + q * 4);
             acc.x = fmaf(xv, w4.x, acc.x); acc.y = fmaf(xv, w4.y, acc.y);
             acc.z = fmaf(xv, w4.z, acc.z); acc.w = fmaf(xv, w4.w, acc.w);
+        };
+        if (VL && a.vl_slot && j0 + t - u_start < P) {
+            // the first P rows of a stream-slot utterance: taps before it read the slot's history
+            const float* hs = slot_rows(a.vl_slot, u, a.st_in, a.st_out, P, true);
+            for (int k = 0; k < K; ++k) tap(k, j0 + t + k - P < u_start ? __ldg(hs + (j0 + t + k - u_start)) : xw[t + k]);
+        } else {
+#pragma unroll
+            for (int k = 0; k < K; ++k) tap(k, (!VL || j0 + t + k - P >= u_start) ? xw[t + k] : 0.f);   // taps before the utterance: its zero pad
         }
         const float4 b4 = *reinterpret_cast<const float4*>(sb + q * 4);
         acc.x += b4.x; acc.y += b4.y; acc.z += b4.z; acc.w += b4.w;
@@ -520,6 +540,19 @@ __global__ void __launch_bounds__(256) stem_kernel(const StemArgs a) {
         for (int r = tid; r < P; r += 256) {
             const long long i = (long long)a.T + r;
             a.st_out[b * P + r] = (i < P) ? a.st_in[b * P + i] : xg[i - P];
+        }
+    }
+    if (VL && a.vl_slot) {
+        // (utterance, state row) pairs of the utterances whose last row lies in this block: rows [T_u, T_u + P) of slot history || chunk
+        const int u_first = vl_find(a.vl_off, 0, a.vl_B, j0);
+        for (int idx = tid;; idx += 256) {
+            const int u = u_first + idx / P, r = idx % P;
+            if (u >= a.vl_B || __ldg(a.vl_off + u) >= j0 + TT) break;
+            const int s0 = __ldg(a.vl_off + u), s1 = __ldg(a.vl_off + u + 1);
+            if (s1 - 1 < j0 || s1 - 1 >= j0 + TT) continue;
+            const int i = s1 - s0 + r;
+            const float v = i < P ? __ldg(slot_rows(a.vl_slot, u, a.st_in, a.st_out, P, true) + i) : __ldg(xg + s0 + i - P);
+            slot_rows(a.vl_slot, u, a.st_in, a.st_out, P, false)[r] = v;
         }
     }
 }
@@ -535,6 +568,7 @@ struct HeadArgs {
     float bias; int pre_act; float slope; int post_tanh;
     float* y; long long y_bs;
     const int* vl_off; int vl_B;         // VL: utterance u is rows [vl_off[u], vl_off[u + 1]) of x and y (B = 1, T = the total)
+    const int* vl_slot;                  // VL: stream slots (ConvArgs::vl_slot), or nullptr
 };
 
 // Eight lanes share one run of R = 8 consecutive outputs: lane c4 owns channels 4*c4..4*c4+3, loads the R + K - 1 window rows of its
@@ -544,7 +578,8 @@ struct HeadArgs {
 // 128 B per output row and does 2*K*CIN flops on it: memory-bound once the LDS traffic of the round-1 version (112 LDS.128 per output)
 // is gone.  BST: bf16 input, state and output (the vocoder's bf16-activation mode); a chunk row enters the window as the bf16 value the
 // state keeps of it, so that a streamed chunk and a one-shot call see the same window.  VL: concatenated utterances, each with a zero
-// left pad (a run of eight outputs may span several of them, so each output masks the taps that fall before its utterance).
+// left pad (a run of eight outputs may span several of them, so each output masks the taps that fall before its utterance); with
+// vl_slot, those taps read the utterance's slot history instead, and the block holding its last row writes the slot's new state.
 template <int CIN, int K, bool BST, bool VL = false>
 __global__ void __launch_bounds__(256) head_kernel(const HeadArgs a) {
     static_assert(CIN == 32, "eight lanes x four channels");
@@ -581,7 +616,10 @@ __global__ void __launch_bounds__(256) head_kernel(const HeadArgs a) {
 #pragma unroll
             for (int k = 0; k < K; ++k) {
                 float4 x = xv[j + k];
-                if (VL && t0 + j + k - P < u_start) x = make_float4(0.f, 0.f, 0.f, 0.f);
+                if (VL && t0 + j + k - P < u_start)
+                    x = a.vl_slot ? ldg4(slot_rows(a.vl_slot, u, reinterpret_cast<const XT*>(a.st_in), reinterpret_cast<XT*>(a.st_out), P * CIN, true) +
+                                         (t0 + j + k - u_start) * CIN + 4 * c4)
+                                  : make_float4(0.f, 0.f, 0.f, 0.f);
                 acc[j] = fmaf(x.x, w[k].x, acc[j]); acc[j] = fmaf(x.y, w[k].y, acc[j]);
                 acc[j] = fmaf(x.z, w[k].z, acc[j]); acc[j] = fmaf(x.w, w[k].w, acc[j]);
             }
@@ -610,6 +648,24 @@ __global__ void __launch_bounds__(256) head_kernel(const HeadArgs a) {
             if (i < P) v = ld4(sg + i * CIN + ci);
             else v = apply_act(ldg4(xg + (i - P) * a.ldx + ci), a.pre_act, a.slope);
             st4(so + r * CIN + ci, v);
+        }
+    }
+    if (VL && a.vl_slot) {
+        // the slot state of every utterance whose last row lies in this block: rows [T_u, T_u + P) of slot history || chunk
+        const int r0 = blockIdx.x * TT;
+        for (int u = vl_find(a.vl_off, 0, a.vl_B, r0); u < a.vl_B && __ldg(a.vl_off + u) < r0 + TT; ++u) {
+            const int s0 = __ldg(a.vl_off + u), s1 = __ldg(a.vl_off + u + 1);
+            if (s1 - 1 < r0 || s1 - 1 >= r0 + TT) continue;
+            const XT* so_rd = slot_rows(a.vl_slot, u, reinterpret_cast<const XT*>(a.st_in), reinterpret_cast<XT*>(a.st_out), P * CIN, true);
+            XT* so_wr = slot_rows(a.vl_slot, u, reinterpret_cast<const XT*>(a.st_in), reinterpret_cast<XT*>(a.st_out), P * CIN, false);
+            for (int idx = tid; idx < P * (CIN / 4); idx += 256) {
+                const int r = idx / (CIN / 4), ci = (idx - r * (CIN / 4)) * 4;
+                const int i = s1 - s0 + r;
+                float4 v;
+                if (i < P) v = ldg4(so_rd + i * CIN + ci);
+                else v = apply_act(ldg4(xg + (long long)(s0 + i - P) * a.ldx + ci), a.pre_act, a.slope);
+                st4(so_wr + r * CIN + ci, v);
+            }
         }
     }
 }
@@ -882,6 +938,16 @@ __global__ void __launch_bounds__(256) unpack_kernel(const PackArgs a) {
         if (v >= a.N) { atomicOr(a.err, 1); v = 0; }
         a.idx[(long long)i * a.nfr + fr] = v + (long long)i * a.N;
     }
+}
+
+// per-stream state copies between stream slots (adec_copy_stream_state, and putting every stream back into the op's current buffer):
+// pair j copies the `per` words of stream pairs[2j] in src to stream pairs[2j + 1] in dst
+__global__ void slot_copy_kernel(float* dst, const float* src, long long per, const int* pairs, int n) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= per * n) return;
+    const int j = (int)(i / per);
+    const long long w = i - (long long)j * per;
+    dst[(long long)__ldg(pairs + 2 * j + 1) * per + w] = src[(long long)__ldg(pairs + 2 * j) * per + w];
 }
 
 // replicate stream 0's state to all streams (adec_set_streams)

@@ -241,9 +241,19 @@ __device__ __forceinline__ void wg_group(float (&d)[WgCfg<NT, PREC>::PW / 2], ui
     wg_fence_regs(d);
 }
 
+// stream slots: history row i (< P) of utterance u's slot, channel offset c within the row, in the buffer the slot is read from.  32-bit
+// element offsets (the host keeps a state buffer below 2^31 elements): the window loop has no registers to spare for 64-bit math.
+template <typename XT>
+__device__ __forceinline__ const XT* slot_hist(const ConvArgs& a, int u, int i, int c) {
+    const int e = __ldg(a.vl_slot + u);
+    const XT* base = reinterpret_cast<const XT*>((e & 1) ? (const void*)a.st_out : (const void*)a.st_in);
+    return base + (((e >> 1) * a.P + i) * a.st_ld + c);
+}
+
 // BST: activations, causal state, residual and output stored as bf16 in HBM (bf16 operands only; no 4-channel strided convs)
 // VL: utterances of different lengths in one stacked row space (ConvArgs::vl_in / vl_out), zero history, no state written; a separate
-// instantiation, so that the uniform kernels keep their code
+// instantiation, so that the uniform kernels keep their code.  With ConvArgs::vl_slot set (a runtime branch, not another instantiation)
+// each utterance is a chunk of one stream slot: history from the slot, new state written back to it.
 template <int NT, bool FUSE, int PRE, int PREC, bool BST, bool VL = false>
 __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(const ConvArgs a, int n_xtiles, int n_ytiles, int n_tiles) {
     static_assert(!BST || (PREC == PREC_BF16 && !FUSE), "bf16 storage is built for the non-fused bf16-operand kernels");
@@ -314,7 +324,7 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
         int wb = 0, wround = 0;                    // window piece counter wp = wround * n_wbuf + wb
         constexpr int RPP = NPROD / 4;             // window rows per pass (4 items of 8 channels per row)
         constexpr int UNR = 6;                     // rows in flight per thread (8 spilled up to 138 B and measured no faster)
-        constexpr int UNR_E = 6;
+        constexpr int UNR_E = VL ? 5 : 6;          // VL: the stream-slot history loads need the registers of one row
         const int c8 = pt & 3, m0 = pt >> 2;
         const size_t bstride = (size_t)wrp * 16;   // K-block pitch of a window plane
         const bool halves = a.RG > 1 && a.Cin < 8; // a 4-channel strided conv: the two halves of an item are different x~ rows
@@ -418,7 +428,10 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                                     long long ti = i - a.P;
                                     if (a.hist_rep && ti < 0) ti = 0;
                                     if (live) {
-                                        if (ti < 0) { if (!VL) ldg8(ss + i * a.st_ld + ci, u[k], v[k]); }   // VL: zero history
+                                        if (ti < 0) {       // VL: zero history, or the utterance's slot history
+                                            if (!VL) ldg8(ss + i * a.st_ld + ci, u[k], v[k]);
+                                            else if (a.vl_slot) ldg8(slot_hist<XT>(a, vu, (int)i, g * a.st_goff + ci), u[k], v[k]);
+                                        }
                                         else if (ti < (VL ? vu_T : a.T)) { ldg8(xs + ti * a.ldx + ci, u[k], v[k]); act |= 3u << (2 * k); }
                                     }
                                 } else {
@@ -431,7 +444,10 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                                         if (a.hist_rep && ti < 0) ti = 0;              // non-streaming transposed conv: replicate the first input row
                                         float4 w4 = make_float4(0.f, 0.f, 0.f, 0.f);
                                         if (live) {
-                                            if (ti < 0) { if (!VL) w4 = __ldg(reinterpret_cast<const float4*>(ss + i * a.st_ld + cc)); }
+                                            if (ti < 0) {
+                                                if (!VL) w4 = __ldg(reinterpret_cast<const float4*>(ss + i * a.st_ld + cc));
+                                                else if (a.vl_slot) w4 = ldg4(slot_hist<XT>(a, vu, (int)i, g * a.st_goff + cc));
+                                            }
                                             else if (ti < (VL ? vu_T : a.T)) { w4 = __ldg(reinterpret_cast<const float4*>(xs + ti * a.ldx + cc)); act |= 1u << (2 * k + hf); }
                                         }
                                         if (hf) v[k] = w4; else u[k] = w4;
@@ -487,6 +503,36 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                         }
                         st4(so + (long long)r * a.st_ld + cc, w4);
                     }
+                }
+            }
+        }
+        // ---- stream slots: every utterance's new state (rows [T_u, T_u + P) of slot history || chunk) goes to the slot's other buffer,
+        // which no CTA of this launch reads, so it is written after the tiles (the window loop keeps its registers), one (utterance,
+        // group) per CTA in turn
+        if (VL && a.vl_slot && a.P > 0) {
+            const long long per = (long long)a.P * a.st_ld;
+            const int nvec = a.P * (a.Cin / 4);
+            for (int w = blockIdx.x; w < a.vl_B * a.st_groups; w += gridDim.x) {
+                const int g = w / a.vl_B, u = w - g * a.vl_B;
+                const int i0 = __ldg(a.vl_in + u), Tu = __ldg(a.vl_in + u + 1) - i0;
+                const XT* xs = reinterpret_cast<const XT*>(a.x) + (long long)i0 * a.ldx + g * a.x_goff;
+                const XT* ss = slot_rows(a.vl_slot, u, reinterpret_cast<const XT*>(a.st_in) + g * a.st_goff,
+                                         reinterpret_cast<XT*>(a.st_out) + g * a.st_goff, per, true);
+                XT* so = slot_rows(a.vl_slot, u, reinterpret_cast<const XT*>(a.st_in) + g * a.st_goff,
+                                   reinterpret_cast<XT*>(a.st_out) + g * a.st_goff, per, false);
+                for (int idx = pt; idx < nvec; idx += NPROD) {
+                    const int r = idx / (a.Cin / 4);
+                    const int cc = (idx - r * (a.Cin / 4)) * 4;
+                    const long long i = (long long)Tu + r;
+                    float4 w4;
+                    if (i < a.P) {
+                        w4 = ldg4(ss + i * a.st_ld + cc);
+                    } else {
+                        w4 = ldg4(xs + (i - a.P) * a.ldx + cc);
+                        if (PRE == ACT_NORM) w4 = norm4(w4, a.mean + cc, a.scale + cc);
+                        else w4 = apply_act_t<PRE>(w4, a.slope);
+                    }
+                    st4(so + (long long)r * a.st_ld + cc, w4);
                 }
             }
         }

@@ -212,3 +212,147 @@ class MultiStreamCodecServer:
                                     if self.wire and st.size else None,
             "per_stream": per_stream,
         }
+
+
+class SessionCodecServer(MultiStreamCodecServer):
+    """Duplex streams that open and close while others run, each advanced only when it has audio.
+
+    The codec handles hold ``capacity`` stream slots plus one template slot (the last) with the warm state that
+    ``load_transmitter`` / ``load_receiver`` left in the objects; the template is never advanced.  ``open()`` copies the template
+    into a free slot, so a new caller starts exactly where a freshly warmed codec starts and inherits nothing of the slot's previous
+    caller.  ``step()`` runs ONE slot call per codec stage (``encode_streams`` -> quantize -> ``decode_streams``) over the open
+    streams that have a frame queued: idle streams are not fed silence, their causal state stays as it is, and a step costs what
+    its streams cost, not what the capacity costs.  ``submit`` / ``poll`` / the drop policy / ``start`` / ``stop`` are the lock-step
+    server's; the per-stream counters in ``statistics()`` are per slot.  The generators must hold ONE warmed stream when the server is
+    built (what load_transmitter / load_receiver leave), since only that stream is replicated into the slots.
+    """
+
+    def __init__(self, tx_encoder, rx_encoder, decoder, capacity: int, frame_size: int = 1500, sample_rate: int = 48000,
+                 max_latency: float = 0.1, device=None, wire: bool = False, clock=time.time):
+        super().__init__(tx_encoder, rx_encoder, decoder, capacity, frame_size=frame_size, sample_rate=sample_rate,
+                         max_latency=max_latency, device=device, wire=wire, clock=clock)
+        self.capacity = capacity
+        self.template = capacity                      # slot index of the warm template
+        self._stateful = [g for i, g in enumerate((tx_encoder, decoder)) if g not in (tx_encoder, decoder)[:i]]
+        for g in self._stateful:
+            if g.n_streams != 1:                      # growing from more than one stream adds zero-history slots: a cold template
+                raise ValueError(f"{type(g).__name__} holds {g.n_streams} streams; SessionCodecServer needs generators with the one "
+                                 "warmed stream that load_transmitter / load_receiver leave")
+        for g in self._stateful:
+            g.set_streams(capacity + 1)               # replicates the one warmed stream into every slot
+        self._free = list(range(capacity))
+        self._open: set = set()
+        self._session = [0] * capacity                # per slot: bumped by every open(), so a step hands out only its own session's frames
+        self._codec_lock = threading.Lock()           # the codec handles are driven by step() and open() from different threads
+
+    # ------------------------------------------------------------------ sessions
+    def open(self) -> int:
+        """Start a stream in a free slot, warm as the template; returns its id.  Raises RuntimeError when every slot is taken."""
+        with self._lock:
+            if not self._free:
+                raise RuntimeError(f"server is full: all {self.capacity} streams are open")
+            s = min(self._free)
+            self._free.remove(s)
+            self._session[s] += 1
+            self._in[s].clear()
+            self._out[s].clear()
+        with self._codec_lock:
+            for g in self._stateful:
+                g.copy_stream_state(self.template, [s])
+        with self._lock:
+            self._open.add(s)
+        return s
+
+    def close(self, stream: int) -> None:
+        """End stream `stream`: its slot becomes free and its queued input and output are dropped."""
+        with self._lock:
+            if stream not in self._open:
+                raise KeyError(f"stream {stream} is not open")
+            self._open.remove(stream)
+            self._in[stream].clear()
+            self._out[stream].clear()
+            self._free.append(stream)
+
+    @property
+    def open_streams(self) -> List[int]:
+        with self._lock:
+            return sorted(self._open)
+
+    def submit(self, stream: int, frame, t_capture: Optional[float] = None) -> None:
+        if stream not in self._open:
+            raise KeyError(f"stream {stream} is not open")
+        super().submit(stream, frame, t_capture)
+
+    # ------------------------------------------------------------------ one step over the streams that have audio
+    def step(self) -> int:
+        """Advance every open stream that has a frame queued by that frame.  Returns the number of streams advanced."""
+        t0 = self._clock()
+        dev = self.device if self.device is not None else torch.device("cpu")
+        x_host = self._staging(dev)
+        x_np = self._x_np
+        streams: List[int] = []
+        stamps: List[float] = []
+        sessions: List[int] = []
+        with self._lock:
+            for s in sorted(self._open):
+                q = self._in[s]
+                if q:
+                    f, t = q.popleft()
+                    x_np[len(streams), 0] = f
+                    streams.append(s)
+                    stamps.append(t)
+                    sessions.append(self._session[s])
+                else:
+                    self.stats[s].underruns += 1
+        n = len(streams)
+        if n == 0:
+            self.step_times.append(self._clock() - t0)
+            return 0
+        with torch.no_grad(), self._codec_lock:
+            x = x_host[:n].to(dev, non_blocking=True).view(n, -1)
+            z, frames = self.tx_encoder.encode_streams(list(x), streams)
+            if self.wire and hasattr(self.tx_encoder, "quantize_fused") and hasattr(self.rx_encoder, "lookup_packed"):
+                _, packed, _ = self.tx_encoder.quantize_fused(z, want_idx=False, want_packed=True, want_zq=False)
+                self.wire_bytes += packed.numel()
+                zq = self.rx_encoder.lookup_packed(packed)
+            elif self.wire:
+                packed = self.tx_encoder.pack(self.tx_encoder.quantize(z))
+                self.wire_bytes += packed.numel()
+                zq = self.rx_encoder.lookup(self.rx_encoder.unpack(packed))
+            else:
+                zq = self.rx_encoder.lookup(self.tx_encoder.quantize(z))
+            ys = self.decoder.decode_streams(zq, frames, streams)
+            y = torch.cat([v.reshape(1, -1) for v in ys]).detach()        # every chunk is frame_size samples: equal frame counts
+            if y.device.type == "cuda":
+                if self._y_host is None or self._y_host.shape != y.shape or self._y_host.dtype != y.dtype:
+                    self._y_host = torch.empty(y.shape, dtype=y.dtype, pin_memory=True)
+                self._y_host.copy_(y, non_blocking=True)
+                torch.cuda.current_stream(y.device).synchronize()
+                y_host = self._y_host
+            else:
+                y_host = y
+        now = self._clock()
+        if y_host.dtype == torch.bfloat16:
+            y_host = y_host.float()
+        y_all = y_host.numpy().reshape(n, -1)[:, :self.frame_size].copy()
+        with self._lock:
+            for k, s in enumerate(streams):
+                if s not in self._open or self._session[s] != sessions[k]:
+                    continue                        # closed (and maybe reopened by a new caller) while the step ran: the frame is dropped
+                st = self.stats[s]
+                self._out[s].append(y_all[k])
+                st.n_frames += 1
+                st.latencies.append(now - stamps[k])
+        self.step_times.append(now - t0)
+        return n
+
+    def statistics(self) -> Dict:
+        """The lock-step server's report, with `n_streams` = the streams open now, `capacity`, and the wire bitrate per second of
+        audio actually advanced (streams come and go, so neither the capacity nor the steps divide it)."""
+        out = super().statistics()
+        n_open = len(self.open_streams)
+        out["capacity"] = self.capacity
+        out["n_streams"] = out["open_streams"] = n_open
+        frames = out["frames"]
+        out["wire_kbps_per_stream"] = (8e-3 * self.wire_bytes) / (frames * self.frame_size / self.sample_rate) if self.wire and frames else None
+        return out

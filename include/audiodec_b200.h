@@ -139,6 +139,21 @@ int adec_decode_offline_varlen(adec_handle *h, const float *zq, const int *frame
 int adec_decode_offline_varlen_bf16(adec_handle *h, const uint16_t *zq, const int *frames, int B, uint16_t *y, void *stream);
 /* The varlen entry points need a tensor-core engine (f16 or tf32); the FFMA engine (ADEC_CONV_PATH=ffma) refuses them. */
 
+/* -- stream slots: advance any subset of the handle's streams, each by a chunk of its own length, in one launch sequence ---------- */
+/* Advance streams[b] (b < B, distinct, each in [0, n_streams)) by one chunk each: x = the chunks concatenated (sum T_b device
+ * floats), lengths HOST (>= 1).  z (code_dim, sum F_b), F_b = adec_frames_for(h, T_b): the B = 1 layout adec_quantize* / adec_lookup*
+ * already take.  Each stream gets exactly what a B = 1 streaming adec_encode of its chunk gives it.  Streams not listed keep their
+ * state untouched, and cost nothing.  Needs a tensor-core engine; every row count must fit in 31 bits. */
+int adec_encode_streams(adec_handle *h, const float *x, const int *lengths, const int *streams, int B, float *z, void *stream);
+/* zq (sum F_b, code_dim) channels-last, frames HOST (>= 1) -> y (sum F_b * hop), stream b at [hop * sum_{i<b} F_i, +hop * F_b). */
+int adec_decode_streams(adec_handle *h, const float *zq, const int *frames, const int *streams, int B, float *y, void *stream);
+/* adec_decode_streams for a compute_dtype 2 handle: bf16 zq and y, 16-byte aligned. */
+int adec_decode_streams_bf16(adec_handle *h, const uint16_t *zq, const int *frames, const int *streams, int B, uint16_t *y, void *stream);
+/* Copy stream src's current causal state (all layers of the handle) into each dst[i]: a joining stream starts warm. */
+int adec_copy_stream_state(adec_handle *h, int src, const int *dst, int n, void *stream);
+/* The uniform streaming calls, adec_set_streams and adec_reset see every stream's latest state after slot calls (a handle that made slot
+ * calls copies the streams whose state sits in the other ping-pong buffer back once, before its next uniform call or resize). */
+
 /* output frames of encode for T input samples: floor((T-1)/s)+1 applied per stride (conv_layer.py:153-156) */
 int adec_frames_for(const adec_handle *h, int T);
 /* product of the strides (utils/audiodec.py:58-62) */
