@@ -1807,60 +1807,80 @@ int adec_profile_report(adec_handle* h, char* buf, int buf_len) {
 // -------------------------------------------------------------------------------------------------
 // single-layer entry points for the unit tests (HOST pointers, reference layouts)
 // -------------------------------------------------------------------------------------------------
-static int run_single(adec_handle* h, Op& op, const float* x, int B, int Cin_real, int T, int groups, int Cout_real_total,
-                      float* state, int P_real, float* y, bool convtr, int stride) {
+// Elements are h->act_bytes() wide: fp32, or bf16 words for a compute_dtype 2 handle.  x (B, Cin_real, T) and state (B, Cin_real, P_real)
+// channels-first (Cin_real: the channels x holds, i.e. those of one group when the op has shared_in); res (B, Cout_real_total, Tout) or
+// nullptr, added after the bias from a workspace buffer as the model wires it.  offline: Generator.forward (zero history, first-row
+// replication in transposed convs); state is neither read nor written and may be nullptr.
+static int run_single(adec_handle* h, Op& op, const void* x, int B, int Cin_real, int T, int Cout_real_total, void* state, int P_real,
+                      void* y, bool convtr, int stride, const void* res = nullptr, bool offline = false) {
+    const size_t eb = h->act_bytes();
+    auto put = [eb](void* dst, size_t i, const void* src, size_t j) { memcpy((char*)dst + i * eb, (const char*)src + j * eb, eb); };
     // x (B, Cin_total, T) channels-first -> channels-last with per-group channel padding
     const int G = op.shared_in ? 1 : op.G;
     const int cin_g = Cin_real / G, ldx = G * op.Cin;
-    std::vector<float> xl((size_t)B * T * ldx, 0.f);
+    std::vector<char> xl((size_t)B * T * ldx * eb, 0);
     for (int b = 0; b < B; ++b)
         for (int g = 0; g < G; ++g)
             for (int c = 0; c < cin_g; ++c)
-                for (int t = 0; t < T; ++t) xl[((size_t)b * T + t) * ldx + g * op.Cin + c] = x[((size_t)b * Cin_real + g * cin_g + c) * T + t];
-    op.hstate.assign((size_t)B * op.P * op.st_C, 0.f);
-    for (int b = 0; b < B; ++b)
-        for (int g = 0; g < G; ++g)
-            for (int c = 0; c < cin_g; ++c)
-                for (int p = 0; p < P_real; ++p)
-                    op.hstate[((size_t)b * op.P + p) * op.st_C + g * op.Cin + c] = state[((size_t)b * Cin_real + g * cin_g + c) * P_real + p];
-    op.in_buf = BUF_EXT_IN; op.ldx = ldx; op.x_goff = op.Cin;
+                for (int t = 0; t < T; ++t) put(xl.data(), ((size_t)b * T + t) * ldx + g * op.Cin + c, x, ((size_t)b * Cin_real + g * cin_g + c) * T + t);
+    const size_t per = (size_t)op.P * op.st_C;
+    std::vector<char> hs(per * B * eb, 0);
+    if (!offline)
+        for (int b = 0; b < B; ++b)
+            for (int g = 0; g < G; ++g)
+                for (int c = 0; c < cin_g; ++c)
+                    for (int p = 0; p < P_real; ++p)
+                        put(hs.data(), ((size_t)b * op.P + p) * op.st_C + g * op.Cin + c, state, ((size_t)b * Cin_real + g * cin_g + c) * P_real + p);
+    op.in_buf = BUF_EXT_IN; op.ldx = ldx; op.x_goff = op.shared_in ? 0 : op.Cin;
     op.out_buf = BUF_EXT_OUT; op.ldy = op.G * op.Cout; op.y_goff = op.Cout;
     if (finalize_op(h, &op)) return 1;
-    const size_t per = (size_t)op.P * op.st_C;
-    for (int i = 0; i < 2; ++i) if (dev_alloc(h, &op.st[i], per * B)) return 1;
-    CK(h, cudaMemcpy(op.st[0], op.hstate.data(), per * B * sizeof(float), cudaMemcpyHostToDevice));
+    for (int i = 0; i < 2; ++i) if (dev_alloc(h, &op.st[i], (per * B * eb + 3) / 4)) return 1;
+    CK(h, cudaMemcpy(op.st[0], hs.data(), hs.size(), cudaMemcpyHostToDevice));
     h->n_streams = B;
     const int Tout = (T - 1) / op.down + 1;
-    float *dx, *dy;
-    if (dev_alloc(h, &dx, xl.size()) || dev_alloc(h, &dy, (size_t)B * Tout * op.ldy)) return 1;
-    CK(h, cudaMemcpy(dx, xl.data(), xl.size() * sizeof(float), cudaMemcpyHostToDevice));
-    std::vector<Op> ops;
-    ops.push_back(op);
-    RunCtx rc{B, dx, dy, 0};
-    if (run_ops(h, ops, rc, T, nullptr)) return 1;
-    CK(h, cudaDeviceSynchronize());
-    std::vector<float> yl((size_t)B * Tout * op.ldy), sl(per * B);
-    CK(h, cudaMemcpy(yl.data(), dy, yl.size() * sizeof(float), cudaMemcpyDeviceToHost));
-    CK(h, cudaMemcpy(sl.data(), ops[0].st[ops[0].cur], sl.size() * sizeof(float), cudaMemcpyDeviceToHost));
-    if (!convtr) {
-        const int cout_g = Cout_real_total / op.G;
+    const int cout_g = Cout_real_total / op.G;
+    if (res) {      // (B, Cout_total, Tout) -> channels-last in workspace 0, as the model's residual operand
+        std::vector<char> rl((size_t)B * Tout * op.ldy * eb, 0);
         for (int b = 0; b < B; ++b)
             for (int g = 0; g < op.G; ++g)
                 for (int c = 0; c < cout_g; ++c)
                     for (int t = 0; t < Tout; ++t)
-                        y[((size_t)b * Cout_real_total + g * cout_g + c) * Tout + t] = yl[((size_t)b * Tout + t) * op.ldy + g * op.Cout + c];
+                        put(rl.data(), ((size_t)b * Tout + t) * op.ldy + g * op.Cout + c, res, ((size_t)b * Cout_real_total + g * cout_g + c) * Tout + t);
+        if (ensure(h, h->ws[0], (rl.size() + 3) / 4)) return 1;
+        CK(h, cudaMemcpy(h->ws[0].p, rl.data(), rl.size(), cudaMemcpyHostToDevice));
+        op.res_buf = 0; op.ldr = op.ldy; op.r_goff = op.Cout;
+    }
+    float *dx, *dy;
+    const size_t ybytes = (size_t)B * Tout * op.ldy * eb;
+    if (dev_alloc(h, &dx, (xl.size() + 3) / 4) || dev_alloc(h, &dy, (ybytes + 3) / 4)) return 1;
+    CK(h, cudaMemcpy(dx, xl.data(), xl.size(), cudaMemcpyHostToDevice));
+    std::vector<Op> ops;
+    ops.push_back(op);
+    RunCtx rc{B, dx, dy, 0, offline};
+    if (run_ops(h, ops, rc, T, nullptr)) return 1;
+    CK(h, cudaDeviceSynchronize());
+    std::vector<char> yl(ybytes), sl(per * B * eb);
+    CK(h, cudaMemcpy(yl.data(), dy, yl.size(), cudaMemcpyDeviceToHost));
+    CK(h, cudaMemcpy(sl.data(), ops[0].st[ops[0].cur], sl.size(), cudaMemcpyDeviceToHost));
+    if (!convtr) {
+        for (int b = 0; b < B; ++b)
+            for (int g = 0; g < op.G; ++g)
+                for (int c = 0; c < cout_g; ++c)
+                    for (int t = 0; t < Tout; ++t)
+                        put(y, ((size_t)b * Cout_real_total + g * cout_g + c) * Tout + t, yl.data(), ((size_t)b * Tout + t) * op.ldy + g * op.Cout + c);
     } else {
         for (int b = 0; b < B; ++b)
             for (int c = 0; c < Cout_real_total; ++c)
                 for (int j = 0; j < Tout; ++j)
                     for (int r = 0; r < stride; ++r)
-                        y[((size_t)b * Cout_real_total + c) * Tout * stride + j * stride + r] = yl[((size_t)b * Tout + j) * op.ldy + r * Cout_real_total + c];
+                        put(y, ((size_t)b * Cout_real_total + c) * Tout * stride + j * stride + r, yl.data(), ((size_t)b * Tout + j) * op.ldy + r * Cout_real_total + c);
     }
-    for (int b = 0; b < B; ++b)
-        for (int g = 0; g < G; ++g)
-            for (int c = 0; c < cin_g; ++c)
-                for (int p = 0; p < P_real; ++p)
-                    state[((size_t)b * Cin_real + g * cin_g + c) * P_real + p] = sl[((size_t)b * op.P + p) * op.st_C + g * op.Cin + c];
+    if (!offline)
+        for (int b = 0; b < B; ++b)
+            for (int g = 0; g < G; ++g)
+                for (int c = 0; c < cin_g; ++c)
+                    for (int p = 0; p < P_real; ++p)
+                        put(state, ((size_t)b * Cin_real + g * cin_g + c) * P_real + p, sl.data(), ((size_t)b * op.P + p) * op.st_C + g * op.Cin + c);
     return 0;
 }
 
@@ -1876,7 +1896,7 @@ int adec_test_causal_conv(int device, const float* x, int B, int Cin, int T, con
     if (bias) { Bt.shape = {Cout}; Bt.data.assign(bias, bias + Cout); }
     Op op;
     int rc = make_conv_op(h, &op, "test_conv", W, bias ? &Bt : nullptr, stride, dil, groups, pre_act, slope, false);
-    if (!rc) rc = run_single(h, op, x, B, Cin, T, groups, Cout, state, (K - 1) * dil, y, false, 1);
+    if (!rc) rc = run_single(h, op, x, B, Cin, T, Cout, state, (K - 1) * dil, y, false, 1);
     if (rc) g_create_error = h->err;
     adec_destroy(h);
     return rc;
@@ -1896,7 +1916,7 @@ int adec_test_residual_unit(int device, const float* x, int B, int C, int T, con
     Op op;
     int rc = make_ru_op(h, &op, "test_ru", W1, W2, dil, ACT_ELU);
     if (!rc && h->use_tc && op.Cout > kTcMaxFuse) rc = h->fail("test_ru: C > 128 runs as two ops on the tensor-core path; test those separately");
-    if (!rc) rc = run_single(h, op, x, B, C, T, 1, C, state, (K - 1) * dil, y, false, 1);
+    if (!rc) rc = run_single(h, op, x, B, C, T, C, state, (K - 1) * dil, y, false, 1);
     if (rc) g_create_error = h->err;
     adec_destroy(h);
     return rc;
@@ -1914,7 +1934,71 @@ int adec_test_causal_convtr(int device, const float* x, int B, int Cin, int T, c
     if (bias) { Bt.shape = {Cout}; Bt.data.assign(bias, bias + Cout); }
     Op op;
     int rc = make_convtr_op(h, &op, "test_convtr", W, bias ? &Bt : nullptr, stride, ACT_NONE, 0.f);
-    if (!rc) rc = run_single(h, op, x, B, Cin, T, 1, Cout, state, 1, y, true, stride);
+    if (!rc) rc = run_single(h, op, x, B, Cin, T, Cout, state, 1, y, true, stride);
+    if (rc) g_create_error = h->err;
+    adec_destroy(h);
+    return rc;
+}
+
+// One vocoder layer as a compute_dtype 1 / 2 HiFi-GAN handle builds and runs it (the same op builders, packer and launch path as
+// build_hifigan / run_ops), so the tests can pin its rounding layer by layer.
+int adec_test_vocoder_layer(int device, int compute_dtype, int kind, const void* x, int B, int Cin, int T, const float* w,
+                            const float* bias, int Cout, int K, int dil, int up, int groups, int shared_in, int pre_act, float slope,
+                            const float* mean, const float* scale, const void* res, int offline, void* state, void* y) {
+    if (compute_dtype != 1 && compute_dtype != 2) {
+        g_create_error = "adec_test_vocoder_layer: compute_dtype must be 1 or 2 (the fp32-grade engines: adec_test_causal_conv / _convtr)";
+        return 1;
+    }
+    adec_config cfg{};
+    cfg.model_type = ADEC_MODEL_HIFIGAN;
+    cfg.compute_dtype = compute_dtype;
+    cfg.in_channels = Cin;
+    adec_handle* h = nullptr;
+    if (adec_create(&cfg, device, &h)) return 1;
+    DeviceGuard dg(device);
+    int rc = 0;
+    Op op;
+    if (!x || !w || !y || B < 1 || T < 1 || (!offline && !state)) {
+        rc = h->fail("adec_test_vocoder_layer: NULL x, w, y or (streaming) state, or B / T < 1");
+    } else if (kind == 0 && (groups < 1 || Cin % groups || Cout % groups)) {
+        rc = h->fail("adec_test_vocoder_layer: Cin and Cout must divide into groups");
+    } else if (kind == 0 && pre_act == ACT_NORM && (groups != 1 || !mean || !scale)) {
+        rc = h->fail("adec_test_vocoder_layer: norm needs groups = 1, mean and scale");
+    } else if (kind == 0) {
+        HostTensor W, Bt;
+        W.shape = {Cout, Cin / groups, K};
+        W.data.assign(w, w + (size_t)Cout * (Cin / groups) * K);
+        if (bias) { Bt.shape = {Cout}; Bt.data.assign(bias, bias + Cout); }
+        rc = make_conv_op(h, &op, "test_conv", W, bias ? &Bt : nullptr, 1, dil, groups, pre_act, slope, shared_in != 0);
+        if (!rc && pre_act == ACT_NORM) {      // padded like build_hifigan's stats
+            std::vector<float> mp(op.Cin, 0.f), sp(op.Cin, 1.f);
+            std::copy(mean, mean + Cin, mp.begin());
+            std::copy(scale, scale + Cin, sp.begin());
+            if (dev_upload(h, &h->d_mean, mp) || dev_upload(h, &h->d_scale, sp)) rc = 1;
+            op.mean = h->d_mean; op.scale = h->d_scale;
+        }
+        // shared_in: x and state hold the Cin / groups channels every group reads
+        if (!rc) rc = run_single(h, op, x, B, shared_in ? Cin / groups : Cin, T, Cout, state, (K - 1) * dil, y, false, 1, res, offline != 0);
+    } else if (res) {
+        rc = h->fail("adec_test_vocoder_layer: a residual is built for kind 0 only");
+    } else if (kind == 1) {
+        HostTensor W, Bt;
+        W.shape = {Cin, Cout, 2 * up};
+        W.data.assign(w, w + (size_t)Cin * Cout * 2 * up);
+        if (bias) { Bt.shape = {Cout}; Bt.data.assign(bias, bias + Cout); }
+        rc = make_convtr_op(h, &op, "test_convtr", W, bias ? &Bt : nullptr, up, ACT_LRELU, slope);
+        if (!rc) rc = run_single(h, op, x, B, Cin, T, Cout, state, 1, y, true, up, nullptr, offline != 0);
+    } else if (kind == 2) {
+        HostTensor W, Bt;      // through the state dict, as build_hifigan builds output_conv
+        W.shape = {Cout, Cin, K};
+        W.data.assign(w, w + (size_t)Cout * Cin * K);
+        h->tensors["test_head.conv.weight"] = W;
+        if (bias) { Bt.shape = {1}; Bt.data.assign(bias, bias + 1); h->tensors["test_head.conv.bias"] = Bt; }
+        rc = build_head(h, &op, "test_head", ACT_LRELU, slope, true);
+        if (!rc) rc = run_single(h, op, x, B, Cin, T, 1, state, op.P, y, false, 1, nullptr, offline != 0);
+    } else {
+        rc = h->fail("adec_test_vocoder_layer: kind must be 0 (conv), 1 (transposed conv) or 2 (head)");
+    }
     if (rc) g_create_error = h->err;
     adec_destroy(h);
     return rc;

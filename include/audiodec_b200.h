@@ -219,6 +219,21 @@ int adec_test_causal_convtr(int device, const float *x, int B, int Cin, int T, c
 int adec_test_residual_unit(int device, const float *x, int B, int C, int T, const float *w1, const float *w2,
                             int K, int dil, float *state, float *y);
 
+/* One HiFi-GAN layer as a compute_dtype 1 / 2 handle runs it.  HOST pointers, channels-first like the other test entry points;
+ * x, res, state and y are fp32 for compute_dtype 1 and bf16 words for 2.
+ * kind 0: causal conv, w (Cout, Cin/groups, K), dilation dil, `groups` groups; shared_in: every group reads the same Cin/groups
+ *         channels (MultiGroupConv1d's repeat, convs1.0), so x and state hold those Cin/groups channels; pre_act none /
+ *         LeakyReLU(slope) / norm ((x - mean) / scale, mean and scale (Cin), groups = 1), the kernels' ACT_* codes; res (B, Cout, T)
+ *         added after the bias, may be NULL.
+ * kind 1: causal transposed conv, w (Cin, Cout, 2*up), LeakyReLU(slope) pre-activation; y (B, Cout, T*up).
+ * kind 2: output head, w (1, 32, 7), LeakyReLU(slope) pre-activation, bias, tanh; y (B, 1, T).
+ * bias may be NULL.  offline != 0: zero history and first-row replication in transposed convs (Generator.forward); state is neither
+ * read nor written and may be NULL.  Otherwise state (B, Cin, P) is read and updated in place, as in adec_test_causal_conv. */
+int adec_test_vocoder_layer(int device, int compute_dtype, int kind, const void *x, int B, int Cin, int T,
+                            const float *w, const float *bias, int Cout, int K, int dil, int up, int groups, int shared_in,
+                            int pre_act, float slope, const float *mean, const float *scale, const void *res, int offline,
+                            void *state, void *y);
+
 #ifdef __cplusplus
 }
 #endif
