@@ -85,6 +85,7 @@ SYMBOLS = {
     "adec_test_causal_conv": (c_int, [c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                       c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     "adec_test_residual_unit": (c_int, [c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "adec_test_wgmma_columns": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "adec_test_causal_convtr": (c_int, [c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int,
                                         c_void_p, c_void_p]),
     "adec_test_vocoder_layer": (c_int, [c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,

@@ -96,12 +96,12 @@ const ConvKernelCfg* find_conv_kernel(int CW, int CO, bool fuse) {
 // (ADEC_CONV_PATH=tf32); PREC_BF16 = bf16 operands, one product (the vocoder's bf16 modes; BST = bf16 activations in HBM as well).
 // Persistent: one CTA per SM loops over (time tile, channel tile, stream) tiles.
 typedef cudaError_t (*TcPersistFn)(const ConvArgs&, int, int, int, int, int, cudaStream_t);
-template <int NT, bool F, int PRE, int PREC, bool BST, bool VL>
+template <int NT, bool F, int PRE, int PREC, bool BST, bool VL, bool PAIR = false>
 cudaError_t launch_wg(const ConvArgs& a, int n_xtiles, int n_ytiles, int n_tiles, int n_ctas, int smem_bytes, cudaStream_t s) {
     static bool configured[64] = {false};
     int dev = 0;
     cudaGetDevice(&dev);
-    auto kern = wg_conv_kernel<NT, F, PRE, PREC, BST, VL>;
+    auto kern = wg_conv_kernel<NT, F, PRE, PREC, BST, VL, PAIR>;
     constexpr int kMaxDyn = 227 * 1024;
     if (dev < 64 && !configured[dev]) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn);
@@ -125,13 +125,19 @@ cudaError_t launch_wg(const ConvArgs& a, int n_xtiles, int n_ytiles, int n_tiles
     cfg.numAttrs = pdl ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, kern, a, n_xtiles, n_ytiles, n_tiles);
 }
-typedef size_t (*TcSmemFn)(int, bool);
-typedef int (*TcWbufFn)(int, bool);
-// pfn_vl: the varlen instantiation (adec_*_offline_varlen)
-struct TcKernelCfg { int NT; bool fuse; int pre, prec; bool bst; int tap_bytes; TcPersistFn pfn, pfn_vl; TcSmemFn smem; TcWbufFn n_wbuf; };
+typedef size_t (*TcSmemFn)(int, bool, bool);
+typedef int (*TcWbufFn)(int, bool, bool);
+// the paired instantiation (two output rows per MMA row): built for the fused fp16-split RU(32) only
+template <int NT, bool F, int PRE, int PREC, bool BST>
+constexpr TcPersistFn pair_fn() {
+    if constexpr (NT == 32 && F && PREC == PREC_F16 && !BST) return launch_wg<NT, F, PRE, PREC, BST, false, true>;
+    else return nullptr;
+}
+// pfn_vl: the varlen instantiation (adec_*_offline_varlen); pfn_pair: the paired one, or nullptr
+struct TcKernelCfg { int NT; bool fuse; int pre, prec; bool bst; int tap_bytes; TcPersistFn pfn, pfn_vl, pfn_pair; TcSmemFn smem; TcWbufFn n_wbuf; };
 #define ADEC_TC1(NT, F, PRE, PREC, BST) \
     {NT, F, PRE, PREC, BST, WgCfg<NT, PREC>::TAP_BYTES, launch_wg<NT, F, PRE, PREC, BST, false>, launch_wg<NT, F, PRE, PREC, BST, true>, \
-     WgCfg<NT, PREC>::smem_bytes, WgCfg<NT, PREC>::n_wbuf}
+     pair_fn<NT, F, PRE, PREC, BST>(), WgCfg<NT, PREC>::smem_bytes, WgCfg<NT, PREC>::n_wbuf}
 #define ADEC_TC_FP32(NT, PREC) \
     ADEC_TC1(NT, true, ACT_ELU, PREC, false), ADEC_TC1(NT, false, ACT_NONE, PREC, false), ADEC_TC1(NT, false, ACT_ELU, PREC, false), \
     ADEC_TC1(NT, false, ACT_LRELU, PREC, false), ADEC_TC1(NT, false, ACT_NORM, PREC, false)
@@ -190,6 +196,7 @@ struct Op {
     int n_pieces = 1, n_co_tiles = 1;
     // device
     float *w = nullptr, *w2 = nullptr, *bias = nullptr;
+    float* w_pair = nullptr;   // the fused RU(32): paired taps [W_j | W_j-1] for the paired kernel (TcKernelCfg::pfn_pair)
     const float *mean = nullptr, *scale = nullptr;
     float head_bias = 0.f;
     long long w_tile_floats = 0;
@@ -513,19 +520,20 @@ int finalize_op_f16(adec_handle* h, Op* op) {
         }
         *p_out = p;
     };
-    auto pack = [&](const float* weff, int G, int ntiles, int pieces, int taps, int cin_eff, int cout, int p2, std::vector<float>* out) {
-        std::vector<uint16_t> img((size_t)G * ntiles * pieces * taps * tap_bytes / 2, 0);
+    // ntw: columns per tile (NT; 2 NT for the paired taps)
+    auto pack = [&](const float* weff, int G, int ntiles, int pieces, int taps, int cin_eff, int cout, int p2, int ntw, std::vector<float>* out) {
+        std::vector<uint16_t> img((size_t)G * ntiles * pieces * taps * npl * KB * ntw * 8, 0);
         size_t o = 0;     // in 16-bit units
         for (int g = 0; g < G; ++g)
             for (int nt = 0; nt < ntiles; ++nt)
                 for (int pc = 0; pc < pieces; ++pc)
                     for (int tap = 0; tap < taps; ++tap) {
                         for (int kb = 0; kb < KB; ++kb)
-                            for (int n = 0; n < NT; ++n)
+                            for (int n = 0; n < ntw; ++n)
                                 for (int e = 0; e < 8; ++e) {
                                     const int k = pc * CP + kb * 8 + e;
-                                    const float w = nt * NT + n < cout ? weff[(((size_t)g * taps + tap) * cin_eff + k) * cout + nt * NT + n] : 0.f;
-                                    const size_t at = o + ((size_t)kb * NT + n) * 8 + e, plane = (size_t)KB * NT * 8;
+                                    const float w = nt * ntw + n < cout ? weff[(((size_t)g * taps + tap) * cin_eff + k) * cout + nt * ntw + n] : 0.f;
+                                    const size_t at = o + ((size_t)kb * ntw + n) * 8 + e, plane = (size_t)KB * ntw * 8;
                                     if (prec == PREC_F16) {
                                         const float ws = std::ldexp(w, p2);
                                         const uint16_t hi = half_bits(ws);
@@ -536,7 +544,7 @@ int finalize_op_f16(adec_handle* h, Op* op) {
                                         img[at] = bf16_bits(w);
                                     }
                                 }
-                        o += (size_t)npl * KB * NT * 8;
+                        o += (size_t)npl * KB * ntw * 8;
                     }
         out->assign((img.size() + 1) / 2, 0.f);
         memcpy(out->data(), img.data(), img.size() * 2);
@@ -545,13 +553,29 @@ int finalize_op_f16(adec_handle* h, Op* op) {
     if (prec == PREC_F16) pow2_scale(op->weff, &p1);
     op->w_scale = std::ldexp(1.0f, -p1);
     std::vector<float> packed;
-    pack(op->weff.data(), op->G, op->n_co_tiles, op->n_pieces, op->Ktaps, op->Cin_eff, op->Cout, p1, &packed);
+    pack(op->weff.data(), op->G, op->n_co_tiles, op->n_pieces, op->Ktaps, op->Cin_eff, op->Cout, p1, NT, &packed);
     if (dev_upload(h, &op->w, packed)) return 1;
+    if (op->tc->pfn_pair && op->Ktaps % 2 == 1) {
+        // the paired kernel's K + 1 taps [W_j | W_j-1] (W_-1 = W_K = 0), 2 NT columns each, same scale; uniform rows run it, stacked
+        // and varlen rows the unpaired kernel with the same one-tap groups (WgCfg::tpg), so both give the same sums
+        const int C = op->Cout, Ci = op->Cin_eff, K = op->Ktaps;
+        std::vector<float> wp((size_t)(K + 1) * Ci * 2 * C, 0.f);
+        for (int j = 0; j <= K; ++j)
+            for (int ci = 0; ci < Ci; ++ci)
+                for (int co = 0; co < C; ++co) {
+                    float* row = wp.data() + ((size_t)j * Ci + ci) * 2 * C;
+                    if (j < K) row[co] = op->weff[((size_t)j * Ci + ci) * C + co];
+                    if (j > 0) row[C + co] = op->weff[((size_t)(j - 1) * Ci + ci) * C + co];
+                }
+        std::vector<float> pkp;
+        pack(wp.data(), 1, 1, op->n_pieces, K + 1, Ci, 2 * C, p1, 2 * NT, &pkp);
+        if (dev_upload(h, &op->w_pair, pkp)) return 1;
+    }
     if (op->fuse) {
         pow2_scale(op->weff2, &p2);
         op->w2_scale = std::ldexp(1.0f, -p2);
         std::vector<float> pk2;
-        pack(op->weff2.data(), 1, 1, op->Cout / CP, 1, op->Cout, op->Cout, p2, &pk2);
+        pack(op->weff2.data(), 1, 1, op->Cout / CP, 1, op->Cout, op->Cout, p2, NT, &pk2);
         if (dev_upload(h, &op->w2, pk2)) return 1;
     }
     if (!op->hbias.empty() && dev_upload(h, &op->bias, op->hbias)) return 1;
@@ -831,7 +855,7 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
             if (h->d_ktrace && h->ktrace_n < 4096) a.dbg = h->d_ktrace + 3 * (size_t)(h->ktrace_n++);
             if (op.tc) {
                 // persistent tensor-core kernels: one CTA per SM loops over (time tile, channel tile, stream) tiles
-                const int wrows = TC_TT + (op.Ktaps - 1) * op.dil;
+                int wrows = TC_TT + (op.Ktaps - 1) * op.dil;
                 dim3 grid((Tout + TC_TT - 1) / TC_TT, op.G * op.n_co_tiles, rc.B);
                 a.n_streams = rc.B;
                 if (vl) {
@@ -850,12 +874,19 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
                         grid = dim3((unsigned)stacked, grid.y, 1);
                     }
                 }
+                // uniform rows of the fused RU(32): the paired kernel, tiles of pair_tt(dil) rows, its window stored as two arrays
+                const bool pair = op.w_pair && !vl && !a.stack_L;
+                if (pair) {
+                    a.w = op.w_pair;
+                    wrows = 2 * pair_rows(op.Ktaps, op.dil);
+                    grid.x = (unsigned)((Tout + pair_tt(op.dil) - 1) / pair_tt(op.dil));
+                }
                 const long long n_tiles = (long long)grid.x * grid.y * grid.z;
                 const int n_ctas = (int)std::min<long long>(n_tiles, h->n_sms);
-                const size_t psmem = op.tc->smem(wrows, op.fuse);
-                a.n_wbuf = op.tc->n_wbuf(wrows, op.fuse);
+                const size_t psmem = op.tc->smem(wrows, op.fuse, pair);
+                a.n_wbuf = op.tc->n_wbuf(wrows, op.fuse, pair);
                 if (a.n_wbuf < 1) return h->fail(fmt("%s: window of %d rows does not fit in shared memory", op.name.c_str(), wrows));
-                e = (vl ? op.tc->pfn_vl : op.tc->pfn)(a, (int)grid.x, (int)grid.y, (int)n_tiles, n_ctas, (int)psmem, rc.stream);
+                e = (vl ? op.tc->pfn_vl : pair ? op.tc->pfn_pair : op.tc->pfn)(a, (int)grid.x, (int)grid.y, (int)n_tiles, n_ctas, (int)psmem, rc.stream);
             } else {
                 const int TT = op.kc->TT;
                 dim3 grid((Tout + TT - 1) / TT, op.G * op.n_co_tiles, rc.B);
@@ -1778,6 +1809,31 @@ int adec_probe_mma(int device, int kind, int NT, int n_groups, double* tflops, d
     const double flops = (double)n_sms * n_groups * 12.0 * 2.0 * 128.0 * NT * (kind == 0 ? 8.0 : 16.0);
     *tflops = flops / (t * 1e-3) / 1e12;
     if (ms) *ms = t;
+    return 0;
+}
+
+int adec_test_wgmma_columns(int device, const void* a, const void* b, float* d64, float* d32) {
+    if (!a || !b || !d64 || !d32) { g_create_error = "test_wgmma_columns: NULL argument"; return 1; }
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) { g_create_error = "test_wgmma_columns: no usable CUDA device"; return 1; }
+    DeviceGuard dg(device);
+    const size_t na = 2 * 4 * 64 * 16, nb = 3 * 4 * 64 * 16, nd = 64 * 64 * sizeof(float);
+    void* buf = nullptr;
+    cudaError_t e = cudaMalloc(&buf, na + nb + 2 * nd);
+    if (e == cudaSuccess) {
+        char* p = static_cast<char*>(buf);
+        e = cudaMemcpy(p, a, na, cudaMemcpyHostToDevice);
+        if (e == cudaSuccess) e = cudaMemcpy(p + na, b, nb, cudaMemcpyHostToDevice);
+        if (e == cudaSuccess) {
+            wgmma_cols_kernel<<<1, 128>>>(reinterpret_cast<const uint4*>(p), reinterpret_cast<const uint4*>(p + na),
+                                          reinterpret_cast<float*>(p + na + nb), reinterpret_cast<float*>(p + na + nb + nd));
+            e = cudaGetLastError();
+        }
+        if (e == cudaSuccess) e = cudaMemcpy(d64, p + na + nb, nd, cudaMemcpyDeviceToHost);
+        if (e == cudaSuccess) e = cudaMemcpy(d32, p + na + nb + nd, nd, cudaMemcpyDeviceToHost);
+        cudaFree(buf);
+    }
+    if (e != cudaSuccess) { g_create_error = fmt("test_wgmma_columns: %s", cudaGetErrorString(e)); return 1; }
     return 0;
 }
 

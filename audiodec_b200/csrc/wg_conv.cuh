@@ -104,28 +104,40 @@ template <int NT, int PREC> struct WgCfg {
     static constexpr int KBB = TC_CP * EB / 16;                    // 16-byte K blocks per 32-channel piece and plane
     static constexpr int NPR = PREC == PREC_F16 ? 3 : PREC == PREC_TF32 ? 2 : 1;   // weight planes per tap: hi | lo (| hi * 2^-11)
     static constexpr int NPL = PREC == PREC_BF16 ? 1 : 2;          // activation planes: hi | lo
-    static constexpr int TPG = PREC == PREC_TF32 ? 1 : 2;          // taps per group (= per weight stage)
+    // taps per group (= per weight stage).  The fused fp16-split unit at NT = 32 (RU(32)) takes one tap per group in every variant:
+    // its paired kernel (PAIR) can only group single taps, and an output's sum must not depend on which variant computed it.
+    __host__ __device__ static constexpr int tpg(bool fuse) { return PREC == PREC_TF32 || (PREC == PREC_F16 && NT == 32 && fuse) ? 1 : 2; }
     static constexpr int TAP_BYTES = NPR * KBB * NT * 16;          // one (piece, tap) of weights
-    static constexpr int STAGE_BYTES = TPG * TAP_BYTES;
-    static constexpr int MID_BYTES = NPL * (NT * EB / 16) * TC_MIDP * 16;   // the fused intermediate (all NT channels, 128 rows)
-    // weight stages: the fused tf32 unit at NT = 128 keeps a 128 KB intermediate, which leaves room for one stage and one window buffer
-    __host__ __device__ static constexpr int stages(bool fuse) { return PREC == PREC_TF32 && NT == 128 && fuse ? 1 : NT == 128 ? 2 : 3; }
+    __host__ __device__ static constexpr int stage_bytes(bool fuse) { return tpg(fuse) * TAP_BYTES; }
+    // the fused intermediate (all NT channels, 128 rows; PAIR: 256 rows, the two halves of the paired outputs)
+    __host__ __device__ static constexpr int mid_bytes(bool pair) { return NPL * (NT * EB / 16) * TC_MIDP * (pair ? 2 : 1) * 16; }
+    // weight stages: the fused tf32 unit at NT = 128 keeps a 128 KB intermediate, which leaves room for one stage and one window buffer.
+    // PAIR: 9, a whole tile's weights (8 paired taps and the 1x1) in flight; 3 stages measured 3 % slower per step on an H100.
+    __host__ __device__ static constexpr int stages(bool fuse, bool pair) { return pair ? 9 : PREC == PREC_TF32 && NT == 128 && fuse ? 1 : NT == 128 ? 2 : 3; }
+    // PAIR: a stage holds one paired tap [W_j | W_j-1], 2 NT columns
+    __host__ __device__ static constexpr int stage_alloc(bool fuse, bool pair) { return pair ? 2 * TAP_BYTES : stage_bytes(fuse); }
     static constexpr int PW = NT < 64 ? NT : 64;                   // columns per wgmma (partial width)
     // 384 threads: a multiple of 128 keeps ptxas' per-thread register budget at 168 (the consumers hold NT / 2 + PW / 2 accumulators)
     static constexpr int NPROD = 96;                               // activation-producer threads
     static constexpr int THREADS = 256 + NPROD + 32;
     __host__ __device__ static constexpr int win_pitch(int wrows) { return ((wrows + 1) & ~3) + 2; }   // rows, == 2 mod 4: conflict-free stores
     __host__ __device__ static constexpr int win_bytes(int wrows) { return NPL * KBB * win_pitch(wrows) * 16; }
-    // window buffers: as many as fit (1..4): the producers run that many pieces ahead of the MMAs
-    static int n_wbuf(int wrows, bool fuse) {
-        const long long avail = 227 * 1024 - 512 - (long long)stages(fuse) * STAGE_BYTES - (fuse ? (long long)MID_BYTES : 0);
+    // window buffers: as many as fit (1..4): the producers run that many pieces ahead of the MMAs.  wrows: stored window rows
+    static int n_wbuf(int wrows, bool fuse, bool pair) {
+        const long long avail = 227 * 1024 - 512 - (long long)stages(fuse, pair) * stage_alloc(fuse, pair) - (fuse ? (long long)mid_bytes(pair) : 0);
         const long long n = avail / win_bytes(wrows);
         return (int)(n > 4 ? 4 : n);
     }
-    static size_t smem_bytes(int wrows, bool fuse) {
-        return 512 + (size_t)stages(fuse) * STAGE_BYTES + (size_t)n_wbuf(wrows, fuse) * win_bytes(wrows) + (fuse ? (size_t)MID_BYTES : 0);
+    static size_t smem_bytes(int wrows, bool fuse, bool pair) {
+        return 512 + (size_t)stages(fuse, pair) * stage_alloc(fuse, pair) + (size_t)n_wbuf(wrows, fuse, pair) * win_bytes(wrows) +
+               (fuse ? (size_t)mid_bytes(pair) : 0);
     }
 };
+
+// PAIR (the fused RU(32), DESIGN §4.0): one MMA row computes the outputs t and t + dil of a tile of pair_tt(dil) rows, and the window is
+// stored de-interleaved by (row / dil) % 2 into an even and an odd array of pair_rows(K, dil) rows each
+__host__ __device__ constexpr int pair_tt(int dil) { return 2 * dil * (TC_TT / dil); }
+__host__ __device__ constexpr int pair_rows(int K, int dil) { return TC_TT + (K - 1) / 2 * dil; }
 
 template <int ACT>
 __device__ __forceinline__ float4 apply_act_t(float4 v, float slope) {
@@ -203,11 +215,11 @@ __device__ __forceinline__ float4 norm4(float4 x, const float* mean, const float
 
 // One group into a fresh partial: ntaps taps of one 32-channel piece, all three products (small terms first).  a_hi / a_lo: this
 // warpgroup's first row of the piece's planes, lbo: their K-block pitch; bw: the weight stage (plus the column-half offset).
-template <int NT, int PREC>
+template <int NT, int PREC, int TPG>
 __device__ __forceinline__ void wg_group(float (&d)[WgCfg<NT, PREC>::PW / 2], uint32_t a_hi, uint32_t a_lo, uint32_t lbo, uint32_t tap_step,
                                          int ntaps, uint32_t bw) {
     using Cfg = WgCfg<NT, PREC>;
-    constexpr int NKS = Cfg::KBB / 2, TPG = Cfg::TPG;
+    constexpr int NKS = Cfg::KBB / 2;
     constexpr uint32_t B_LBO = NT * 16u, B_KS = 2u * NT * 16u, B_T = Cfg::TAP_BYTES, B_PL = Cfg::KBB * NT * 16u;
     constexpr uint32_t PL_SMALL = PREC == PREC_F16 ? 2u : 0u;      // plane multiplied by A_lo: W_his (fp16) or W_hi (tf32)
     uint32_t acc = 0u;
@@ -254,17 +266,21 @@ __device__ __forceinline__ const XT* slot_hist(const ConvArgs& a, int u, int i, 
 // VL: utterances of different lengths in one stacked row space (ConvArgs::vl_in / vl_out), zero history, no state written; a separate
 // instantiation, so that the uniform kernels keep their code.  With ConvArgs::vl_slot set (a runtime branch, not another instantiation)
 // each utterance is a chunk of one stream slot: history from the slot, new state written back to it.
-template <int NT, bool FUSE, int PRE, int PREC, bool BST, bool VL = false>
+// PAIR: the fused RU(32) with two output rows per MMA row (m64n64 over K + 1 paired taps [W_j | W_j-1], DESIGN §4.0); uniform rows only
+// (no VL, no stacked rows), which the host guarantees.
+template <int NT, bool FUSE, int PRE, int PREC, bool BST, bool VL = false, bool PAIR = false>
 __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(const ConvArgs a, int n_xtiles, int n_ytiles, int n_tiles) {
     static_assert(!BST || (PREC == PREC_BF16 && !FUSE), "bf16 storage is built for the non-fused bf16-operand kernels");
+    static_assert(!PAIR || (NT == 32 && FUSE && PREC == PREC_F16 && !BST && !VL), "the paired kernel is built for the fused fp16-split RU(32)");
     using Cfg = WgCfg<NT, PREC>;
     using XT = typename std::conditional<BST, __nv_bfloat16, float>::type;
-    constexpr int S = Cfg::stages(FUSE), CP = TC_CP, TT = TC_TT, KBB = Cfg::KBB, EB = Cfg::EB, TPG = Cfg::TPG, PW = Cfg::PW;
+    constexpr int S = Cfg::stages(FUSE, PAIR), CP = TC_CP, TT = TC_TT, KBB = Cfg::KBB, EB = Cfg::EB, TPG = Cfg::tpg(FUSE), PW = Cfg::PW;
     constexpr int NPROD = Cfg::NPROD, WWARP = (256 + NPROD) / 32;         // weight producer warp
-    constexpr int STAGE_BYTES = Cfg::STAGE_BYTES, TAP_BYTES = Cfg::TAP_BYTES;
+    constexpr int STAGE_BYTES = Cfg::stage_alloc(FUSE, PAIR), TAP_BYTES = Cfg::TAP_BYTES;
     constexpr int NH = NT / PW;                                  // column halves per group
-    constexpr int NACC = NT / 2;                                 // accumulators per consumer thread (2 rows x NT / 4 columns)
+    constexpr int NACC = PAIR ? NT : NT / 2;                     // accumulators per consumer thread (2 rows x NT / 4 columns; PAIR: x 2)
     constexpr int MBLK = NT * EB / 16;                           // K blocks of the fused intermediate per plane
+    constexpr int MIDP = PAIR ? 2 * TC_MIDP : TC_MIDP;           // rows of the fused intermediate
 
     extern __shared__ __align__(128) unsigned char smem_raw[];
     uint64_t* b_full = reinterpret_cast<uint64_t*>(smem_raw);     // [S] weights landed
@@ -272,11 +288,22 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
     uint64_t* w_full = b_empty + S;                                // [4] window piece written
     uint64_t* w_empty = w_full + 4;                                // [4] window piece consumed (both consumer warpgroups)
     unsigned char* bst = smem_raw + 512;
-    const int wrows = TT + (a.Ktaps - 1) * a.dil;
-    const int wrp = Cfg::win_pitch(wrows);
-    const int win_b = Cfg::win_bytes(wrows);
+    const int ttile = PAIR ? pair_tt(a.dil) : TT;                  // output rows per tile
+    const int wrows = ttile + (a.Ktaps - 1) * a.dil;               // window rows (time)
+    const int prows = PAIR ? pair_rows(a.Ktaps, a.dil) : 0;        // PAIR: rows of the even array; the odd array follows it
+    const int wrp = Cfg::win_pitch(PAIR ? 2 * prows : wrows);
+    const int win_b = Cfg::win_bytes(PAIR ? 2 * prows : wrows);
     unsigned char* wbuf0 = bst + S * STAGE_BYTES;                  // a.n_wbuf window buffers of win_b bytes
-    unsigned char* mbuf = wbuf0 + (size_t)a.n_wbuf * win_b;        // FUSE only: [plane][MBLK][128 rows][16 B]
+    unsigned char* mbuf = wbuf0 + (size_t)a.n_wbuf * win_b;        // FUSE only: [plane][MBLK][MIDP rows][16 B]
+    // PAIR: window row m (time) -> its row in the de-interleaved storage
+    auto srow = [&](int m) -> int {
+        if constexpr (PAIR) {
+            const int blk = m / a.dil;
+            return (blk & 1) * prows + (blk >> 1) * a.dil + (m - blk * a.dil);
+        } else {
+            return m;
+        }
+    };
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
@@ -298,21 +325,22 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
         // ------------------------------------------------ weight producer: one bulk copy per group (TPG taps)
         if (lane == 0) {
             int c = 0;
-            auto stream = [&](const unsigned char* base, int pieces, int taps) {
+            auto stream = [&](const unsigned char* base, int pieces, int taps, int tap_bytes) {
                 for (int p = 0; p < pieces; ++p)
                     for (int t0 = 0; t0 < taps; t0 += TPG, ++c) {
                         const int s = c % S, it = c / S;
-                        const uint32_t bytes = (uint32_t)(taps - t0 >= TPG ? TPG : taps - t0) * TAP_BYTES;
+                        const uint32_t bytes = (uint32_t)(taps - t0 >= TPG ? TPG : taps - t0) * tap_bytes;
                         if (it > 0) mbar_wait(&b_empty[s], (it - 1) & 1, 100);
                         mbar_arrive_expect_tx(&b_full[s], bytes);
-                        bulk_g2s(bst + s * STAGE_BYTES, base + ((long long)p * taps + t0) * TAP_BYTES, bytes, &b_full[s]);
+                        bulk_g2s(bst + s * STAGE_BYTES, base + ((long long)p * taps + t0) * tap_bytes, bytes, &b_full[s]);
                     }
             };
             const unsigned char* w1 = reinterpret_cast<const unsigned char*>(a.w);
             const unsigned char* w2 = reinterpret_cast<const unsigned char*>(a.w2);
             for (TileIter it(blockIdx.x, gridDim.x, n_xtiles, n_ytiles); it.tile < n_tiles; it.next(gridDim.x)) {
-                stream(w1 + (long long)it.y * a.w_tile_floats * 4, a.n_pieces, a.Ktaps);
-                if (FUSE) stream(w2, NT / CP, 1);
+                // PAIR: K + 1 paired taps of 2 NT columns
+                stream(w1 + (long long)it.y * a.w_tile_floats * 4, a.n_pieces, PAIR ? a.Ktaps + 1 : a.Ktaps, PAIR ? 2 * TAP_BYTES : TAP_BYTES);
+                if (FUSE) stream(w2, NT / CP, 1, TAP_BYTES);
             }
         }
     } else if (warp >= 8) {
@@ -332,7 +360,7 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
             const int xt = it.xt, y = it.y, b = it.b;
             int g = 0, co_tile = y;
             if (a.n_co_tiles != n_ytiles) { g = y / a.n_co_tiles; co_tile = y - g * a.n_co_tiles; }
-            const int j0 = xt * TT;
+            const int j0 = xt * ttile;
             const XT* xg = reinterpret_cast<const XT*>(a.x) + (long long)b * a.x_bs + g * a.x_goff;
             const XT* sg = reinterpret_cast<const XT*>(a.st_in) + (long long)b * a.P * a.st_ld + g * a.st_goff;
             // VL: the utterance u0 that owns row j0, the first rows of it and of the next one, its input rows and length
@@ -382,7 +410,7 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
 #pragma unroll
                         for (int k = 0; k < UNR; ++k) {
                             const int m = mb + k * RPP;
-                            if (m < wrows) split_store<PREC>(hi + m * 16, lo + m * 16, bstride, apply_act_t<PRE>(u[k], a.slope), apply_act_t<PRE>(v[k], a.slope));
+                            if (m < wrows) split_store<PREC>(hi + srow(m) * 16, lo + srow(m) * 16, bstride, apply_act_t<PRE>(u[k], a.slope), apply_act_t<PRE>(v[k], a.slope));
                         }
                     }
                 } else {
@@ -463,7 +491,7 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                                 float4 x0 = u[k], x1 = v[k];
                                 if ((act >> (2 * k)) & 1u) x0 = PRE == ACT_NORM ? norm4(x0, a.mean + ci, a.scale + ci) : apply_act_t<PRE>(x0, a.slope);
                                 if ((act >> (2 * k)) & 2u) x1 = PRE == ACT_NORM ? norm4(x1, a.mean + ci2, a.scale + ci2) : apply_act_t<PRE>(x1, a.slope);
-                                split_store<PREC>(hi + m * 16, lo + m * 16, bstride, x0, x1);
+                                split_store<PREC>(hi + srow(m) * 16, lo + srow(m) * 16, bstride, x0, x1);
                             }
                         }
                     }
@@ -478,10 +506,10 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                     // streams whose last valid row sm * L + Tout - 1 lies in [j0, j0 + TT)
                     s_lo = (j0 - (a.Tout - 1) + a.stack_L - 1) / a.stack_L;
                     if (j0 < a.Tout - 1) s_lo = 0;
-                    s_hi = (j0 + TT - 1 - (a.Tout - 1)) / a.stack_L;
-                    if (j0 + TT - 1 < a.Tout - 1) s_hi = -1;
+                    s_hi = (j0 + ttile - 1 - (a.Tout - 1)) / a.stack_L;
+                    if (j0 + ttile - 1 < a.Tout - 1) s_hi = -1;
                     if (s_hi > a.n_streams - 1) s_hi = a.n_streams - 1;
-                } else if (xt == (a.Tout - 1) / TT) {
+                } else if (xt == (a.Tout - 1) / ttile) {
                     s_hi = b;
                 }
                 for (int sm = s_lo; sm <= s_hi; ++sm) {
@@ -543,12 +571,14 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
         const int wrow = 64 * wg + 16 * (warp & 3) + (lane >> 2), col2 = 2 * (lane & 3);
         const uint32_t row0_off = (uint32_t)(64 * wg) * 16u;            // this warpgroup's first operand row
         const uint32_t wbuf0_u = smem_u32(wbuf0), mbuf_u = smem_u32(mbuf), bst_u = smem_u32(bst);
-        const uint32_t lbo1 = (uint32_t)wrp * 16u, lbo2 = (uint32_t)TC_MIDP * 16u;
+        const uint32_t lbo1 = (uint32_t)wrp * 16u, lbo2 = (uint32_t)MIDP * 16u;
         const uint32_t tap_step = (uint32_t)a.dil * 16u;
+        constexpr int NPART = PAIR ? PW : PW / 2;           // PAIR: the conv's partial is m64n64
         float racc[NACC];
-        float part[PW / 2];
+        float part[NPART];
+        float (&part_h)[PW / 2] = *reinterpret_cast<float (*)[PW / 2]>(part);   // an NT-wide partial
 #pragma unroll
-        for (int i = 0; i < PW / 2; ++i) part[i] = 0.f;
+        for (int i = 0; i < NPART; ++i) part[i] = 0.f;
         int c = 0, wb = 0, wround = 0;
         float vmax = 0.f;                                   // largest magnitude this thread produced (fp16-split range check)
         // one group (weight stage c): partials per column half, round-to-nearest adds, stage released to the weight producer
@@ -558,19 +588,31 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
             const uint32_t bw = bst_u + (uint32_t)s * STAGE_BYTES;
 #pragma unroll
             for (int h = 0; h < NH; ++h) {
-                wg_group<NT, PREC>(part, a_hi + row_off, a_lo + row_off, lbo, tap_step, ntaps, bw + (uint32_t)h * PW * 16u);
+                wg_group<NT, PREC, TPG>(part_h, a_hi + row_off, a_lo + row_off, lbo, tap_step, ntaps, bw + (uint32_t)h * PW * 16u);
 #pragma unroll
-                for (int i = 0; i < PW / 2; ++i) racc[h * (PW / 2) + i] = __fadd_rn(racc[h * (PW / 2) + i], part[i]);
+                for (int i = 0; i < PW / 2; ++i) racc[h * (PW / 2) + i] = __fadd_rn(racc[h * (PW / 2) + i], part_h[i]);
             }
             if (threadIdx.x % 128 == 0) mbar_arrive(&b_empty[s]);
             ++c;
+        };
+        // PAIR: one paired tap [W_j | W_j-1] as one m64n64 group (columns 0..NT-1: output t, NT..2NT-1: output t + dil)
+        auto pgroup = [&](uint32_t a_hi, uint32_t a_lo, uint32_t row_off) {
+            if constexpr (PAIR) {
+                const int s = c % S;
+                mbar_wait(&b_full[s], (c / S) & 1, 300);
+                wg_group<2 * NT, PREC, 1>(part, a_hi + row_off, a_lo + row_off, lbo1, tap_step, 1, bst_u + (uint32_t)s * STAGE_BYTES);
+#pragma unroll
+                for (int i = 0; i < NACC; ++i) racc[i] = __fadd_rn(racc[i], part[i]);
+                if (threadIdx.x % 128 == 0) mbar_arrive(&b_empty[s]);
+                ++c;
+            }
         };
         // racc index of (half h, fragment register i) -> column h * PW + 8 * (i >> 2) + col2 + (i & 1), row wrow + 8 * ((i >> 1) & 1)
         for (TileIter it(blockIdx.x, gridDim.x, n_xtiles, n_ytiles); it.tile < n_tiles; it.next(gridDim.x)) {
             const int xt = it.xt, y = it.y, b = it.b;
             int g = 0, co_tile = y;
             if (a.n_co_tiles != n_ytiles) { g = y / a.n_co_tiles; co_tile = y - g * a.n_co_tiles; }
-            const int j0 = xt * TT;
+            const int j0 = xt * ttile;
 #pragma unroll
             for (int i = 0; i < NACC; ++i) racc[i] = 0.f;
             for (int p = 0; p < a.n_pieces; ++p) {
@@ -578,41 +620,71 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                 mbar_wait(&w_full[buf], wround & 1, 200);
                 if (++wb == a.n_wbuf) { wb = 0; ++wround; }
                 const uint32_t a_hi = wbuf0_u + (uint32_t)buf * (uint32_t)win_b;
-                for (int t0 = 0; t0 < a.Ktaps; t0 += TPG)
-                    group(a_hi, a_hi + (uint32_t)KBB * lbo1, lbo1, row0_off + (uint32_t)t0 * tap_step, a.Ktaps - t0 >= TPG ? TPG : a.Ktaps - t0);
+                if constexpr (PAIR) {
+                    // paired tap j reads window row t + j dil of the even-block rows t: the even array (j even) or the odd one, shifted
+                    for (int j = 0; j <= a.Ktaps; ++j)
+                        pgroup(a_hi, a_hi + (uint32_t)KBB * lbo1, row0_off + (uint32_t)((j & 1) * prows + (j >> 1) * a.dil) * 16u);
+                } else {
+                    for (int t0 = 0; t0 < a.Ktaps; t0 += TPG)
+                        group(a_hi, a_hi + (uint32_t)KBB * lbo1, lbo1, row0_off + (uint32_t)t0 * tap_step, a.Ktaps - t0 >= TPG ? TPG : a.Ktaps - t0);
+                }
                 if (threadIdx.x % 128 == 0) mbar_arrive(&w_empty[buf]);
             }
             if (FUSE) {
-                // weight scale out, activation, split into the 1x1 conv's A operand: this warpgroup's 64 rows of the intermediate
+                // weight scale out, activation, split into the 1x1 conv's A operand: this warpgroup's 64 rows of the intermediate (PAIR:
+                // its 64 MMA rows of each half, the half of output t + dil in rows TC_MIDP.. of the intermediate)
+                // PAIR: MMA rows from ttile / 2 on (dil 3, 9) read window rows past the tile, computed and dropped
+                const bool ok0 = !PAIR || wrow < ttile / 2, ok8 = !PAIR || wrow + 8 < ttile / 2;
 #pragma unroll
                 for (int i = 0; i < NACC; i += 4) {
                     const float4 m4 = apply_act_t<PRE>(make_float4(racc[i] * a.w_scale, racc[i + 1] * a.w_scale, racc[i + 2] * a.w_scale, racc[i + 3] * a.w_scale), a.slope);
                     racc[i] = m4.x; racc[i + 1] = m4.y; racc[i + 2] = m4.z; racc[i + 3] = m4.w;
-                    vmax = fmaxf(vmax, fmaxf(fmaxf(fabsf(m4.x), fabsf(m4.y)), fmaxf(fabsf(m4.z), fabsf(m4.w))));
+                    if (PAIR) {
+                        if (ok0) vmax = fmaxf(vmax, fmaxf(fabsf(m4.x), fabsf(m4.y)));
+                        if (ok8) vmax = fmaxf(vmax, fmaxf(fabsf(m4.z), fabsf(m4.w)));
+                    } else {
+                        vmax = fmaxf(vmax, fmaxf(fmaxf(fabsf(m4.x), fabsf(m4.y)), fmaxf(fabsf(m4.z), fabsf(m4.w))));
+                    }
                 }
 #pragma unroll
                 for (int i = 0; i < NACC; i += 2) {
-                    const int h = i / (PW / 2), fi = i % (PW / 2);
-                    const int co = h * PW + 8 * (fi >> 2) + col2, row = wrow + 8 * ((fi >> 1) & 1);
+                    const int h = PAIR ? 0 : i / (PW / 2), fi = PAIR ? i : i % (PW / 2);
+                    int co = h * PW + 8 * (fi >> 2) + col2, row = wrow + 8 * ((fi >> 1) & 1);
+                    if (PAIR) { row += (co / NT) * TC_MIDP; co %= NT; }
                     const int blk = co * EB / 16, off = (co * EB) & 15;
-                    unsigned char* hp = mbuf + ((size_t)blk * TC_MIDP + row) * 16 + off;
+                    unsigned char* hp = mbuf + ((size_t)blk * MIDP + row) * 16 + off;
                     uint2 hi, lo;
                     split2<PREC>(racc[i], racc[i + 1], hi, lo);
                     if (PREC == PREC_TF32) {
                         *reinterpret_cast<uint2*>(hp) = hi;
-                        *reinterpret_cast<uint2*>(hp + (size_t)MBLK * TC_MIDP * 16) = lo;
+                        *reinterpret_cast<uint2*>(hp + (size_t)MBLK * MIDP * 16) = lo;
                     } else {
                         *reinterpret_cast<uint32_t*>(hp) = hi.x;
-                        if (PREC == PREC_F16) *reinterpret_cast<uint32_t*>(hp + (size_t)MBLK * TC_MIDP * 16) = lo.x;
+                        if (PREC == PREC_F16) *reinterpret_cast<uint32_t*>(hp + (size_t)MBLK * MIDP * 16) = lo.x;
                     }
                 }
                 fence_async_smem();
                 named_bar_sync(1 + wg, 128);
 #pragma unroll
                 for (int i = 0; i < NACC; ++i) racc[i] = 0.f;
-                for (int p = 0; p < NT / CP; ++p) {
-                    const uint32_t m_hi = mbuf_u + (uint32_t)(p * KBB) * lbo2;
-                    group(m_hi, m_hi + (uint32_t)MBLK * lbo2, lbo2, row0_off, 1);
+                if constexpr (PAIR) {
+                    // the 1x1 conv as two NT-wide passes over the two halves, one weight stage: the unpaired kernel's MMAs, row for row
+                    const int s = c % S;
+                    mbar_wait(&b_full[s], (c / S) & 1, 300);
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh) {
+                        const uint32_t m_hi = mbuf_u + row0_off + (uint32_t)(hh * TC_MIDP * 16);
+                        wg_group<NT, PREC, 1>(part_h, m_hi, m_hi + (uint32_t)MBLK * lbo2, lbo2, tap_step, 1, bst_u + (uint32_t)s * STAGE_BYTES);
+#pragma unroll
+                        for (int i = 0; i < PW / 2; ++i) racc[hh * (PW / 2) + i] = __fadd_rn(racc[hh * (PW / 2) + i], part_h[i]);
+                    }
+                    if (threadIdx.x % 128 == 0) mbar_arrive(&b_empty[s]);
+                    ++c;
+                } else {
+                    for (int p = 0; p < NT / CP; ++p) {
+                        const uint32_t m_hi = mbuf_u + (uint32_t)(p * KBB) * lbo2;
+                        group(m_hi, m_hi + (uint32_t)MBLK * lbo2, lbo2, row0_off, 1);
+                    }
                 }
                 // every thread's 1x1 MMAs have completed (wgmma.wait_group) before the next tile rewrites its rows of the intermediate
             }
@@ -626,6 +698,38 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                 vu_start = vl_row(a.vl_out, halo, vu);
                 vu_next = vl_row(a.vl_out, halo, vu + 1);
             }
+            if constexpr (PAIR) {
+                // MMA row mr holds outputs t and t + dil (hp = 1); every residual is loaded before the first store, so the loads of
+                // all four (row, half) blocks are in flight together (one block at a time measured slower than the unpaired epilogue)
+                const float* rb = reinterpret_cast<const float*>(a.res) + (long long)b * a.res_bs;
+                float* yb = reinterpret_cast<float*>(a.y) + (long long)b * a.y_bs;
+                int trow[4];
+#pragma unroll
+                for (int rr = 0; rr < 4; ++rr) {
+                    const int mr = wrow + 8 * (rr & 1), blk = mr / a.dil;
+                    const int t = j0 + blk * 2 * a.dil + (mr - blk * a.dil) + (rr >> 1) * a.dil;
+                    trow[rr] = mr < ttile / 2 && t < a.Tout ? t : -1;
+                }
+                float2 r2[NACC / 2];
+#pragma unroll
+                for (int k = 0; k < NACC / 2; ++k) {        // k = 4 rr + column block; racc index 16 hp + 2 hr + 4 (k & 3)
+                    const int rr = k >> 2;
+                    r2[k] = trow[rr] >= 0 ? ldg2(rb + (long long)trow[rr] * a.ldr + 8 * (k & 3) + col2) : make_float2(0.f, 0.f);
+                }
+#pragma unroll
+                for (int k = 0; k < NACC / 2; ++k) {
+                    const int rr = k >> 2, i = (rr >> 1) * (PW / 2) + 2 * (rr & 1) + 4 * (k & 3), co = 8 * (k & 3) + col2;
+                    if (trow[rr] < 0) continue;
+                    float v0 = racc[i] * oscale, v1 = racc[i + 1] * oscale;
+                    if (a.bias) {
+                        const float2 b2 = __ldg(reinterpret_cast<const float2*>(a.bias + co));
+                        v0 += b2.x; v1 += b2.y;
+                    }
+                    v0 = r2[k].x + v0; v1 = r2[k].y + v1;
+                    vmax = fmaxf(vmax, fmaxf(fabsf(v0), fabsf(v1)));
+                    st2(yb + (long long)trow[rr] * a.ldy + co, v0, v1);
+                }
+            } else {
 #pragma unroll
             for (int hr = 0; hr < 2; ++hr) {
                 int bo = b, t = j0 + wrow + 8 * hr;
@@ -662,6 +766,7 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                         st2(reinterpret_cast<XT*>(a.y) + (long long)bo * a.y_bs + (long long)t * a.ldy + g * a.y_goff + co_l, v0, v1);
                     }
                 }
+            }
             }
         }
         // every activation is some launch's output: one check here bounds the operands of the next launch's fp16 split
@@ -712,6 +817,37 @@ __global__ void __launch_bounds__(256) mma_probe_kernel(int n_groups, int a_pitc
         }
     }
     if (sink != 0.f) g_probe_sink = sink;                   // operands are zeros: only keeps the result live
+}
+
+// wgmma_cols_kernel: one warpgroup runs the fp16-split group of one 32-channel tap (wg_group) as m64n64, and as m64n32 on each
+// 32-column half of the same weights.  The paired RU(32) kernel gives the same sums as the unpaired one only if the two agree column
+// for column, which NVIDIA does not document.  a: [plane 2][kb 4][64 rows][8 fp16], b: [plane 3][kb 4][64 columns][8 fp16];
+// d64 / d32: [64 rows][64 columns] fp32.
+__global__ void __launch_bounds__(128) wgmma_cols_kernel(const uint4* a, const uint4* b, float* d64, float* d32) {
+    __shared__ __align__(128) uint4 sa[2 * 4 * 64];
+    __shared__ __align__(128) uint4 sb[3 * 4 * 64];
+    __shared__ __align__(128) uint4 sh[2][3 * 4 * 32];      // the two column halves of sb as N = 32 images
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    for (int i = tid; i < 2 * 4 * 64; i += 128) sa[i] = a[i];
+    for (int i = tid; i < 3 * 4 * 64; i += 128) {
+        sb[i] = b[i];
+        sh[(i % 64) / 32][(i / 64) * 32 + i % 32] = b[i];
+    }
+    fence_async_smem();
+    __syncthreads();
+    const uint32_t au = smem_u32(sa), lbo = 64u * 16u;
+    float d[32], h[16];
+    wg_group<64, PREC_F16, 1>(d, au, au + 4u * lbo, lbo, 0u, 1, smem_u32(sb));
+    // fragment register i: row 16 warp + lane / 4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (lane & 3) + (i & 1)
+    const int r0 = 16 * warp + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) d64[(r0 + 8 * ((i >> 1) & 1)) * 64 + 8 * (i >> 2) + c0 + (i & 1)] = d[i];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+        wg_group<32, PREC_F16, 1>(h, au, au + 4u * lbo, lbo, 0u, 1, smem_u32(sh[hh]));
+#pragma unroll
+        for (int i = 0; i < 16; ++i) d32[(r0 + 8 * ((i >> 1) & 1)) * 64 + 32 * hh + 8 * (i >> 2) + c0 + (i & 1)] = h[i];
+    }
 }
 
 }  // namespace adec

@@ -219,6 +219,11 @@ int adec_test_causal_convtr(int device, const float *x, int B, int Cin, int T, c
 int adec_test_residual_unit(int device, const float *x, int B, int C, int T, const float *w1, const float *w2,
                             int K, int dil, float *state, float *y);
 
+/* The fp16-split MMA group of one 32-channel tap (three products, two K steps) as wgmma m64n64 and, on each 32-column half of the
+ * same weights, as m64n32.  a: 2 x 4 x 64 x 8 fp16 (activation hi | lo, K block, row), b: 3 x 4 x 64 x 8 fp16 (weight plane, K block,
+ * column); d64, d32: 64 x 64 fp32, row-major.  HOST pointers.  The paired RU(32) kernel relies on the two being equal bit for bit. */
+int adec_test_wgmma_columns(int device, const void *a, const void *b, float *d64, float *d32);
+
 /* One HiFi-GAN layer as a compute_dtype 1 / 2 handle runs it.  HOST pointers, channels-first like the other test entry points;
  * x, res, state and y are fp32 for compute_dtype 1 and bf16 words for 2.
  * kind 0: causal conv, w (Cout, Cin/groups, K), dilation dil, `groups` groups; shared_in: every group reads the same Cin/groups
