@@ -852,7 +852,7 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
             a.mid_act = op.mid_act;
             a.hist_rep = (rc.offline && op.up > 1) ? 1 : 0;
             a.w_scale = op.w_scale; a.w2_scale = op.w2_scale; a.err = h->d_err;
-            if (h->d_ktrace && h->ktrace_n < 4096) a.dbg = h->d_ktrace + 3 * (size_t)(h->ktrace_n++);
+            if (h->d_ktrace && h->ktrace_n < 4096) a.dbg = h->d_ktrace + KT_REC * (size_t)(h->ktrace_n++);
             if (op.tc) {
                 // persistent tensor-core kernels: one CTA per SM loops over (time tile, channel tile, stream) tiles
                 int wrows = TC_TT + (op.Ktaps - 1) * op.dil;
@@ -1294,7 +1294,11 @@ int adec_create(const adec_config* cfg, int device, adec_handle** out) {
     h->use_tc = h->engine != 0;
     if (const char* sr = getenv("ADEC_STACK_ROWS")) h->stack_rows = atoi(sr) != 0;
     if (const char* kt = getenv("ADEC_KTRACE")) {
-        if (atoi(kt)) { DeviceGuard dgk(device); cudaMalloc((void**)&h->d_ktrace, 4096 * 3 * sizeof(unsigned long long)); }
+        if (atoi(kt)) {
+            DeviceGuard dgk(device);
+            if (cudaMalloc((void**)&h->d_ktrace, 4096 * KT_REC * sizeof(unsigned long long)) == cudaSuccess)
+                cudaMemset(h->d_ktrace, 0, 4096 * KT_REC * sizeof(unsigned long long));    // the phase counters accumulate
+        }
     }
     h->bf16 = cfg->compute_dtype == 1 || cfg->compute_dtype == 2;
     h->act_bf16 = cfg->compute_dtype == 2;
@@ -1768,7 +1772,8 @@ int adec_ktrace(adec_handle* h, unsigned long long* out, int max_records) {
     if (!h || !h->d_ktrace || !out) return -1;
     DeviceGuard dg(h->device);
     const int n = std::min(h->ktrace_n, max_records);
-    if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(out, h->d_ktrace, (size_t)n * 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
+    if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(out, h->d_ktrace, (size_t)n * KT_REC * sizeof(unsigned long long), cudaMemcpyDeviceToHost) != cudaSuccess ||
+        cudaMemset(h->d_ktrace, 0, 4096 * KT_REC * sizeof(unsigned long long)) != cudaSuccess) return -1;
     h->ktrace_n = 0;
     return n;
 }

@@ -167,6 +167,19 @@ template <bool BST> __device__ __forceinline__ float4 stored4(float4 v) { return
 //     s*Cin channels, which turns them into 2-tap stride-1 convs (and keeps smem reads conflict-free);
 //   * transposed convs (k = 2s, crop [s:-s], conv_layer.py:197) are 2-tap convs with s*Cout outputs:
 //     y[j*s+r] = b + W[:,:,r]^T x[j] + W[:,:,s+r]^T x[j-1]; the (T, s*Cout) result *is* (T*s, Cout).
+// ADEC_PHASES (a diagnostic build, tools/conv_phases.py): wg_conv_kernel counts SM cycles per role and phase.  A ConvArgs::dbg record
+// is then {start ns, end ns, CTA 0 cycles, launch descriptor, Tout, PH_N, cycle sums [PH_N]}; the sums are over the CTAs of the
+// launch, from one thread per consumer warpgroup, activation-producer thread 0 and the weight-producer lane.
+enum { PH_WIN, PH_WGT, PH_MMA, PH_MID, PH_EPI,      // consumers: wait for a window piece, for a weight stage, MMA groups,
+                                                    //   fused intermediate, epilogue
+       PH_FREE, PH_LOAD, PH_CONV,                   // activation producers: wait for a free window buffer, global loads, convert
+       PH_WFREE, PH_WISSUE,                         // weight producer: wait for a free stage, everything else
+       PH_N };
+#ifdef ADEC_PHASES
+constexpr int KT_REC = 6 + PH_N;
+#else
+constexpr int KT_REC = 3;
+#endif
 struct ConvArgs {
     // input activations, channels-last; group g reads channels [g*x_goff, g*x_goff + Cin)
     const float* x;
@@ -207,7 +220,8 @@ struct ConvArgs {
     // the next stream and are computed but never stored.  0 = one row space per stream (blockIdx-style b dimension).
     int stack_L, n_streams;
     int* err;            // device flag word: bit 1 = an activation left the fp16-split range (|a| >= 6e4)
-    unsigned long long* dbg;   // ADEC_KTRACE: {globaltimer at start, at end, SM cycles} of CTA 0, one record per launch (nullptr = off)
+    unsigned long long* dbg;   // ADEC_KTRACE: {globaltimer at start, at end, SM cycles} of CTA 0, one record of KT_REC per launch
+                               // (nullptr = off); ADEC_PHASES builds append the phase cycle counters of wg_conv_kernel
     // varlen (the VL kernels): vl_B utterances of different lengths, concatenated along time in x, res and y.  Utterance u's input rows
     // are [vl_in[u], vl_in[u + 1]) and its output rows [vl_out[u], vl_out[u + 1]) (B + 1 entries each); in the tiles' row space it owns
     // the stacked rows [vl_row(u), vl_row(u + 1)), vl_row(u) = vl_out[u] + u * (Ktaps - 1) * dil, as stack_L does for equal lengths.

@@ -44,6 +44,18 @@ constexpr float F16_LO_SCALE = 2048.f; // 2^11
 enum { PREC_BF16 = 1, PREC_TF32 = 2, PREC_F16 = 3 };
 
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// ADEC_PHASES builds (kernels.cuh): ADEC_PH(k) adds the SM cycles since the previous mark of this thread to phase k.  The default build
+// compiles none of it.
+#ifdef ADEC_PHASES
+#define ADEC_PH_START() (ph_t = (uint32_t)clock())
+#define ADEC_PH(k) do { const uint32_t ph_now = (uint32_t)clock(); ph[k] += ph_now - ph_t; ph_t = ph_now; } while (0)
+#define ADEC_PH_USE(x) (ph_sink += __float_as_uint(x))   // waits for a load: the producers' load phase ends when the data is there
+#else
+#define ADEC_PH_USE(x) ((void)0)
+#define ADEC_PH_START() ((void)0)
+#define ADEC_PH(k) ((void)0)
+#endif
 __device__ __forceinline__ float tf32_rna(float x) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
@@ -310,6 +322,9 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
     unsigned long long kt0 = 0;
     long long kc0 = 0;
     if (a.dbg && blockIdx.x == 0 && tid == 0) { asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(kt0)); kc0 = clock64(); }
+#ifdef ADEC_PHASES
+    uint32_t ph[PH_N] = {}, ph_t = 0, ph_sink = 0;
+#endif
     if (tid == 0) {
         for (int s = 0; s < S; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 2); }
         for (int i = 0; i < 4; ++i) { mbar_init(&w_full[i], NPROD); mbar_init(&w_empty[i], 2); }
@@ -325,12 +340,15 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
         // ------------------------------------------------ weight producer: one bulk copy per group (TPG taps)
         if (lane == 0) {
             int c = 0;
+            ADEC_PH_START();
             auto stream = [&](const unsigned char* base, int pieces, int taps, int tap_bytes) {
                 for (int p = 0; p < pieces; ++p)
                     for (int t0 = 0; t0 < taps; t0 += TPG, ++c) {
                         const int s = c % S, it = c / S;
                         const uint32_t bytes = (uint32_t)(taps - t0 >= TPG ? TPG : taps - t0) * tap_bytes;
+                        ADEC_PH(PH_WISSUE);
                         if (it > 0) mbar_wait(&b_empty[s], (it - 1) & 1, 100);
+                        ADEC_PH(PH_WFREE);
                         mbar_arrive_expect_tx(&b_full[s], bytes);
                         bulk_g2s(bst + s * STAGE_BYTES, base + ((long long)p * taps + t0) * tap_bytes, bytes, &b_full[s]);
                     }
@@ -342,6 +360,7 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                 stream(w1 + (long long)it.y * a.w_tile_floats * 4, a.n_pieces, PAIR ? a.Ktaps + 1 : a.Ktaps, PAIR ? 2 * TAP_BYTES : TAP_BYTES);
                 if (FUSE) stream(w2, NT / CP, 1, TAP_BYTES);
             }
+            ADEC_PH(PH_WISSUE);
         }
     } else if (warp >= 8) {
         // ------------------------------------------------ activation producers: one item = 8 channels (32 B of fp32 / 16 B of bf16) of one
@@ -356,6 +375,7 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
         const int c8 = pt & 3, m0 = pt >> 2;
         const size_t bstride = (size_t)wrp * 16;   // K-block pitch of a window plane
         const bool halves = a.RG > 1 && a.Cin < 8; // a 4-channel strided conv: the two halves of an item are different x~ rows
+        ADEC_PH_START();
         for (TileIter it(blockIdx.x, gridDim.x, n_xtiles, n_ytiles); it.tile < n_tiles; it.next(gridDim.x)) {
             const int xt = it.xt, y = it.y, b = it.b;
             int g = 0, co_tile = y;
@@ -406,12 +426,19 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
 #pragma unroll
                         for (int k = 0; k < UNR; ++k)
                             if (mb + k * RPP < wrows) ldg8(xp + k * xstep, u[k], v[k]);
+                        ADEC_PH(PH_LOAD);
                         if (!waited) { mbar_wait(&w_empty[buf], wpar, 500); waited = true; }
+                        ADEC_PH(PH_FREE);
+#pragma unroll
+                        for (int k = 0; k < UNR; ++k)
+                            if (mb + k * RPP < wrows) { ADEC_PH_USE(u[k].x); ADEC_PH_USE(v[k].w); }
+                        ADEC_PH(PH_LOAD);
 #pragma unroll
                         for (int k = 0; k < UNR; ++k) {
                             const int m = mb + k * RPP;
                             if (m < wrows) split_store<PREC>(hi + srow(m) * 16, lo + srow(m) * 16, bstride, apply_act_t<PRE>(u[k], a.slope), apply_act_t<PRE>(v[k], a.slope));
                         }
+                        ADEC_PH(PH_CONV);
                     }
                 } else {
                     // edge piece: rows from the causal state (stored post-activation), the chunk, or beyond its end (zeros)
@@ -483,7 +510,13 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                                 }
                             }
                         }
+                        ADEC_PH(PH_LOAD);
                         if (!waited) { mbar_wait(&w_empty[buf], wpar, 500); waited = true; }
+                        ADEC_PH(PH_FREE);
+#pragma unroll
+                        for (int k = 0; k < UNR_E; ++k)
+                            if (mb + k * RPP < wrows) { ADEC_PH_USE(u[k].x); ADEC_PH_USE(v[k].w); }
+                        ADEC_PH(PH_LOAD);
 #pragma unroll
                         for (int k = 0; k < UNR_E; ++k) {
                             const int m = mb + k * RPP;
@@ -494,6 +527,7 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                                 split_store<PREC>(hi + srow(m) * 16, lo + srow(m) * 16, bstride, x0, x1);
                             }
                         }
+                        ADEC_PH(PH_CONV);
                     }
                 }
                 fence_async_smem();
@@ -577,14 +611,14 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
         float racc[NACC];
         float part[NPART];
         float (&part_h)[PW / 2] = *reinterpret_cast<float (*)[PW / 2]>(part);   // an NT-wide partial
-#pragma unroll
-        for (int i = 0; i < NPART; ++i) part[i] = 0.f;
         int c = 0, wb = 0, wround = 0;
         float vmax = 0.f;                                   // largest magnitude this thread produced (fp16-split range check)
+        ADEC_PH_START();
         // one group (weight stage c): partials per column half, round-to-nearest adds, stage released to the weight producer
         auto group = [&](uint32_t a_hi, uint32_t a_lo, uint32_t lbo, uint32_t row_off, int ntaps) {
             const int s = c % S;
             mbar_wait(&b_full[s], (c / S) & 1, 300);
+            ADEC_PH(PH_WGT);
             const uint32_t bw = bst_u + (uint32_t)s * STAGE_BYTES;
 #pragma unroll
             for (int h = 0; h < NH; ++h) {
@@ -592,6 +626,7 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
 #pragma unroll
                 for (int i = 0; i < PW / 2; ++i) racc[h * (PW / 2) + i] = __fadd_rn(racc[h * (PW / 2) + i], part_h[i]);
             }
+            ADEC_PH(PH_MMA);
             if (threadIdx.x % 128 == 0) mbar_arrive(&b_empty[s]);
             ++c;
         };
@@ -600,9 +635,11 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
             if constexpr (PAIR) {
                 const int s = c % S;
                 mbar_wait(&b_full[s], (c / S) & 1, 300);
+                ADEC_PH(PH_WGT);
                 wg_group<2 * NT, PREC, 1>(part, a_hi + row_off, a_lo + row_off, lbo1, tap_step, 1, bst_u + (uint32_t)s * STAGE_BYTES);
 #pragma unroll
                 for (int i = 0; i < NACC; ++i) racc[i] = __fadd_rn(racc[i], part[i]);
+                ADEC_PH(PH_MMA);
                 if (threadIdx.x % 128 == 0) mbar_arrive(&b_empty[s]);
                 ++c;
             }
@@ -615,9 +652,14 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
             const int j0 = xt * ttile;
 #pragma unroll
             for (int i = 0; i < NACC; ++i) racc[i] = 0.f;
+            // the first MMA of a group ignores the partial (scale-d = 0); zeroing it here rather than once leaves its registers free
+            // for the epilogue's loads
+#pragma unroll
+            for (int i = 0; i < NPART; ++i) part[i] = 0.f;
             for (int p = 0; p < a.n_pieces; ++p) {
                 const int buf = wb;
                 mbar_wait(&w_full[buf], wround & 1, 200);
+                ADEC_PH(PH_WIN);
                 if (++wb == a.n_wbuf) { wb = 0; ++wround; }
                 const uint32_t a_hi = wbuf0_u + (uint32_t)buf * (uint32_t)win_b;
                 if constexpr (PAIR) {
@@ -667,10 +709,12 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                 named_bar_sync(1 + wg, 128);
 #pragma unroll
                 for (int i = 0; i < NACC; ++i) racc[i] = 0.f;
+                ADEC_PH(PH_MID);
                 if constexpr (PAIR) {
                     // the 1x1 conv as two NT-wide passes over the two halves, one weight stage: the unpaired kernel's MMAs, row for row
                     const int s = c % S;
                     mbar_wait(&b_full[s], (c / S) & 1, 300);
+                    ADEC_PH(PH_WGT);
 #pragma unroll
                     for (int hh = 0; hh < 2; ++hh) {
                         const uint32_t m_hi = mbuf_u + row0_off + (uint32_t)(hh * TC_MIDP * 16);
@@ -680,6 +724,7 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                     }
                     if (threadIdx.x % 128 == 0) mbar_arrive(&b_empty[s]);
                     ++c;
+                    ADEC_PH(PH_MMA);
                 } else {
                     for (int p = 0; p < NT / CP; ++p) {
                         const uint32_t m_hi = mbuf_u + (uint32_t)(p * KBB) * lbo2;
@@ -688,90 +733,116 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                 }
                 // every thread's 1x1 MMAs have completed (wgmma.wait_group) before the next tile rewrites its rows of the intermediate
             }
-            // ---- epilogue: rows wrow and wrow + 8 of the tile, column pairs of this thread's fragment
+            // ---- epilogue: this thread's output rows (NR: wrow and wrow + 8; PAIR: those MMA rows of the outputs t and t + dil) x
+            // column pairs co_tile * NT + 8 k + col2 (k < NCB), racc index 4 k + 2 (rr & 1) + (PW / 2) (rr >> 1).  The stores may alias
+            // the loads for all the compiler knows, so it keeps every load after the stores before it; the epilogue therefore runs in
+            // batches of KB column blocks over all NR rows, each issuing its bias and residual loads before its first store: one round
+            // trip per batch instead of one per column pair (DESIGN §4.0).
+            // Each output is round(round(round(racc * oscale) + bias) + residual), three separately rounded operations, never an FMA.
+            constexpr int PB = NT < 128 ? 16 : (PREC == PREC_TF32 && FUSE) || VL ? 4 : 8;   // residual pairs per batch: larger ones spill
+            constexpr int NR = PAIR ? 4 : 2, NCB = NACC / (2 * NR), KB = NCB < PB / NR ? NCB : PB / NR;
             const float oscale = FUSE ? a.w2_scale : a.w_scale;
-            // VL: the utterance of row j0 + wrow (then of row + 8) and where its stacked rows start and end
-            int vu = 0, vu_start = 0, vu_next = 0;
-            const int halo = (a.Ktaps - 1) * a.dil;
-            if constexpr (VL) {
-                vu = vl_find(a.vl_out, halo, a.vl_B, j0 + wrow);
-                vu_start = vl_row(a.vl_out, halo, vu);
-                vu_next = vl_row(a.vl_out, halo, vu + 1);
-            }
-            if constexpr (PAIR) {
-                // MMA row mr holds outputs t and t + dil (hp = 1); every residual is loaded before the first store, so the loads of
-                // all four (row, half) blocks are in flight together (one block at a time measured slower than the unpaired epilogue)
-                const float* rb = reinterpret_cast<const float*>(a.res) + (long long)b * a.res_bs;
-                float* yb = reinterpret_cast<float*>(a.y) + (long long)b * a.y_bs;
-                int trow[4];
-#pragma unroll
-                for (int rr = 0; rr < 4; ++rr) {
-                    const int mr = wrow + 8 * (rr & 1), blk = mr / a.dil;
-                    const int t = j0 + blk * 2 * a.dil + (mr - blk * a.dil) + (rr >> 1) * a.dil;
-                    trow[rr] = mr < ttile / 2 && t < a.Tout ? t : -1;
-                }
-                float2 r2[NACC / 2];
-#pragma unroll
-                for (int k = 0; k < NACC / 2; ++k) {        // k = 4 rr + column block; racc index 16 hp + 2 hr + 4 (k & 3)
-                    const int rr = k >> 2;
-                    r2[k] = trow[rr] >= 0 ? ldg2(rb + (long long)trow[rr] * a.ldr + 8 * (k & 3) + col2) : make_float2(0.f, 0.f);
-                }
-#pragma unroll
-                for (int k = 0; k < NACC / 2; ++k) {
-                    const int rr = k >> 2, i = (rr >> 1) * (PW / 2) + 2 * (rr & 1) + 4 * (k & 3), co = 8 * (k & 3) + col2;
-                    if (trow[rr] < 0) continue;
-                    float v0 = racc[i] * oscale, v1 = racc[i + 1] * oscale;
-                    if (a.bias) {
-                        const float2 b2 = __ldg(reinterpret_cast<const float2*>(a.bias + co));
-                        v0 += b2.x; v1 += b2.y;
-                    }
-                    v0 = r2[k].x + v0; v1 = r2[k].y + v1;
-                    vmax = fmaxf(vmax, fmaxf(fabsf(v0), fabsf(v1)));
-                    st2(yb + (long long)trow[rr] * a.ldy + co, v0, v1);
-                }
-            } else {
-#pragma unroll
-            for (int hr = 0; hr < 2; ++hr) {
-                int bo = b, t = j0 + wrow + 8 * hr;
+            const int co0 = co_tile * NT + col2;     // columns from Cout_g on: the zero-padded part of a channel tile (96 outputs of 128)
+            int rt[NR], rbo[NR];                     // output row and stream of row rr, rt = -1: not stored
+            {
+                // VL: the utterance of row j0 + wrow (then of row + 8) and where its stacked rows start and end
+                const int halo = (a.Ktaps - 1) * a.dil;
+                int vu = 0, vu_start = 0, vu_next = 0;
                 if constexpr (VL) {
-                    // local row t - vu_start of the utterance; rows past its Tout are the receptive-field overlap, computed and dropped
-                    while (vu + 1 < a.vl_B && t >= vu_next) { ++vu; vu_start = vu_next; vu_next = vl_row(a.vl_out, halo, vu + 1); }
-                    const int o0 = __ldg(a.vl_out + vu), ml = t - vu_start;
-                    if (ml >= __ldg(a.vl_out + vu + 1) - o0) continue;
-                    t = o0 + ml;
-                } else {
-                    if (a.stack_L) { bo = t / a.stack_L; t -= bo * a.stack_L; }
-                    if (!(t < a.Tout && bo < a.n_streams)) continue;
+                    vu = vl_find(a.vl_out, halo, a.vl_B, j0 + wrow);
+                    vu_start = vl_row(a.vl_out, halo, vu);
+                    vu_next = vl_row(a.vl_out, halo, vu + 1);
                 }
 #pragma unroll
-                for (int i = 2 * hr; i < NACC; i += 4) {
-                    const int h = i / (PW / 2), fi = i % (PW / 2);
-                    const int co_l = co_tile * NT + h * PW + 8 * (fi >> 2) + col2;
-                    if (co_l >= a.Cout_g) continue;                // zero-padded part of a channel tile (e.g. 96 outputs in a 128-wide tile)
-                    float v0 = racc[i] * oscale, v1 = racc[i + 1] * oscale;
-                    if (a.bias) {
-                        const float2 b2 = __ldg(reinterpret_cast<const float2*>(a.bias + g * a.Cout_g + co_l));
-                        v0 += b2.x; v1 += b2.y;
-                    }
-                    if (a.res) {
-                        const float2 r2 = ldg2(reinterpret_cast<const XT*>(a.res) + (long long)bo * a.res_bs + (long long)t * a.ldr + g * a.r_goff + co_l);
-                        v0 = r2.x + v0; v1 = r2.y + v1;
-                    }
-                    vmax = fmaxf(vmax, fmaxf(fabsf(v0), fabsf(v1)));
-                    if (a.out_nct) {
-                        XT* yp = reinterpret_cast<XT*>(a.y) + (long long)bo * a.y_bs + (long long)(g * a.y_goff + co_l) * a.Tout + t;
-                        st1(yp, v0);
-                        st1(yp + a.Tout, v1);
+                for (int rr = 0; rr < NR; ++rr) {
+                    int bo = b, t = j0 + wrow + 8 * rr;
+                    bool ok;
+                    if constexpr (PAIR) {
+                        // MMA row mr holds outputs t and t + dil (rr >> 1 = 1)
+                        const int mr = wrow + 8 * (rr & 1), blk = mr / a.dil;
+                        t = j0 + blk * 2 * a.dil + (mr - blk * a.dil) + (rr >> 1) * a.dil;
+                        ok = mr < ttile / 2 && t < a.Tout;
+                    } else if constexpr (VL) {
+                        // local row t - vu_start of the utterance; rows past its Tout are the receptive-field overlap, computed and dropped
+                        while (vu + 1 < a.vl_B && t >= vu_next) { ++vu; vu_start = vu_next; vu_next = vl_row(a.vl_out, halo, vu + 1); }
+                        const int o0 = __ldg(a.vl_out + vu), ml = t - vu_start;
+                        ok = ml < __ldg(a.vl_out + vu + 1) - o0;
+                        t = o0 + ml;
                     } else {
-                        st2(reinterpret_cast<XT*>(a.y) + (long long)bo * a.y_bs + (long long)t * a.ldy + g * a.y_goff + co_l, v0, v1);
+                        if (a.stack_L) { bo = t / a.stack_L; t -= bo * a.stack_L; }
+                        ok = t < a.Tout && bo < a.n_streams;
+                    }
+                    rt[rr] = ok ? t : -1;
+                    rbo[rr] = bo;
+                }
+            }
+#pragma unroll
+            for (int k0 = 0; k0 < NCB; k0 += KB) {
+                float2 bb[KB], r2[NR][KB];
+                if (a.bias) {
+#pragma unroll
+                    for (int k = 0; k < KB; ++k) {
+                        const int co_l = co0 + 8 * (k0 + k);
+                        bb[k] = co_l < a.Cout_g ? __ldg(reinterpret_cast<const float2*>(a.bias + g * a.Cout_g + co_l)) : make_float2(0.f, 0.f);
+                    }
+                }
+                if (a.res) {
+#pragma unroll
+                    for (int rr = 0; rr < NR; ++rr)
+#pragma unroll
+                        for (int k = 0; k < KB; ++k) {
+                            const int t = rt[rr], co_l = co0 + 8 * (k0 + k);
+                            r2[rr][k] = t >= 0 && co_l < a.Cout_g
+                                            ? ldg2(reinterpret_cast<const XT*>(a.res) + (long long)rbo[rr] * a.res_bs + (long long)t * a.ldr + g * a.r_goff + co_l)
+                                            : make_float2(0.f, 0.f);
+                        }
+                }
+#pragma unroll
+                for (int rr = 0; rr < NR; ++rr) {
+                    const int t = rt[rr], bo = rbo[rr];
+                    if (t < 0) continue;
+#pragma unroll
+                    for (int k = 0; k < KB; ++k) {
+                        const int co_l = co0 + 8 * (k0 + k), i = 4 * (k0 + k) + 2 * (rr & 1) + (PW / 2) * (rr >> 1);
+                        if (co_l >= a.Cout_g) continue;
+                        float v0 = __fmul_rn(racc[i], oscale), v1 = __fmul_rn(racc[i + 1], oscale);
+                        if (a.bias) { v0 = __fadd_rn(v0, bb[k].x); v1 = __fadd_rn(v1, bb[k].y); }
+                        if (a.res) { v0 = __fadd_rn(r2[rr][k].x, v0); v1 = __fadd_rn(r2[rr][k].y, v1); }
+                        vmax = fmaxf(vmax, fmaxf(fabsf(v0), fabsf(v1)));
+                        if (a.out_nct) {
+                            XT* yp = reinterpret_cast<XT*>(a.y) + (long long)bo * a.y_bs + (long long)(g * a.y_goff + co_l) * a.Tout + t;
+                            st1(yp, v0);
+                            st1(yp + a.Tout, v1);
+                        } else {
+                            st2(reinterpret_cast<XT*>(a.y) + (long long)bo * a.y_bs + (long long)t * a.ldy + g * a.y_goff + co_l, v0, v1);
+                        }
                     }
                 }
             }
-            }
+            ADEC_PH(PH_EPI);
         }
         // every activation is some launch's output: one check here bounds the operands of the next launch's fp16 split
         if (PREC == PREC_F16 && a.err && !(vmax < 60000.f)) atomicOr(a.err, 2);
     }
+#ifdef ADEC_PHASES
+    if (a.dbg) {
+        // one reporting thread per consumer warpgroup, activation-producer thread 0 and the weight-producer lane
+        if (warp < 8 ? tid % 128 == 0 : warp == WWARP ? lane == 0 : tid == 256) {
+            if (ph_sink == 0x7fc00001u) ph[PH_CONV] += 1u;     // keeps the loads the load phase waits for
+            for (int k = 0; k < PH_N; ++k)
+                if (ph[k]) atomicAdd(a.dbg + 6 + k, (unsigned long long)ph[k]);
+        }
+        if (blockIdx.x == 0 && tid == 0) {
+            // launch descriptor: NT | FUSE << 8 | res << 9 | PAIR << 10 | VL << 11 | BST << 12 | PREC << 13 | Ktaps << 16 | dil << 24 |
+            // input channels << 32 | Cout_g << 48
+            a.dbg[3] = (unsigned long long)NT | (FUSE ? 1ull << 8 : 0) | (a.res ? 1ull << 9 : 0) | (PAIR ? 1ull << 10 : 0) |
+                       (VL ? 1ull << 11 : 0) | (BST ? 1ull << 12 : 0) | ((unsigned long long)PREC << 13) | ((unsigned long long)a.Ktaps << 16) |
+                       ((unsigned long long)a.dil << 24) | ((unsigned long long)(a.n_pieces * CP) << 32) | ((unsigned long long)a.Cout_g << 48);
+            a.dbg[4] = (unsigned long long)a.Tout;
+            a.dbg[5] = PH_N;
+        }
+    }
+#endif
     if (a.dbg && blockIdx.x == 0 && tid == 0) {
         unsigned long long kt1;
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(kt1));

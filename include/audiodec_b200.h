@@ -189,7 +189,9 @@ int64_t adec_launch_count(const adec_handle *h);
 
 /* Diagnostics (handles created with ADEC_KTRACE=1 in the environment): copies up to max_records {start ns, end ns, SM cycles} records
  * of the tensor-core conv launches issued since the last call (CTA 0's globaltimer / clock64) and resets the trace; returns the
- * number of records or -1.  Used to measure the effective SM clock and the gaps between back-to-back launches. */
+ * number of records or -1.  Used to measure the effective SM clock and the gaps between back-to-back launches.  A library built with
+ * -DADEC_PHASES writes records of 16 values instead of 3: the three above, then the per-phase cycle counters of the conv engine
+ * (KT_REC in csrc/kernels.cuh, read by tools/conv_phases.py). */
 int adec_ktrace(adec_handle *h, unsigned long long *out, int max_records);
 
 /* Measured compute ceiling of the conv engine for bench.py's roofline: every SM streams `n_groups` x 12 wgmma per 64-column slice
