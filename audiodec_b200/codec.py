@@ -217,6 +217,76 @@ class _StreamGeneratorBase:
         arr, n = _int_array(dst)
         _check(self._lib.adec_copy_stream_state(self._h, int(src), arr, n, self._stream()), self._h)
 
+    # ---- decode plumbing shared by both generators
+    def _fn(self, name):
+        """The C entry point `name`, or its bf16 twin (`name`_bf16) when the handle has bf16 activations."""
+        return getattr(self._lib, name + "_bf16" if self._act_bf16 else name)
+
+    def _zq_dim(self):
+        return getattr(self, "code_dim", None) or self.in_channels
+
+    def _zq_in(self, zq):
+        """zq on the codec's device, contiguous, in the decoder's activation dtype (bf16 with bf16 activations), 16-byte aligned."""
+        zq = self._in(zq, torch.bfloat16 if self._act_bf16 else torch.float32)
+        if self._act_bf16 and zq.data_ptr() % 16:
+            zq = zq.clone()                  # the bf16 kernels read zq as 16-byte vectors: realign an offset view
+        return zq
+
+    def _decode(self, zq):
+        """the streaming decode of zq (B,F,D) channels-last, checked by the caller -> y (B,1,F*hop)"""
+        zq = self._zq_in(zq)
+        b, f, _ = zq.shape
+        self._batch(b)
+        y = torch.empty(b, 1, f * self._lib.adec_hop_length(self._h), device=self._device, dtype=zq.dtype)
+        _check(self._fn("adec_decode")(self._h, _ptr(zq), b, f, _ptr(y), self._stream()), self._h)
+        return y
+
+    def _decode_offline(self, zq):
+        self._ready()
+        self._want(zq, "decode_offline / forward", 1, self._zq_dim())
+        zq_cl = self._zq_in(zq.transpose(1, 2))                     # the kernels' native channels-last (B,F,D)
+        b, f, _ = zq_cl.shape
+        y = torch.empty(b, 1, f * self._lib.adec_hop_length(self._h), device=self._device, dtype=zq_cl.dtype)
+        _check(self._fn("adec_decode_offline")(self._h, _ptr(zq_cl), b, f, _ptr(y), self._stream()), self._h)
+        return y
+
+    def _decode_varlen(self, name, zq_cl, frames, *slots):
+        """Decode zq_cl (sum F_b, D) channels-last as one varlen row space through entry point `name` (its stream array: `slots`) ->
+        list of B waveforms (1, 1, F_b * hop), views of one output buffer."""
+        zq_cl = self._zq_in(zq_cl)
+        hop = self._lib.adec_hop_length(self._h)
+        y = torch.empty(sum(frames) * hop, device=self._device, dtype=zq_cl.dtype)
+        arr, b = _int_array(frames)
+        _check(self._fn(name)(self._h, _ptr(zq_cl), arr, *slots, b, _ptr(y), self._stream()), self._h)
+        out, o = [], 0
+        for f in frames:
+            out.append(y[o * hop:(o + f) * hop].view(1, 1, f * hop))
+            o += f
+        return out
+
+    def _decode_offline_varlen(self, zq, frames):
+        self._ready()
+        self._want(zq, "decode_offline_varlen / forward_varlen", 1, self._zq_dim())
+        frames = [int(f) for f in frames]
+        if zq.size(0) != 1 or zq.size(2) != sum(frames):
+            raise RuntimeError(f"audiodec_b200: decode_offline_varlen / forward_varlen: expected (1, D, {sum(frames)}) for frames summing to "
+                               f"{sum(frames)}, got {tuple(zq.shape)}")
+        return self._decode_varlen("adec_decode_offline_varlen", zq[0].transpose(0, 1), frames)
+
+    def _decode_streams(self, zq, frames, streams):
+        self._ready()
+        d = self._zq_dim()
+        frames = [int(f) for f in frames]
+        if zq.dim() == 3 and zq.size(0) == 1:
+            zq = zq[0]
+        if zq.dim() != 2 or zq.size(0) != sum(frames) or zq.size(1) != d:
+            raise RuntimeError(f"audiodec_b200: decode_streams: expected (1, {sum(frames)}, {d}) channels-last for frames summing to "
+                               f"{sum(frames)}, got {tuple(zq.shape)}")
+        if len(frames) != len(streams):
+            raise RuntimeError(f"audiodec_b200: decode_streams: {len(frames)} frame counts for {len(streams)} streams")
+        sarr, _ = _int_array(streams)
+        return self._decode_varlen("adec_decode_streams", zq, frames, sarr)
+
 
 class SymADStreamGenerator(_StreamGeneratorBase):
     """models/autoencoder/AudioDec.py:166-256."""
@@ -347,49 +417,42 @@ class SymADStreamGenerator(_StreamGeneratorBase):
         (z (1, code_dim, sum F_b), [F_b]); utterance b's frames are columns [sum_{i<b} F_i, +F_b) and equal encode_offline of that
         utterance alone.  z is quantize_offline's B = 1 layout, so one quantize_offline call quantizes the whole batch."""
         self._ready()
-        flat = []
-        for x in xs:
-            x = x[0] if x.dim() == 2 and x.size(0) == 1 else x
-            if x.dim() != 1:
-                raise RuntimeError(f"audiodec_b200: encode_offline_varlen: expected 1-D (T,) or (1, T) utterances, got {tuple(x.shape)}")
-            flat.append(self._in(x))
-        if not flat:
+        if len(xs) == 0:
             raise RuntimeError("audiodec_b200: encode_offline_varlen: no utterances")
-        lengths = [x.numel() for x in flat]
-        frames, offsets = varlen_layout(lengths, self.enc_strides)
-        x = torch.cat(flat)
-        z = torch.empty(1, self.code_dim, offsets[-1], device=self._device, dtype=torch.float32)
-        arr, b = _int_array(lengths)
-        _check(self._lib.adec_encode_offline_varlen(self._h, _ptr(x), arr, b, _ptr(z), self._stream()), self._h)
-        return z, frames
+        return self._encode_varlen(self._lib.adec_encode_offline_varlen, "encode_offline_varlen", "utterances", xs)
 
     def encode_streams(self, chunks, streams):
         """Advance streams[b] by chunks[b] (1-D (T_b,) or (1, T_b); lengths may differ) in one launch sequence.  Returns
         (z (1, code_dim, sum F_b), [F_b]) laid out like encode_offline_varlen; stream b's frames equal a B = 1 streaming encode of its
         chunk.  Streams not listed keep their state untouched."""
         self._ready()
+        if len(chunks) != len(streams):
+            raise RuntimeError(f"audiodec_b200: encode_streams: {len(chunks)} chunks for {len(streams)} streams")
+        sarr, _ = _int_array(streams)
+        return self._encode_varlen(self._lib.adec_encode_streams, "encode_streams", "chunks", chunks, sarr)
+
+    def _encode_varlen(self, fn, what, noun, xs, *slots):
+        """Encode 1-D (T_b,) or (1, T_b) tensors concatenated into one varlen row space through `fn` (its stream array: `slots`) ->
+        (z (1, code_dim, sum F_b), [F_b])."""
         flat = []
-        for x in chunks:
+        for x in xs:
             x = x[0] if x.dim() == 2 and x.size(0) == 1 else x
             if x.dim() != 1:
-                raise RuntimeError(f"audiodec_b200: encode_streams: expected 1-D (T,) or (1, T) chunks, got {tuple(x.shape)}")
+                raise RuntimeError(f"audiodec_b200: {what}: expected 1-D (T,) or (1, T) {noun}, got {tuple(x.shape)}")
             flat.append(self._in(x))
-        if len(flat) != len(streams):
-            raise RuntimeError(f"audiodec_b200: encode_streams: {len(flat)} chunks for {len(streams)} streams")
         lengths = [x.numel() for x in flat]
         frames, offsets = varlen_layout(lengths, self.enc_strides)
         x = torch.cat(flat) if flat else torch.empty(0, device=self._device)
         z = torch.empty(1, self.code_dim, offsets[-1], device=self._device, dtype=torch.float32)
         arr, b = _int_array(lengths)
-        sarr, _ = _int_array(streams)
-        _check(self._lib.adec_encode_streams(self._h, _ptr(x), arr, sarr, b, _ptr(z), self._stream()), self._h)
+        _check(fn(self._h, _ptr(x), arr, *slots, b, _ptr(z), self._stream()), self._h)
         return z, frames
 
     def decode_streams(self, zq, frames, streams):
         """Advance streams[b] by frames[b] frames of zq ((1, sum F_b, code_dim) or (sum F_b, code_dim) channels-last, as lookup
         returns it) in one launch sequence -> list of B waveforms (1, 1, F_b * hop), views of one output buffer, each equal to a
         B = 1 streaming decode of those frames.  Streams not listed keep their state untouched."""
-        return _decode_streams(self, zq, frames, streams)
+        return self._decode_streams(zq, frames, streams)
 
     def quantize_offline(self, z):
         """z (B,code_dim,F) -> (zq (B,code_dim,F) channels-first like Quantizer.forward (quantizer.py:31-34), idx (Nq,B,F))."""
@@ -406,13 +469,13 @@ class SymADStreamGenerator(_StreamGeneratorBase):
     def decode_offline(self, zq):
         """zq (B,code_dim,F) channels-first (what Decoder.forward takes, decoder.py:135-140) -> y (B,1,F*hop); transposed convs
         replicate their first input frame (conv_layer.py:189-192)."""
-        return _decode_offline(self, zq)
+        return self._decode_offline(zq)
 
     def decode_offline_varlen(self, zq, frames):
         """zq (1, code_dim, sum F_b) channels-first holding utterances of `frames` frames each (what encode_offline_varlen +
         quantize_offline give) -> list of B waveforms (1, 1, F_b * hop), views of one output buffer, each equal to decode_offline of
         that utterance alone."""
-        return _decode_offline_varlen(self, zq, frames)
+        return self._decode_offline_varlen(zq, frames)
 
     # ---- index bitstream (SURVEY.md 8(f) rank 2; the reference queues the raw int64 tensor, bin/stream.py:224)
     def packed_frame_bytes(self):
@@ -459,76 +522,7 @@ class SymADStreamGenerator(_StreamGeneratorBase):
         """zq (B,F,D) channels-last -> y (B,1,F*hop)   (AudioDec.py:246-247)"""
         self._ready()
         self._want(zq, "decode", 2, self.code_dim)
-        zq = self._in(zq)
-        b, f, _ = zq.shape
-        self._batch(b)
-        y = torch.empty(b, 1, f * self._lib.adec_hop_length(self._h), device=self._device, dtype=torch.float32)
-        _check(self._lib.adec_decode(self._h, _ptr(zq), b, f, _ptr(y), self._stream()), self._h)
-        return y
-
-
-def _decode_offline(gen, zq):
-    gen._ready()
-    gen._want(zq, "decode_offline / forward", 1, getattr(gen, "code_dim", None) or gen.in_channels)
-    dtype = torch.bfloat16 if gen._act_bf16 else torch.float32
-    zq = gen._in(zq, dtype)
-    b, _, f = zq.shape
-    zq_cl = zq.transpose(1, 2).contiguous()                       # the kernels' native channels-last (B,F,D)
-    y = torch.empty(b, 1, f * gen._lib.adec_hop_length(gen._h), device=gen._device, dtype=dtype)
-    fn = gen._lib.adec_decode_offline_bf16 if gen._act_bf16 else gen._lib.adec_decode_offline
-    _check(fn(gen._h, _ptr(zq_cl), b, f, _ptr(y), gen._stream()), gen._h)
-    return y
-
-
-def _decode_offline_varlen(gen, zq, frames):
-    gen._ready()
-    gen._want(zq, "decode_offline_varlen / forward_varlen", 1, getattr(gen, "code_dim", None) or gen.in_channels)
-    frames = [int(f) for f in frames]
-    if zq.size(0) != 1 or zq.size(2) != sum(frames):
-        raise RuntimeError(f"audiodec_b200: decode_offline_varlen / forward_varlen: expected (1, D, {sum(frames)}) for frames summing to "
-                           f"{sum(frames)}, got {tuple(zq.shape)}")
-    dtype = torch.bfloat16 if gen._act_bf16 else torch.float32
-    zq_cl = gen._in(zq, dtype)[0].transpose(0, 1).contiguous()     # the kernels' native channels-last (sum F, D)
-    if gen._act_bf16 and zq_cl.data_ptr() % 16:
-        zq_cl = zq_cl.clone()                                       # the bf16 kernels read zq as 16-byte vectors
-    hop = gen._lib.adec_hop_length(gen._h)
-    y = torch.empty(sum(frames) * hop, device=gen._device, dtype=dtype)
-    arr, b = _int_array(frames)
-    fn = gen._lib.adec_decode_offline_varlen_bf16 if gen._act_bf16 else gen._lib.adec_decode_offline_varlen
-    _check(fn(gen._h, _ptr(zq_cl), arr, b, _ptr(y), gen._stream()), gen._h)
-    out, o = [], 0
-    for f in frames:
-        out.append(y[o * hop:(o + f) * hop].view(1, 1, f * hop))
-        o += f
-    return out
-
-
-def _decode_streams(gen, zq, frames, streams):
-    gen._ready()
-    d = getattr(gen, "code_dim", None) or gen.in_channels
-    frames = [int(f) for f in frames]
-    if zq.dim() == 3 and zq.size(0) == 1:
-        zq = zq[0]
-    if zq.dim() != 2 or zq.size(0) != sum(frames) or zq.size(1) != d:
-        raise RuntimeError(f"audiodec_b200: decode_streams: expected (1, {sum(frames)}, {d}) channels-last for frames summing to "
-                           f"{sum(frames)}, got {tuple(zq.shape)}")
-    if len(frames) != len(streams):
-        raise RuntimeError(f"audiodec_b200: decode_streams: {len(frames)} frame counts for {len(streams)} streams")
-    dtype = torch.bfloat16 if gen._act_bf16 else torch.float32
-    zq = gen._in(zq, dtype)
-    if gen._act_bf16 and zq.data_ptr() % 16:
-        zq = zq.clone()                                             # the bf16 kernels read zq as 16-byte vectors
-    hop = gen._lib.adec_hop_length(gen._h)
-    y = torch.empty(sum(frames) * hop, device=gen._device, dtype=dtype)
-    arr, b = _int_array(frames)
-    sarr, _ = _int_array(streams)
-    fn = gen._lib.adec_decode_streams_bf16 if gen._act_bf16 else gen._lib.adec_decode_streams
-    _check(fn(gen._h, _ptr(zq), arr, sarr, b, _ptr(y), gen._stream()), gen._h)
-    out, o = [], 0
-    for f in frames:
-        out.append(y[o * hop:(o + f) * hop].view(1, 1, f * hop))
-        o += f
-    return out
+        return self._decode(zq)
 
 
 class HiFiGANStreamGenerator(_StreamGeneratorBase):
@@ -587,21 +581,12 @@ class HiFiGANStreamGenerator(_StreamGeneratorBase):
         zq may be bf16 or fp32 (cast on the device) and y is bf16."""
         self._ready()
         self._want(c, "decode", 2, self.in_channels)
-        dtype = torch.bfloat16 if self._act_bf16 else torch.float32
-        c = self._in(c, dtype)
-        if self._act_bf16 and c.data_ptr() % 16:
-            c = c.clone()                  # the bf16 kernels read zq as 16-byte vectors: realign an offset view
-        b, f, _ = c.shape
-        self._batch(b)
-        y = torch.empty(b, 1, f * self._lib.adec_hop_length(self._h), device=self._device, dtype=dtype)
-        fn = self._lib.adec_decode_bf16 if self._act_bf16 else self._lib.adec_decode
-        _check(fn(self._h, _ptr(c), b, f, _ptr(y), self._stream()), self._h)
-        return y
+        return self._decode(c)
 
     def forward(self, c):
         """Generator.forward (HiFiGAN.py:140-160), the non-streaming path: c (B,in_channels,F) channels-first -> y (B,1,F*hop).
         Discards the streaming state."""
-        return _decode_offline(self, c)
+        return self._decode_offline(c)
 
     __call__ = forward
 
@@ -609,13 +594,13 @@ class HiFiGANStreamGenerator(_StreamGeneratorBase):
         """Generator.forward over utterances of different lengths in one launch sequence: c (1, in_channels, sum F_b) channels-first,
         utterance b at columns [sum_{i<b} F_i, +F_b) -> list of B waveforms (1, 1, F_b * hop), views of one output buffer (bf16 with
         bf16 activations), each equal to forward of that utterance alone."""
-        return _decode_offline_varlen(self, c, frames)
+        return self._decode_offline_varlen(c, frames)
 
     def decode_streams(self, c, frames, streams):
         """Advance streams[b] by frames[b] frames of c ((1, sum F_b, in_channels) or (sum F_b, in_channels) channels-last) in one
         launch sequence -> list of B waveforms (1, 1, F_b * hop), views of one output buffer (bf16 with bf16 activations), each equal to
         a B = 1 streaming decode of those frames.  Streams not listed keep their state untouched."""
-        return _decode_streams(self, c, frames, streams)
+        return self._decode_streams(c, frames, streams)
 
 
 class OfflineCodec:

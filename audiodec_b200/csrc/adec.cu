@@ -145,7 +145,6 @@ struct TcKernelCfg { int NT; bool fuse; int pre, prec; bool bst; int tap_bytes; 
     ADEC_TC1(NT, false, ACT_NONE, PREC_BF16, BST), ADEC_TC1(NT, false, ACT_LRELU, PREC_BF16, BST), ADEC_TC1(NT, false, ACT_NORM, PREC_BF16, BST)
 #define ADEC_TC(NT) ADEC_TC_FP32(NT, PREC_F16), ADEC_TC_FP32(NT, PREC_TF32), ADEC_TC_BF16(NT, false), ADEC_TC_BF16(NT, true)
 const TcKernelCfg kTcKernels[] = {ADEC_TC(128), ADEC_TC(64), ADEC_TC(32)};
-int kTcMaxFuse = 128;    // residual units wider than this run as two launches on the tensor-core path (ADEC_TC_MAXFUSE)
 
 const TcKernelCfg* find_tc_kernel(int NT, bool fuse, int pre, int prec, bool bst) {
     for (const auto& k : kTcKernels)
@@ -235,7 +234,7 @@ struct adec_handle {
     int n_streams = 1;
     int st_cap = 1;        // streams the state buffers were allocated for
     int engine = 2;               // ADEC_CONV_PATH: 2 = f16 (fp16-split wgmma, default), 1 = tf32 (3xTF32 wgmma), 0 = ffma (CUDA cores)
-    bool use_tc = true;           // any tensor-core engine
+    int tc_max_fuse = 128;        // ADEC_TC_MAXFUSE: residual units wider than this run as two launches on the tensor-core engines
     bool bf16 = false;            // cfg.compute_dtype >= 1: bf16 operands (HiFi-GAN vocoder, f16 engine only)
     bool act_bf16 = false;        // cfg.compute_dtype == 2: bf16 activations, causal state and decode I/O as well
     int act_bytes() const { return act_bf16 ? 2 : 4; }   // bytes per stored activation / state element
@@ -444,117 +443,79 @@ int pick_piece_width(const Op& op) {
     return 0;
 }
 
-// 3xTF32 engine: choose the kernel instantiation, pack + upload weights
-int finalize_op_tc(adec_handle* h, Op* op) {
+// wgmma engines (wg_conv.cuh): weights in K-major, no-swizzle blocks of 16 bytes, the layout WgCfg streams:
+//   [group g][co tile][piece][tap][plane][kb = 16-byte K block][ntw columns][16 B]
+// ntw: columns per tile (NT; 2 NT for the paired taps); one (piece, tap) at ntw = NT is TAP_BYTES.  The planes of a weight w:
+// 3xTF32 hi | lo (4 bytes each), fp16 hi | lo | hi * 2^-11 of w * 2^p (2 bytes each), or one bf16 plane.
+std::vector<float> pack_wg(int prec, const float* weff, int G, int ntiles, int pieces, int taps, int cin_eff, int cout, int p, int ntw) {
+    const int eb = prec == PREC_TF32 ? 4 : 2, npl = prec == PREC_F16 ? 3 : prec == PREC_TF32 ? 2 : 1;
+    const int epb = 16 / eb, KB = TC_CP / epb;     // elements per block, K blocks per piece
+    const size_t plane = (size_t)KB * ntw * epb;    // elements
+    std::vector<uint8_t> img((size_t)G * ntiles * pieces * taps * npl * plane * eb, 0);
+    size_t o = 0;     // in elements
+    for (int g = 0; g < G; ++g)
+        for (int nt = 0; nt < ntiles; ++nt)
+            for (int pc = 0; pc < pieces; ++pc)
+                for (int tap = 0; tap < taps; ++tap) {
+                    for (int kb = 0; kb < KB; ++kb)
+                        for (int n = 0; n < ntw; ++n)
+                            for (int e = 0; e < epb; ++e) {
+                                const int k = pc * TC_CP + kb * epb + e;
+                                const float w = nt * ntw + n < cout ? weff[(((size_t)g * taps + tap) * cin_eff + k) * cout + nt * ntw + n] : 0.f;
+                                uint32_t v[3];
+                                if (prec == PREC_TF32) {
+                                    const float hi = tf32_round_host(w), lo = tf32_round_host(w - hi);
+                                    memcpy(&v[0], &hi, 4);
+                                    memcpy(&v[1], &lo, 4);
+                                } else if (prec == PREC_F16) {
+                                    const float ws = std::ldexp(w, p);
+                                    v[0] = half_bits(ws);
+                                    v[1] = half_bits(ws - half_value(v[0]));
+                                    v[2] = half_bits(half_value(v[0]) * (1.0f / 2048.0f));
+                                } else {
+                                    v[0] = bf16_bits(w);
+                                }
+                                for (int pl = 0; pl < npl; ++pl) {
+                                    uint8_t* at = img.data() + (o + pl * plane + ((size_t)kb * ntw + n) * epb + e) * eb;
+                                    for (int i = 0; i < eb; ++i) at[i] = (uint8_t)(v[pl] >> (8 * i));    // little-endian, as the device reads it
+                                }
+                            }
+                    o += npl * plane;
+                }
+    std::vector<float> out(img.size() / 4);
+    memcpy(out.data(), img.data(), img.size());
+    return out;
+}
+
+// wgmma engines: choose the kernel instantiation and the weight scales, pack and upload the weights
+int finalize_op_wg(adec_handle* h, Op* op) {
     int NT = op->Cout % 128 == 0 ? 128 : op->Cout % 64 == 0 ? 64 : 32;
     // 96 outputs (transposed conv 64 -> 3*32): one zero-padded 128-wide tile beats three 32-wide tiles that each rebuild the
     // same activation window (the epilogue masks per column pair)
     const bool pad_tile = !op->fuse && NT == 32 && op->Cout > 64 && op->Cout < 128;
     if (pad_tile) NT = 128;
-    op->tc = find_tc_kernel(NT, op->fuse, op->pre_act, PREC_TF32, false);
-    if (!op->tc || (op->fuse && (NT != op->Cout || op->mid_act != op->pre_act))) return h->fail(op->name + ": no tensor-core kernel");
-    const int KS = TC_CP, CP = TC_CP;
-    op->n_pieces = op->Cin_eff / CP;
-    op->n_co_tiles = pad_tile ? 1 : op->Cout / NT;
-    op->w_tile_floats = (long long)op->Ktaps * op->Cin_eff * NT * 2;
-    // one (piece, tap): [hi: (KS/4) K blocks][NT][4] | [lo: same]   (K-major, no swizzle)
-    auto pack = [&](const float* weff, int G, int ntiles, int pieces, int taps, int cin_eff, int cout, std::vector<float>* out) {
-        out->assign((size_t)G * ntiles * taps * cin_eff * NT * 2, 0.f);
-        size_t o = 0;
-        for (int g = 0; g < G; ++g)
-            for (int nt = 0; nt < ntiles; ++nt)
-                for (int pc = 0; pc < pieces; ++pc)
-                    for (int tap = 0; tap < taps; ++tap)
-                        for (int ks = 0; ks < CP / KS; ++ks) {
-                            float* hi = out->data() + o;
-                            float* lo = hi + (size_t)KS * NT;
-                            for (int c4 = 0; c4 < KS / 4; ++c4)
-                                for (int n = 0; n < NT; ++n)
-                                    for (int e = 0; e < 4; ++e) {
-                                        const int k = pc * CP + ks * KS + c4 * 4 + e;
-                                        const float w = nt * NT + n < cout ? weff[(((size_t)g * taps + tap) * cin_eff + k) * cout + nt * NT + n] : 0.f;
-                                        const float wh = tf32_round_host(w);
-                                        hi[((size_t)c4 * NT + n) * 4 + e] = wh;
-                                        lo[((size_t)c4 * NT + n) * 4 + e] = tf32_round_host(w - wh);
-                                    }
-                            o += (size_t)2 * KS * NT;
-                        }
-    };
-    std::vector<float> packed;
-    pack(op->weff.data(), op->G, op->n_co_tiles, op->n_pieces, op->Ktaps, op->Cin_eff, op->Cout, &packed);
-    if (dev_upload(h, &op->w, packed)) return 1;
-    if (op->fuse) {
-        std::vector<float> p2;
-        pack(op->weff2.data(), 1, 1, op->Cout / CP, 1, op->Cout, op->Cout, &p2);
-        if (dev_upload(h, &op->w2, p2)) return 1;
-    }
-    if (!op->hbias.empty() && dev_upload(h, &op->bias, op->hbias)) return 1;
-    std::vector<float>().swap(op->weff);
-    std::vector<float>().swap(op->weff2);
-    return 0;
-}
-
-// fp16-split / bf16 engine: weights as fp16 (hi | lo | hi * 2^-11) of w * 2^p, or one bf16 plane, in K-major no-swizzle blocks:
-//   [group g][co tile][piece][tap][plane][kb = 8-channel block][NT rows][8 x 16 bit]
-// one (piece, tap) = TAP_BYTES; the kernel's weight producer copies one or two consecutive taps per stage (wg_conv.cuh).
-int finalize_op_f16(adec_handle* h, Op* op) {
-    int NT = op->Cout % 128 == 0 ? 128 : op->Cout % 64 == 0 ? 64 : 32;
-    const bool pad_tile = !op->fuse && NT == 32 && op->Cout > 64 && op->Cout < 128;     // e.g. transposed conv 64 -> 3*32: one padded 128-wide tile
-    if (pad_tile) NT = 128;
-    const int prec = (h->bf16 && !op->fuse) ? PREC_BF16 : PREC_F16;
+    const int prec = h->engine == 1 ? PREC_TF32 : (h->bf16 && !op->fuse) ? PREC_BF16 : PREC_F16;
     if (h->act_bf16 && op->RG > 1) return h->fail(op->name + ": bf16 activations are built for stride-1 and transposed convs only");
     op->tc = find_tc_kernel(NT, op->fuse, op->pre_act, prec, h->act_bf16);
     if (!op->tc || (op->fuse && (NT != op->Cout || op->mid_act != op->pre_act))) return h->fail(op->name + ": no tensor-core kernel");
-    const int CP = TC_CP, KB = TC_CP / 8, npl = prec == PREC_F16 ? 3 : 1;
-    op->n_pieces = op->Cin_eff / CP;
+    op->n_pieces = op->Cin_eff / TC_CP;
     op->n_co_tiles = pad_tile ? 1 : op->Cout / NT;
-    const size_t tap_bytes = (size_t)op->tc->tap_bytes;
-    op->w_tile_floats = (long long)((size_t)op->n_pieces * op->Ktaps * tap_bytes / 4);
-    auto pow2_scale = [](const std::vector<float>& w, int* p_out) {
+    op->w_tile_floats = (long long)((size_t)op->n_pieces * op->Ktaps * op->tc->tap_bytes / 4);
+    // fp16 planes hold w * 2^p with max |w * 2^p| in [4096, 8192); the kernel scales the sums back by 2^-p.  The other precisions: p = 0
+    auto pow2_scale = [prec](const std::vector<float>& w) {
         float wmax = 0.f;
         for (float v : w) wmax = std::max(wmax, std::fabs(v));
         int p = 0;
-        if (wmax > 0.f && std::isfinite(wmax)) {
+        if (prec == PREC_F16 && wmax > 0.f && std::isfinite(wmax)) {
             while (std::ldexp(wmax, p) < 4096.f) ++p;
             while (std::ldexp(wmax, p) >= 8192.f) --p;
         }
-        *p_out = p;
+        return p;
     };
-    // ntw: columns per tile (NT; 2 NT for the paired taps)
-    auto pack = [&](const float* weff, int G, int ntiles, int pieces, int taps, int cin_eff, int cout, int p2, int ntw, std::vector<float>* out) {
-        std::vector<uint16_t> img((size_t)G * ntiles * pieces * taps * npl * KB * ntw * 8, 0);
-        size_t o = 0;     // in 16-bit units
-        for (int g = 0; g < G; ++g)
-            for (int nt = 0; nt < ntiles; ++nt)
-                for (int pc = 0; pc < pieces; ++pc)
-                    for (int tap = 0; tap < taps; ++tap) {
-                        for (int kb = 0; kb < KB; ++kb)
-                            for (int n = 0; n < ntw; ++n)
-                                for (int e = 0; e < 8; ++e) {
-                                    const int k = pc * CP + kb * 8 + e;
-                                    const float w = nt * ntw + n < cout ? weff[(((size_t)g * taps + tap) * cin_eff + k) * cout + nt * ntw + n] : 0.f;
-                                    const size_t at = o + ((size_t)kb * ntw + n) * 8 + e, plane = (size_t)KB * ntw * 8;
-                                    if (prec == PREC_F16) {
-                                        const float ws = std::ldexp(w, p2);
-                                        const uint16_t hi = half_bits(ws);
-                                        img[at] = hi;
-                                        img[at + plane] = half_bits(ws - half_value(hi));
-                                        img[at + 2 * plane] = half_bits(half_value(hi) * (1.0f / 2048.0f));
-                                    } else {
-                                        img[at] = bf16_bits(w);
-                                    }
-                                }
-                        o += (size_t)npl * KB * ntw * 8;
-                    }
-        out->assign((img.size() + 1) / 2, 0.f);
-        memcpy(out->data(), img.data(), img.size() * 2);
-    };
-    int p1 = 0, p2 = 0;
-    if (prec == PREC_F16) pow2_scale(op->weff, &p1);
+    const int p1 = pow2_scale(op->weff);
     op->w_scale = std::ldexp(1.0f, -p1);
-    std::vector<float> packed;
-    pack(op->weff.data(), op->G, op->n_co_tiles, op->n_pieces, op->Ktaps, op->Cin_eff, op->Cout, p1, NT, &packed);
-    if (dev_upload(h, &op->w, packed)) return 1;
+    if (dev_upload(h, &op->w, pack_wg(prec, op->weff.data(), op->G, op->n_co_tiles, op->n_pieces, op->Ktaps, op->Cin_eff, op->Cout, p1, NT)))
+        return 1;
     if (op->tc->pfn_pair && op->Ktaps % 2 == 1) {
         // the paired kernel's K + 1 taps [W_j | W_j-1] (W_-1 = W_K = 0), 2 NT columns each, same scale; uniform rows run it, stacked
         // and varlen rows the unpaired kernel with the same one-tap groups (WgCfg::tpg), so both give the same sums
@@ -567,27 +528,18 @@ int finalize_op_f16(adec_handle* h, Op* op) {
                     if (j < K) row[co] = op->weff[((size_t)j * Ci + ci) * C + co];
                     if (j > 0) row[C + co] = op->weff[((size_t)(j - 1) * Ci + ci) * C + co];
                 }
-        std::vector<float> pkp;
-        pack(wp.data(), 1, 1, op->n_pieces, K + 1, Ci, 2 * C, p1, 2 * NT, &pkp);
-        if (dev_upload(h, &op->w_pair, pkp)) return 1;
+        if (dev_upload(h, &op->w_pair, pack_wg(prec, wp.data(), 1, 1, op->n_pieces, K + 1, Ci, 2 * C, p1, 2 * NT))) return 1;
     }
     if (op->fuse) {
-        pow2_scale(op->weff2, &p2);
+        const int p2 = pow2_scale(op->weff2);
         op->w2_scale = std::ldexp(1.0f, -p2);
-        std::vector<float> pk2;
-        pack(op->weff2.data(), 1, 1, op->Cout / CP, 1, op->Cout, op->Cout, p2, NT, &pk2);
-        if (dev_upload(h, &op->w2, pk2)) return 1;
+        if (dev_upload(h, &op->w2, pack_wg(prec, op->weff2.data(), 1, 1, op->Cout / TC_CP, 1, op->Cout, op->Cout, p2, NT))) return 1;
     }
-    if (!op->hbias.empty() && dev_upload(h, &op->bias, op->hbias)) return 1;
-    std::vector<float>().swap(op->weff);
-    std::vector<float>().swap(op->weff2);
     return 0;
 }
 
-int finalize_op(adec_handle* h, Op* op) {
-    if (op->kind != OP_CONV) return 0;
-    if (h->engine == 2) return finalize_op_f16(h, op);
-    if (h->use_tc) return finalize_op_tc(h, op);
+// FFMA engine (conv_gemm_kernel): choose the kernel instantiation, pack and upload the weights
+int finalize_op_ffma(adec_handle* h, Op* op) {
     int CW, CO;
     if (op->fuse) {
         CW = CO = op->Cout;
@@ -614,9 +566,13 @@ int finalize_op(adec_handle* h, Op* op) {
                             for (int co = 0; co < CO; ++co) packed[o++] = src[co];
                         }
     if (dev_upload(h, &op->w, packed)) return 1;
-    if (op->fuse) {
-        if (dev_upload(h, &op->w2, op->weff2)) return 1;   // [ci][co] == [chunk][kc][co] for CO == C
-    }
+    if (op->fuse && dev_upload(h, &op->w2, op->weff2)) return 1;   // [ci][co] == [chunk][kc][co] for CO == C
+    return 0;
+}
+
+int finalize_op(adec_handle* h, Op* op) {
+    if (op->kind != OP_CONV) return 0;
+    if (h->engine != 0 ? finalize_op_wg(h, op) : finalize_op_ffma(h, op)) return 1;
     if (!op->hbias.empty() && dev_upload(h, &op->bias, op->hbias)) return 1;
     std::vector<float>().swap(op->weff);
     std::vector<float>().swap(op->weff2);
@@ -663,15 +619,23 @@ void load_pad_buffer(adec_handle* h, Op* op, const std::string& key, int c_real)
 // ------------------------------------------------------------------------------------------------
 // plan execution
 // ------------------------------------------------------------------------------------------------
+// What a codec call runs over, and so what it does to the causal state (run_call):
+//   CALL_STREAM   B = n_streams uniform streams, each advanced by T rows                       (adec_encode / adec_decode)
+//   CALL_OFFLINE  B uniform utterances from zero history; transposed convs replicate their first input row instead of reading state
+//   CALL_VARLEN   CALL_OFFLINE over B utterances of their own lengths, concatenated along time  (adec_*_offline_varlen)
+//   CALL_SLOTS    B distinct streams of the handle, each advanced by a chunk of its own length  (adec_*_streams)
+enum CallMode { CALL_STREAM, CALL_OFFLINE, CALL_VARLEN, CALL_SLOTS };
+
 struct RunCtx {
     int B;
     const float* ext_in;
     float* ext_out;
     cudaStream_t stream;
-    bool offline = false;   // non-streaming forward: transposed convs replicate their first input row instead of reading state
-    const int* vl_len = nullptr;   // varlen: HOST lengths of the B utterances, concatenated along time in ext_in / ext_out
+    CallMode mode = CALL_STREAM;
+    const int* lengths = nullptr;  // CALL_VARLEN / CALL_SLOTS: HOST lengths of the B utterances, concatenated along time in ext_in / ext_out
+    const int* slots = nullptr;    // CALL_SLOTS: HOST stream slot of each utterance
     const char* what = "";         // entry point, for messages
-    const int* slots = nullptr;    // varlen streaming (adec_*_streams): HOST stream slot of each utterance; nullptr = offline varlen
+    bool varlen() const { return mode == CALL_VARLEN || mode == CALL_SLOTS; }
 };
 
 SlotBits* slot_bits(adec_handle* h, const std::vector<Op>& ops) {
@@ -723,7 +687,7 @@ struct VlPlan {
 };
 int plan_varlen(adec_handle* h, const std::vector<Op>& ops, const RunCtx& rc, VlPlan* pl) {
     const int B = rc.B;
-    std::vector<long long> len(rc.vl_len, rc.vl_len + B);
+    std::vector<long long> len(rc.lengths, rc.lengths + B);
     pl->tab.assign(ops.size() * 2 * (B + 1), 0);
     for (size_t k = 0; k < ops.size(); ++k) {
         const Op& op = ops[k];
@@ -748,9 +712,11 @@ int plan_varlen(adec_handle* h, const std::vector<Op>& ops, const RunCtx& rc, Vl
     return 0;
 }
 
+// The launches of one call.  Reads each stateful op's history from st[cur] (slot calls: from the buffer the stream's slot bit names)
+// and writes the new state to the other buffer; what that does to `cur` and the slot bits is the caller's (run_call).
 int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, int* T_out_final) {
     // pass 1: workspace sizes (varlen: the row tables, uploaded in one copy on the call's stream)
-    const bool vl = rc.vl_len != nullptr;
+    const bool vl = rc.varlen();
     VlPlan pl;
     if (vl) {
         if (plan_varlen(h, ops, rc, &pl)) return 1;
@@ -775,26 +741,22 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
     if (!vl && rc.B != h->n_streams) return h->fail(fmt("batch %d != n_streams %d (call adec_set_streams)", rc.B, h->n_streams));
     const int* vl_tab = nullptr;
     const int* vl_slot = nullptr;
-    SlotBits* sb = slot_bits(h, ops);
-    if (vl && rc.slots) {
-        // streaming varlen: the slot table (2 * slot + bit per utterance, the same for every op) follows the row tables in the one copy
-        for (const Op& op : ops)      // the conv kernels address a slot's history rows with 32-bit element offsets
-            if ((long long)h->n_streams * op.P * op.st_C >= (1ll << 31))
-                return h->fail(fmt("%s: %d streams of %s state exceed 2^31 elements per buffer; use fewer streams per handle", rc.what,
-                                   h->n_streams, op.name.c_str()));
-        const size_t at = pl.tab.size();
-        for (int b = 0; b < rc.B; ++b) pl.tab.push_back(2 * rc.slots[b] + sb->bit[rc.slots[b]]);
+    if (vl) {
+        size_t at = 0;
+        if (rc.mode == CALL_SLOTS) {
+            // the slot table (2 * slot + bit per utterance, the same for every op) follows the row tables in the one copy
+            for (const Op& op : ops)      // the conv kernels address a slot's history rows with 32-bit element offsets
+                if ((long long)h->n_streams * op.P * op.st_C >= (1ll << 31))
+                    return h->fail(fmt("%s: %d streams of %s state exceed 2^31 elements per buffer; use fewer streams per handle", rc.what,
+                                       h->n_streams, op.name.c_str()));
+            const SlotBits* sb = slot_bits(h, ops);
+            at = pl.tab.size();
+            for (int b = 0; b < rc.B; ++b) pl.tab.push_back(2 * rc.slots[b] + sb->bit[rc.slots[b]]);
+        }
         if (ensure(h, h->vl_tab, pl.tab.size())) return 1;
         CK(h, cudaMemcpyAsync(h->vl_tab.p, pl.tab.data(), pl.tab.size() * sizeof(int), cudaMemcpyHostToDevice, rc.stream));
         vl_tab = reinterpret_cast<const int*>(h->vl_tab.p);
-        vl_slot = vl_tab + at;
-    } else if (vl) {
-        if (adec_reset(h, (void*)rc.stream)) return 1;      // discards the streaming state, as the uniform offline calls do
-        if (ensure(h, h->vl_tab, pl.tab.size())) return 1;
-        CK(h, cudaMemcpyAsync(h->vl_tab.p, pl.tab.data(), pl.tab.size() * sizeof(int), cudaMemcpyHostToDevice, rc.stream));
-        vl_tab = reinterpret_cast<const int*>(h->vl_tab.p);
-    } else if (slot_fixup(h, ops, rc.stream)) {
-        return 1;
+        if (rc.mode == CALL_SLOTS) vl_slot = vl_tab + at;
     }
 
     int T = T_in;
@@ -850,7 +812,7 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
             a.y = yout; a.ldy = op.ldy; a.y_goff = op.y_goff; a.out_nct = op.out_nct;
             a.y_bs = op.out_nct ? (long long)op.G * op.Cout * Tout : (long long)Tout * op.ldy;
             a.mid_act = op.mid_act;
-            a.hist_rep = (rc.offline && op.up > 1) ? 1 : 0;
+            a.hist_rep = ((rc.mode == CALL_OFFLINE || rc.mode == CALL_VARLEN) && op.up > 1) ? 1 : 0;
             a.w_scale = op.w_scale; a.w2_scale = op.w2_scale; a.err = h->d_err;
             if (h->d_ktrace && h->ktrace_n < 4096) a.dbg = h->d_ktrace + KT_REC * (size_t)(h->ktrace_n++);
             if (op.tc) {
@@ -909,12 +871,7 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
             else if (op.res_buf >= 0) bytes += eb * nb * cout * Tout;
             h->prof_bytes.push_back(bytes);
         }
-        if (op.P > 0 && !vl) op.cur ^= 1;       // offline varlen calls neither read nor write the causal state; slot calls flip bits below
         T = Tout * op.up;
-    }
-    if (vl_slot) {
-        for (int b = 0; b < rc.B; ++b) sb->bit[rc.slots[b]] ^= 1;
-        sb->dirty = true;
     }
     if (T_out_final) *T_out_final = T;
     return 0;
@@ -989,7 +946,7 @@ int push_ru(adec_handle* h, std::vector<Op>* ops, Wire* w, const std::string& ru
     Op op;
     if (make_ru_op(h, &op, ru, W1, W2, dil, ACT_ELU)) return 1;
     load_pad_buffer(h, &op, ru + ".conv1.pad_buffer", ch);
-    if (h->use_tc && op.Cout > kTcMaxFuse) {
+    if (h->engine != 0 && op.Cout > h->tc_max_fuse) {
         Op conv, pw;
         split_ru_op(op, &conv, &pw);
         const int x_buf = w->cur;
@@ -1291,8 +1248,8 @@ int adec_create(const adec_config* cfg, int device, adec_handle** out) {
         else if (!strcmp(pth, "f16") || !strcmp(pth, "tc") || !*pth) h->engine = 2;
         else { g_create_error = std::string("ADEC_CONV_PATH must be f16, tf32 or ffma, not ") + pth; delete h; return 1; }
     }
-    h->use_tc = h->engine != 0;
     if (const char* sr = getenv("ADEC_STACK_ROWS")) h->stack_rows = atoi(sr) != 0;
+    if (const char* mf = getenv("ADEC_TC_MAXFUSE")) h->tc_max_fuse = atoi(mf);
     if (const char* kt = getenv("ADEC_KTRACE")) {
         if (atoi(kt)) {
             DeviceGuard dgk(device);
@@ -1318,7 +1275,6 @@ int adec_create(const adec_config* cfg, int device, adec_handle** out) {
         delete h;
         return 1;
     }
-    if (const char* mf = getenv("ADEC_TC_MAXFUSE")) kTcMaxFuse = atoi(mf);
     cudaDeviceGetAttribute(&h->n_sms, cudaDevAttrMultiProcessorCount, device);
     DeviceGuard dg(device);
     if (cudaMalloc((void**)&h->d_err, sizeof(int)) != cudaSuccess || cudaMemset(h->d_err, 0, sizeof(int)) != cudaSuccess) {
@@ -1431,13 +1387,6 @@ int adec_set_streams(adec_handle* h, int n) {
     return resize_state(h, n, /*replicate=*/h->n_streams == 1);
 }
 
-// Non-streaming forward (codecTest.py:78-95): any batch size, every causal conv starts from a zero left-pad
-// (conv_layer.py:148-151) = zeroed state for exactly B streams.  Discards the handle's streaming state.
-static int offline_state(adec_handle* h, int B, cudaStream_t s) {
-    if (B != h->n_streams && resize_state(h, B, false)) return 1;
-    return adec_reset(h, (void*)s);
-}
-
 int adec_reset(adec_handle* h, void* stream) {
     if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
     DeviceGuard dg(h->device);
@@ -1463,16 +1412,7 @@ int adec_frames_for(const adec_handle* h, int T) {
 
 int adec_hop_length(const adec_handle* h) { return h ? hop_of(h) : -1; }
 
-int adec_encode(adec_handle* h, const float* x, int B, int T, float* z, void* stream) {
-    if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    if (h->cfg.model_type != ADEC_MODEL_SYMAD) return h->fail("encode: not a symAD handle");
-    if (B < 1 || T < 1) return h->fail("encode: empty input");
-    DeviceGuard dg(h->device);
-    RunCtx rc{B, x, z, (cudaStream_t)stream};
-    return run_ops(h, h->enc_ops, rc, T, nullptr);
-}
-
-// the host arguments of a varlen offline call: B >= 1 utterances of >= 1 samples / frames each
+// the host arguments of a varlen call: B >= 1 utterances of >= 1 samples / frames each
 static int varlen_args(adec_handle* h, const char* name, const int* lengths, int B) {
     if (B < 1) return h->fail(fmt("%s: B must be >= 1, got %d", name, B));
     if (!lengths) return h->fail(fmt("%s: lengths is NULL", name));
@@ -1495,92 +1435,120 @@ static int stream_args(adec_handle* h, const char* name, const int* streams, int
     return 0;
 }
 
-// decode / decode_offline / decode_offline_varlen / decode_streams in either activation dtype: the entry point's I/O dtype must be the
-// handle's (compute_dtype 2 = bf16).  vl: a varlen call, vl_frames the HOST frame counts of its B utterances (F unused); slots: a
-// streaming varlen call (adec_decode_streams), the HOST stream of each utterance.
-static int decode_common(adec_handle* h, const void* zq, int B, int F, void* y, void* stream, bool offline, bool bf16_io,
-                         bool vl = false, const int* vl_frames = nullptr, const int* slots = nullptr, bool slot_call = false) {
+// One codec entry point: the direction, the mode and the I/O dtype name it (adec_<encode|decode><mode>[_bf16]).  Only decode has bf16
+// I/O, which must match the handle's activations (compute_dtype 2).  lengths / slots: HOST arrays of B entries for the varlen modes.
+struct Call {
+    bool decode;
+    CallMode mode;
+    bool bf16_io;
+    const int* lengths = nullptr;
+    const int* slots = nullptr;
+};
+
+static int run_call(adec_handle* h, const Call& c, const void* in, int B, int T, void* out, void* stream) {
     if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    const char* base = slot_call ? "decode_streams" : vl ? "decode_offline_varlen" : offline ? "decode_offline" : "decode";
-    const std::string name = std::string(base) + (bf16_io ? "_bf16" : "");
-    if (h->act_bf16 && !bf16_io)
-        return h->fail(fmt("%s: this handle has bf16 activations (compute_dtype 2); call adec_%s_bf16 with bf16 zq / y", name.c_str(), base));
-    if (!h->act_bf16 && bf16_io)
+    static const char* const kModeName[] = {"", "_offline", "_offline_varlen", "_streams"};
+    const std::string base = std::string(c.decode ? "decode" : "encode") + kModeName[c.mode];
+    const std::string name = base + (c.bf16_io ? "_bf16" : "");
+    if (!c.decode && h->cfg.model_type != ADEC_MODEL_SYMAD) return h->fail(name + ": not a symAD handle");
+    if (h->act_bf16 && !c.bf16_io)
+        return h->fail(fmt("%s: this handle has bf16 activations (compute_dtype 2); call adec_%s_bf16 with bf16 zq / y", name.c_str(),
+                           base.c_str()));
+    if (!h->act_bf16 && c.bf16_io)
         return h->fail(fmt("%s: this handle has fp32 activations (compute_dtype %d); call adec_%s with fp32 zq / y", name.c_str(),
-                           h->cfg.compute_dtype, base));
-    if (bf16_io && (((uintptr_t)zq | (uintptr_t)y) & 15)) return h->fail(fmt("%s: zq and y must be 16-byte aligned", name.c_str()));
-    if (vl) {
-        if (varlen_args(h, name.c_str(), vl_frames, B)) return 1;
-        if (slot_call && stream_args(h, name.c_str(), slots, B)) return 1;
-    } else if (B < 1 || F < 1) {
-        return h->fail(fmt("%s: empty input", name.c_str()));
+                           h->cfg.compute_dtype, base.c_str()));
+    if (c.bf16_io && (((uintptr_t)in | (uintptr_t)out) & 15)) return h->fail(name + ": zq and y must be 16-byte aligned");
+    RunCtx rc{B, (const float*)in, (float*)out, (cudaStream_t)stream, c.mode, c.lengths, c.slots, name.c_str()};
+    if (rc.varlen()) {
+        if (varlen_args(h, rc.what, c.lengths, B)) return 1;
+        if (c.mode == CALL_SLOTS && stream_args(h, rc.what, c.slots, B)) return 1;
+        T = 1;
+    } else if (B < 1 || T < 1) {
+        return h->fail(name + ": empty input");
     }
     DeviceGuard dg(h->device);
-    if (offline && !vl && offline_state(h, B, (cudaStream_t)stream)) return 1;
-    RunCtx rc{B, (const float*)zq, (float*)y, (cudaStream_t)stream, offline, vl ? vl_frames : nullptr, name.c_str(), slots};
-    return run_ops(h, h->dec_ops, rc, vl ? 1 : F, nullptr);
+    std::vector<Op>& ops = c.decode ? h->dec_ops : h->enc_ops;
+    switch (c.mode) {     // the causal state the launches read
+    case CALL_STREAM:     // every stream's state back in st[cur]
+        if (slot_fixup(h, ops, rc.stream)) return 1;
+        break;
+    case CALL_OFFLINE:    // Generator.forward (codecTest.py:78-95): every causal conv starts from a zero left-pad (conv_layer.py:148-151)
+        if (B != h->n_streams && resize_state(h, B, false)) return 1;
+        if (adec_reset(h, stream)) return 1;
+        break;
+    case CALL_VARLEN:     // the state is neither read nor written; it is discarded, as the uniform offline calls discard it
+        if (adec_reset(h, stream)) return 1;
+        break;
+    case CALL_SLOTS:      // each stream's history is where its slot bit says
+        break;
+    }
+    if (run_ops(h, ops, rc, T, nullptr)) return 1;
+    switch (c.mode) {     // where the new state went
+    case CALL_STREAM:
+    case CALL_OFFLINE:
+        for (Op& op : ops)
+            if (op.P > 0) op.cur ^= 1;
+        break;
+    case CALL_SLOTS: {
+        SlotBits* sb = slot_bits(h, ops);
+        for (int b = 0; b < B; ++b) sb->bit[c.slots[b]] ^= 1;
+        sb->dirty = true;
+        break;
+    }
+    case CALL_VARLEN:
+        break;
+    }
+    return 0;
 }
 
-int adec_decode(adec_handle* h, const float* zq, int B, int F, float* y, void* stream) {
-    return decode_common(h, zq, B, F, y, stream, false, false);
-}
-
-int adec_decode_bf16(adec_handle* h, const uint16_t* zq, int B, int F, uint16_t* y, void* stream) {
-    return decode_common(h, zq, B, F, y, stream, false, true);
+int adec_encode(adec_handle* h, const float* x, int B, int T, float* z, void* stream) {
+    return run_call(h, {false, CALL_STREAM, false}, x, B, T, z, stream);
 }
 
 int adec_encode_offline(adec_handle* h, const float* x, int B, int T, float* z, void* stream) {
-    if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    if (h->cfg.model_type != ADEC_MODEL_SYMAD) return h->fail("encode_offline: not a symAD handle");
-    if (B < 1 || T < 1) return h->fail("encode_offline: empty input");
-    DeviceGuard dg(h->device);
-    if (offline_state(h, B, (cudaStream_t)stream)) return 1;
-    RunCtx rc{B, x, z, (cudaStream_t)stream, true};
-    return run_ops(h, h->enc_ops, rc, T, nullptr);
-}
-
-int adec_decode_offline(adec_handle* h, const float* zq, int B, int F, float* y, void* stream) {
-    return decode_common(h, zq, B, F, y, stream, true, false);
-}
-
-int adec_decode_offline_bf16(adec_handle* h, const uint16_t* zq, int B, int F, uint16_t* y, void* stream) {
-    return decode_common(h, zq, B, F, y, stream, true, true);
+    return run_call(h, {false, CALL_OFFLINE, false}, x, B, T, z, stream);
 }
 
 int adec_encode_offline_varlen(adec_handle* h, const float* x, const int* lengths, int B, float* z, void* stream) {
-    if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    if (h->cfg.model_type != ADEC_MODEL_SYMAD) return h->fail("encode_offline_varlen: not a symAD handle");
-    if (varlen_args(h, "encode_offline_varlen", lengths, B)) return 1;
-    DeviceGuard dg(h->device);
-    RunCtx rc{B, x, z, (cudaStream_t)stream, true, lengths, "encode_offline_varlen"};
-    return run_ops(h, h->enc_ops, rc, 1, nullptr);
-}
-
-int adec_decode_offline_varlen(adec_handle* h, const float* zq, const int* frames, int B, float* y, void* stream) {
-    return decode_common(h, zq, B, 0, y, stream, true, false, true, frames);
-}
-
-int adec_decode_offline_varlen_bf16(adec_handle* h, const uint16_t* zq, const int* frames, int B, uint16_t* y, void* stream) {
-    return decode_common(h, zq, B, 0, y, stream, true, true, true, frames);
+    return run_call(h, {false, CALL_VARLEN, false, lengths}, x, B, 0, z, stream);
 }
 
 // Stream slots: advance B distinct streams of the handle by one chunk each, every chunk with its own length, in one launch sequence.
 // The varlen row space with each utterance's history read from, and its new state written to, its stream's slot (ConvArgs::vl_slot).
 int adec_encode_streams(adec_handle* h, const float* x, const int* lengths, const int* streams, int B, float* z, void* stream) {
-    if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    if (h->cfg.model_type != ADEC_MODEL_SYMAD) return h->fail("encode_streams: not a symAD handle");
-    if (varlen_args(h, "encode_streams", lengths, B) || stream_args(h, "encode_streams", streams, B)) return 1;
-    DeviceGuard dg(h->device);
-    RunCtx rc{B, x, z, (cudaStream_t)stream, false, lengths, "encode_streams", streams};
-    return run_ops(h, h->enc_ops, rc, 1, nullptr);
+    return run_call(h, {false, CALL_SLOTS, false, lengths, streams}, x, B, 0, z, stream);
+}
+
+int adec_decode(adec_handle* h, const float* zq, int B, int F, float* y, void* stream) {
+    return run_call(h, {true, CALL_STREAM, false}, zq, B, F, y, stream);
+}
+
+int adec_decode_bf16(adec_handle* h, const uint16_t* zq, int B, int F, uint16_t* y, void* stream) {
+    return run_call(h, {true, CALL_STREAM, true}, zq, B, F, y, stream);
+}
+
+int adec_decode_offline(adec_handle* h, const float* zq, int B, int F, float* y, void* stream) {
+    return run_call(h, {true, CALL_OFFLINE, false}, zq, B, F, y, stream);
+}
+
+int adec_decode_offline_bf16(adec_handle* h, const uint16_t* zq, int B, int F, uint16_t* y, void* stream) {
+    return run_call(h, {true, CALL_OFFLINE, true}, zq, B, F, y, stream);
+}
+
+int adec_decode_offline_varlen(adec_handle* h, const float* zq, const int* frames, int B, float* y, void* stream) {
+    return run_call(h, {true, CALL_VARLEN, false, frames}, zq, B, 0, y, stream);
+}
+
+int adec_decode_offline_varlen_bf16(adec_handle* h, const uint16_t* zq, const int* frames, int B, uint16_t* y, void* stream) {
+    return run_call(h, {true, CALL_VARLEN, true, frames}, zq, B, 0, y, stream);
 }
 
 int adec_decode_streams(adec_handle* h, const float* zq, const int* frames, const int* streams, int B, float* y, void* stream) {
-    return decode_common(h, zq, B, 0, y, stream, false, false, true, frames, streams, true);
+    return run_call(h, {true, CALL_SLOTS, false, frames, streams}, zq, B, 0, y, stream);
 }
 
 int adec_decode_streams_bf16(adec_handle* h, const uint16_t* zq, const int* frames, const int* streams, int B, uint16_t* y, void* stream) {
-    return decode_common(h, zq, B, 0, y, stream, false, true, true, frames, streams, true);
+    return run_call(h, {true, CALL_SLOTS, true, frames, streams}, zq, B, 0, y, stream);
 }
 
 int adec_copy_stream_state(adec_handle* h, int src, const int* dst, int n, void* stream) {
@@ -1917,12 +1885,12 @@ static int run_single(adec_handle* h, Op& op, const void* x, int B, int Cin_real
     CK(h, cudaMemcpy(dx, xl.data(), xl.size(), cudaMemcpyHostToDevice));
     std::vector<Op> ops;
     ops.push_back(op);
-    RunCtx rc{B, dx, dy, 0, offline};
+    RunCtx rc{B, dx, dy, 0, offline ? CALL_OFFLINE : CALL_STREAM};
     if (run_ops(h, ops, rc, T, nullptr)) return 1;
     CK(h, cudaDeviceSynchronize());
     std::vector<char> yl(ybytes), sl(per * B * eb);
     CK(h, cudaMemcpy(yl.data(), dy, yl.size(), cudaMemcpyDeviceToHost));
-    CK(h, cudaMemcpy(sl.data(), ops[0].st[ops[0].cur], sl.size(), cudaMemcpyDeviceToHost));
+    CK(h, cudaMemcpy(sl.data(), ops[0].st[ops[0].cur ^ 1], sl.size(), cudaMemcpyDeviceToHost));     // the new state (run_ops)
     if (!convtr) {
         for (int b = 0; b < B; ++b)
             for (int g = 0; g < op.G; ++g)
@@ -1976,7 +1944,7 @@ int adec_test_residual_unit(int device, const float* x, int B, int C, int T, con
     W2.data.assign(w2, w2 + (size_t)C * C);
     Op op;
     int rc = make_ru_op(h, &op, "test_ru", W1, W2, dil, ACT_ELU);
-    if (!rc && h->use_tc && op.Cout > kTcMaxFuse) rc = h->fail("test_ru: C > 128 runs as two ops on the tensor-core path; test those separately");
+    if (!rc && h->engine != 0 && op.Cout > h->tc_max_fuse) rc = h->fail("test_ru: C > 128 runs as two ops on the tensor-core path; test those separately");
     if (!rc) rc = run_single(h, op, x, B, C, T, C, state, (K - 1) * dil, y, false, 1);
     if (rc) g_create_error = h->err;
     adec_destroy(h);

@@ -21,6 +21,7 @@ the class also runs on stand-ins in the CPU tests.
 from __future__ import annotations
 
 import collections
+import contextlib
 import threading
 import time
 from typing import Deque, Dict, List, Optional, Tuple
@@ -127,34 +128,7 @@ class MultiStreamCodecServer:
                     x_np[s, 0] = 0.0
                     self.stats[s].underruns += 1
         live = sum(t is not None for t in stamps)
-        with torch.no_grad():
-            x = x_host.to(dev, non_blocking=True)
-            z = self.tx_encoder.encode(x)                                       # utils/audiodec.py:100-102
-            if self.wire and hasattr(self.tx_encoder, "quantize_fused") and hasattr(self.rx_encoder, "lookup_packed"):
-                # the RVQ kernel writes the bitstream itself; the receiver looks the codewords up straight from the packed bytes
-                _, packed, _ = self.tx_encoder.quantize_fused(z, want_idx=False, want_packed=True, want_zq=False)
-                self.wire_bytes += packed.numel()
-                zq = self.rx_encoder.lookup_packed(packed)
-            elif self.wire:
-                packed = self.tx_encoder.pack(self.tx_encoder.quantize(z))
-                self.wire_bytes += packed.numel()
-                zq = self.rx_encoder.lookup(self.rx_encoder.unpack(packed))
-            else:
-                zq = self.rx_encoder.lookup(self.tx_encoder.quantize(z))
-            y = self.decoder.decode(zq).detach()                                # utils/audiodec.py:104-106
-            if y.device.type == "cuda":
-                # device -> PINNED host buffer (a pageable destination is staged through a driver bounce buffer), then one synchronise
-                if self._y_host is None or self._y_host.shape != y.shape:
-                    self._y_host = torch.empty(y.shape, dtype=y.dtype, pin_memory=True)
-                self._y_host.copy_(y, non_blocking=True)
-                torch.cuda.current_stream(y.device).synchronize()
-                y_host = self._y_host
-            else:
-                y_host = y
-        now = self._clock()
-        if y_host.dtype == torch.bfloat16:
-            y_host = y_host.float()             # a bf16-activation decoder: half the D2H bytes, widened here; frames out stay float32
-        y_all = y_host.numpy().reshape(self.n_streams, -1)[:, :self.frame_size].copy()    # one copy; the queues hold row views of it
+        y_all, now = self._codec_pass(x_host, dev)
         with self._lock:
             for s in range(self.n_streams):
                 t = stamps[s]
@@ -166,6 +140,46 @@ class MultiStreamCodecServer:
                 st.latencies.append(now - t)
         self.step_times.append(now - t0)
         return live
+
+    def _codec_pass(self, x_host, dev, streams=None, codec_lock=None):
+        """encode -> [wire] hand-off -> decode of the staged frames x_host (n, 1, frame_size), then the decoded frames back to the host.
+        streams: the slots the frames advance (encode_streams / decode_streams), or None for all streams in lock step.  codec_lock is
+        held while the codec runs.  Returns (decoded frames (n, frame_size) float32, the clock when they reached the host)."""
+        n = x_host.shape[0]
+        with torch.no_grad(), codec_lock or contextlib.nullcontext():
+            x = x_host.to(dev, non_blocking=True)
+            if streams is None:
+                z = self.tx_encoder.encode(x)                                   # utils/audiodec.py:100-102
+            else:
+                z, frames = self.tx_encoder.encode_streams(list(x.view(n, -1)), streams)
+            if self.wire and hasattr(self.tx_encoder, "quantize_fused") and hasattr(self.rx_encoder, "lookup_packed"):
+                # the RVQ kernel writes the bitstream itself; the receiver looks the codewords up straight from the packed bytes
+                _, packed, _ = self.tx_encoder.quantize_fused(z, want_idx=False, want_packed=True, want_zq=False)
+                self.wire_bytes += packed.numel()
+                zq = self.rx_encoder.lookup_packed(packed)
+            elif self.wire:
+                packed = self.tx_encoder.pack(self.tx_encoder.quantize(z))
+                self.wire_bytes += packed.numel()
+                zq = self.rx_encoder.lookup(self.rx_encoder.unpack(packed))
+            else:
+                zq = self.rx_encoder.lookup(self.tx_encoder.quantize(z))
+            if streams is None:
+                y = self.decoder.decode(zq).detach()                            # utils/audiodec.py:104-106
+            else:                           # every chunk is frame_size samples: equal frame counts
+                y = torch.cat([v.reshape(1, -1) for v in self.decoder.decode_streams(zq, frames, streams)]).detach()
+            if y.device.type == "cuda":
+                # device -> PINNED host buffer (a pageable destination is staged through a driver bounce buffer), then one synchronise
+                if self._y_host is None or self._y_host.shape != y.shape or self._y_host.dtype != y.dtype:
+                    self._y_host = torch.empty(y.shape, dtype=y.dtype, pin_memory=True)
+                self._y_host.copy_(y, non_blocking=True)
+                torch.cuda.current_stream(y.device).synchronize()
+                y_host = self._y_host
+            else:
+                y_host = y
+        now = self._clock()
+        if y_host.dtype == torch.bfloat16:
+            y_host = y_host.float()             # a bf16-activation decoder: half the D2H bytes, widened here; frames out stay float32
+        return y_host.numpy().reshape(n, -1)[:, :self.frame_size].copy(), now    # one copy; the queues hold row views of it
 
     # ------------------------------------------------------------------ real-time loop (the two worker threads of the reference, merged)
     def start(self, period: Optional[float] = None) -> None:
@@ -308,33 +322,7 @@ class SessionCodecServer(MultiStreamCodecServer):
         if n == 0:
             self.step_times.append(self._clock() - t0)
             return 0
-        with torch.no_grad(), self._codec_lock:
-            x = x_host[:n].to(dev, non_blocking=True).view(n, -1)
-            z, frames = self.tx_encoder.encode_streams(list(x), streams)
-            if self.wire and hasattr(self.tx_encoder, "quantize_fused") and hasattr(self.rx_encoder, "lookup_packed"):
-                _, packed, _ = self.tx_encoder.quantize_fused(z, want_idx=False, want_packed=True, want_zq=False)
-                self.wire_bytes += packed.numel()
-                zq = self.rx_encoder.lookup_packed(packed)
-            elif self.wire:
-                packed = self.tx_encoder.pack(self.tx_encoder.quantize(z))
-                self.wire_bytes += packed.numel()
-                zq = self.rx_encoder.lookup(self.rx_encoder.unpack(packed))
-            else:
-                zq = self.rx_encoder.lookup(self.tx_encoder.quantize(z))
-            ys = self.decoder.decode_streams(zq, frames, streams)
-            y = torch.cat([v.reshape(1, -1) for v in ys]).detach()        # every chunk is frame_size samples: equal frame counts
-            if y.device.type == "cuda":
-                if self._y_host is None or self._y_host.shape != y.shape or self._y_host.dtype != y.dtype:
-                    self._y_host = torch.empty(y.shape, dtype=y.dtype, pin_memory=True)
-                self._y_host.copy_(y, non_blocking=True)
-                torch.cuda.current_stream(y.device).synchronize()
-                y_host = self._y_host
-            else:
-                y_host = y
-        now = self._clock()
-        if y_host.dtype == torch.bfloat16:
-            y_host = y_host.float()
-        y_all = y_host.numpy().reshape(n, -1)[:, :self.frame_size].copy()
+        y_all, now = self._codec_pass(x_host[:n], dev, streams, self._codec_lock)
         with self._lock:
             for k, s in enumerate(streams):
                 if s not in self._open or self._session[s] != sessions[k]:
