@@ -16,9 +16,10 @@
  *   residual -= quantize                                      vq_module.py:143
  *
  * The orders above were found by probing torch on the build container and are pinned by
- * tests/test_oracle_golden.py::test_c_rvq_matches_torch (bit-exact distances on random data).
+ * tests/test_host_cpu.py::test_c_rvq_oracle_matches_torch_bitwise (bit-exact distances on random data).
+ * tests/test_rvq_spec_gpu.py holds rvq_kernel / lookup_kernel to this file with no tolerance.
  *
- * build: gcc -O2 -ffp-contract=off -shared -fPIC -o oracle/_build/librvq_oracle.so oracle/rvq_oracle.c -lm
+ * build (oracle/rvq_spec.py): gcc -O2 -ffp-contract=off -shared -fPIC -o oracle/_build/librvq_oracle.so oracle/rvq_oracle.c -lm
  */
 #include <math.h>
 #include <stdint.h>
@@ -60,21 +61,20 @@ void adec_oracle_codeword_norms(const float *embed, int d, int n, float *e2)
     }
 }
 
-/* x: (frames, D) residual input (modified copy kept internally); embeds: (nq, D, N);
- * idx out: (nq, frames) int64 flat (+ N*i); zq out (frames, D) = sum of quantize; dist_out optional
- * (nq, frames, N) for tests. */
-void adec_oracle_rvq(const float *x, int frames, int d, const float *embeds, int nq, int n,
-                     int64_t *idx, float *zq, float *dist_out)
+/* adec_oracle_rvq with the codeword norms given: e2s (nq, N).  With the norms of
+ * adec_oracle_codeword_norms this is the spec; tests pass other norms to model a host that sums
+ * them in another order. */
+void adec_oracle_rvq_e2(const float *x, int frames, int d, const float *embeds, const float *e2s,
+                        int nq, int n, int64_t *idx, float *zq, float *dist_out)
 {
     float *r = (float *)malloc(sizeof(float) * d);
-    float *e2 = (float *)malloc(sizeof(float) * n);
     float *qsum = (float *)malloc(sizeof(float) * d);
     for (int f = 0; f < frames; ++f) {
         memcpy(r, x + (size_t)f * d, sizeof(float) * d);
         for (int k = 0; k < d; ++k) qsum[k] = 0.f;
         for (int i = 0; i < nq; ++i) {
             const float *E = embeds + (size_t)i * d * n;
-            adec_oracle_codeword_norms(E, d, n, e2);
+            const float *e2 = e2s + (size_t)i * n;
             float x2 = sumsq_inner(r, d);
             int best = 0;
             float bestv = 0.f;
@@ -96,7 +96,19 @@ void adec_oracle_rvq(const float *x, int frames, int d, const float *embeds, int
         }
         if (zq) memcpy(zq + (size_t)f * d, qsum, sizeof(float) * d);
     }
-    free(r); free(e2); free(qsum);
+    free(r); free(qsum);
+}
+
+/* x: (frames, D) residual input (modified copy kept internally); embeds: (nq, D, N);
+ * idx out: (nq, frames) int64 flat (+ N*i); zq out (frames, D) = sum of quantize; dist_out optional
+ * (nq, frames, N) for tests. */
+void adec_oracle_rvq(const float *x, int frames, int d, const float *embeds, int nq, int n,
+                     int64_t *idx, float *zq, float *dist_out)
+{
+    float *e2s = (float *)malloc(sizeof(float) * (size_t)nq * n);
+    for (int i = 0; i < nq; ++i) adec_oracle_codeword_norms(embeds + (size_t)i * d * n, d, n, e2s + (size_t)i * n);
+    adec_oracle_rvq_e2(x, frames, d, embeds, e2s, nq, n, idx, zq, dist_out);
+    free(e2s);
 }
 
 /* lookup: zq[f] = sum_i codebook[idx[i][f]], codebook (nq*N, D), summed in i order (torch.sum dim 0) */

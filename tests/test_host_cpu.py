@@ -148,23 +148,13 @@ def test_c_rvq_oracle_matches_torch_bitwise():
     and decisions bit-for-bit on random data (the summation orders in its header were found by probing)."""
     import numpy as np
     from oracle import audiodec_oracle as O
-    so = os.path.join(REPO, "oracle", "_build", "librvq_oracle.so")
-    if not os.path.exists(so):
-        import __graft_entry__ as g
-        g.build()
-    lib = ctypes.CDLL(so)
+    from oracle import rvq_spec
     torch.manual_seed(5)
     nq, d, n, frames = 8, 64, 1024, 200
     embeds = [torch.randn(d, n) * 0.55 * 0.88 ** i for i in range(nq)]
     x = torch.randn(1, frames, d) * 0.6
     zq, idx = O.rvq_forward_index(x, embeds, True)
-    E = np.ascontiguousarray(torch.stack(embeds).numpy())
-    xi = np.ascontiguousarray(x[0].numpy())
-    oidx = np.zeros((nq, frames), np.int64)
-    ozq = np.zeros((frames, d), np.float32)
-    od = np.zeros((nq, frames, n), np.float32)
-    p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    lib.adec_oracle_rvq(p(xi), frames, d, p(E), nq, n, p(oidx), p(ozq), p(od))
+    oidx, ozq, od = rvq_spec.rvq_frames(x[0].numpy(), torch.stack(embeds).numpy(), dist=True)
     np.testing.assert_array_equal(oidx, idx.squeeze(1).numpy())
     fl = x.reshape(-1, d)
     dist0 = fl.pow(2).sum(1, keepdim=True) - 2 * fl @ embeds[0] + embeds[0].pow(2).sum(0, keepdim=True)

@@ -138,14 +138,19 @@ def test_v1_vocoder_bf16_mode(golden_dir, symad_sd, hifigan_sd):
 
 
 def test_quantize_bit_exact_vs_oracle_same_z(symad_sd):
-    """Given the SAME z, the CUDA RVQ reproduces torch-CPU's decisions: compare 64x160 frames x 8 stages."""
+    """Given the SAME z, the CUDA RVQ reproduces torch-CPU's decisions: compare 64x160 frames x 8 stages.  It also equals the
+    C spec (oracle/rvq_oracle.c) on every one of the 81 920 decisions with no tolerance: that comparison does not rest on the
+    CPU's MKL summation order, which the torch comparison below does."""
     from oracle import audiodec_oracle as O
+    from oracle import rvq_spec
     tx, rx, dec, _ = _codec(symad_sd)
     torch.manual_seed(3)
     z = 0.6 * torch.randn(64, 64, 160)
     orc = O.SymADOracle(S.SYMAD_PARAMS, symad_sd)
     ridx, margins = orc.quantize(z, return_margins=True)
     idx = tx.quantize(z.cuda()).cpu()
+    sidx, _ = rvq_spec.quantize(z.numpy(), torch.stack(orc.embeds).numpy())
+    np.testing.assert_array_equal(idx.numpy(), sidx)
     bad = (idx != ridx)
     # a differing decision is only tolerated on a numerical tie of the reference itself
     assert bad.sum().item() == 0 or margins[bad].max().item() < 1e-6, f"{bad.sum().item()} mismatches"
