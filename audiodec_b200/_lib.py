@@ -55,6 +55,8 @@ SYMBOLS = {
     "adec_encode": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "adec_quantize": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "adec_quantize_ex": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "adec_quantize_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "adec_zq_moments": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), c_int, c_void_p, c_void_p, c_void_p]),
     "adec_lookup": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "adec_lookup_packed": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "adec_decode": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),

@@ -466,6 +466,38 @@ class SymADStreamGenerator(_StreamGeneratorBase):
         _check(self._lib.adec_lookup(self._h, _ptr(idx), b, f, _ptr(zq), self._stream()), self._h)
         return zq.transpose(1, 2), idx
 
+    def quantize_forward(self, z):
+        """z (B,code_dim,F) -> (zq (B,code_dim,F) channels-first, idx (Nq,B,F)): Quantizer.forward's zq (quantizer.py:31-34), the
+        sum over stages of r + (e - r) from 0. (vq_module.py:136-143), in one launch.  The indices equal quantize(); zq can differ from
+        quantize_offline's codeword sum in the last bits.  The channels-last storage behind zq is what zq_moments reads."""
+        self._ready()
+        self._want(z, "quantize_forward", 1, self.code_dim)
+        z = self._in(z)
+        b, _, f = z.shape
+        idx = torch.empty(self.codebook_num, b, f, device=self._device, dtype=torch.int64)
+        zq = torch.empty(b, f, self.code_dim, device=self._device, dtype=torch.float32)
+        _check(self._lib.adec_quantize_forward(self._h, _ptr(z), b, f, _ptr(idx), _ptr(zq), self._stream()), self._h)
+        return zq.transpose(1, 2), idx
+
+    def zq_moments(self, zq, frames):
+        """Per-utterance moments of a varlen zq: zq (1, code_dim, sum F_b) as quantize_forward returns it for encode_offline_varlen's
+        z (channels-last storage), or (sum F_b, code_dim) channels-last; utterance b holds frames[b] rows.  Returns fp64 device
+        tensors (sum (B, code_dim), m2 (B, code_dim)): sum_f x and the corrected centred sum_f (x - T)^2 - (sum_f (x - T))^2 / F_b,
+        T = sum / F_b, what StandardScaler.partial_fit computes for one utterance.  Deterministic, and independent of the batch
+        around an utterance."""
+        self._ready()
+        if zq.dim() == 3 and zq.size(0) == 1 and zq.size(1) == self.code_dim:
+            zq = zq[0].transpose(0, 1)                     # (sum F, D): a view of quantize_forward's channels-last storage
+        if zq.dim() != 2 or zq.size(1) != self.code_dim:
+            raise RuntimeError(f"audiodec_b200: zq_moments: expected (1, {self.code_dim}, F) or (F, {self.code_dim}), got {tuple(zq.shape)}")
+        zq = self._in(zq)
+        arr, b = _int_array(frames)
+        if sum(int(f) for f in frames) != zq.size(0):
+            raise RuntimeError(f"audiodec_b200: zq_moments: frames add up to {sum(int(f) for f in frames)}, zq has {zq.size(0)} rows")
+        out = torch.empty(2, b, self.code_dim, device=self._device, dtype=torch.float64)
+        _check(self._lib.adec_zq_moments(self._h, _ptr(zq), arr, b, _ptr(out[0]), _ptr(out[1]), self._stream()), self._h)
+        return out[0], out[1]
+
     def decode_offline(self, zq):
         """zq (B,code_dim,F) channels-first (what Decoder.forward takes, decoder.py:135-140) -> y (B,1,F*hop); transposed convs
         replicate their first input frame (conv_layer.py:189-192)."""

@@ -256,6 +256,7 @@ struct adec_handle {
     // host-path scratch
     DevBuf hx, hz, hzq, hy;
     DevBuf vl_tab;                // varlen row tables of the last call (ints)
+    DevBuf mom_tab;               // row offsets of the last adec_zq_moments call (ints)
     SlotBits enc_slots, dec_slots;
     DevBuf slot_tab;              // stream pairs of the last state copy (ints)
     long long* hidx = nullptr;
@@ -1294,7 +1295,7 @@ void adec_destroy(adec_handle* h) {
         for (Op& op : *ops)
             for (int i = 0; i < 2; ++i) if (op.st[i]) cudaFree(op.st[i]);
     for (auto& b : h->ws) if (b.p) cudaFree(b.p);
-    for (DevBuf* b : {&h->hx, &h->hz, &h->hzq, &h->hy, &h->vl_tab, &h->slot_tab}) if (b->p) cudaFree(b->p);
+    for (DevBuf* b : {&h->hx, &h->hz, &h->hzq, &h->hy, &h->vl_tab, &h->mom_tab, &h->slot_tab}) if (b->p) cudaFree(b->p);
     if (h->hidx) cudaFree(h->hidx);
     if (h->d_err) cudaFree(h->d_err);
     if (h->d_ktrace) cudaFree(h->d_ktrace);
@@ -1581,10 +1582,10 @@ int adec_packed_frame_bytes(const adec_handle* h) {
 }
 
 // residual VQ launch: pick frames-per-pass FP and passes per block so that the grid is ONE wave with the smallest idle tail
-extern "C++" template <int FP>
+extern "C++" template <int FP, bool FWD>
 cudaError_t launch_rvq(const adec_handle* h, RvqArgs a, cudaStream_t s, int* cost) {
     static int per_sm[64] = {0};
-    auto kern = rvq_kernel<64, 4, FP>;
+    auto kern = rvq_kernel<64, 4, FP, FWD>;
     const int dev = h->device;
     const auto smem_of = [&](int n_pass) { const int FR = n_pass * FP; return (size_t)FR * (3 * 64 + 1 + 2 * (RVQ_THREADS / 32) + a.nq) * 4; };
     if (dev < 64 && !per_sm[dev]) {
@@ -1603,7 +1604,18 @@ cudaError_t launch_rvq(const adec_handle* h, RvqArgs a, cudaStream_t s, int* cos
     return cudaGetLastError();
 }
 
-int adec_quantize_ex(adec_handle* h, const float* z, int B, int F, int64_t* idx, uint8_t* packed, float* zq, void* stream) {
+extern "C++" template <bool FWD>
+cudaError_t launch_rvq_best(const adec_handle* h, const RvqArgs& a, cudaStream_t s) {
+    int c16 = 0, c12 = 0, c8 = 0;
+    launch_rvq<16, FWD>(h, a, nullptr, &c16); launch_rvq<12, FWD>(h, a, nullptr, &c12); launch_rvq<8, FWD>(h, a, nullptr, &c8);
+    return (c12 <= c16 && c12 <= c8) ? launch_rvq<12, FWD>(h, a, s, nullptr)
+         : (c16 <= c8)               ? launch_rvq<16, FWD>(h, a, s, nullptr)
+                                     : launch_rvq<8, FWD>(h, a, s, nullptr);
+}
+
+// fwd: zq receives ResidualVQ.forward's sum instead of lookup's (rvq_kernel's FWD)
+static int quantize_common(adec_handle* h, const float* z, int B, int F, int64_t* idx, uint8_t* packed, float* zq, bool fwd,
+                           void* stream) {
     if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
     if (h->cfg.model_type != ADEC_MODEL_SYMAD) return h->fail("quantize: not a symAD handle");
     if (B < 1 || F < 1) return h->fail("quantize: empty input");
@@ -1612,13 +1624,44 @@ int adec_quantize_ex(adec_handle* h, const float* z, int B, int F, int64_t* idx,
     RvqArgs a{};
     a.z = z; a.B = B; a.F = F; a.nq = h->cfg.codebook_num; a.embed = h->d_embed; a.e2 = h->d_e2; a.idx = (long long*)idx;
     a.packed = packed; a.zq = zq; a.bits = index_bits(h->cfg.codebook_size); a.bpf = adec_packed_frame_bytes(h);
-    int c16 = 0, c12 = 0, c8 = 0;
-    launch_rvq<16>(h, a, nullptr, &c16); launch_rvq<12>(h, a, nullptr, &c12); launch_rvq<8>(h, a, nullptr, &c8);
-    cudaError_t e = (c12 <= c16 && c12 <= c8) ? launch_rvq<12>(h, a, (cudaStream_t)stream, nullptr)
-                  : (c16 <= c8)               ? launch_rvq<16>(h, a, (cudaStream_t)stream, nullptr)
-                                              : launch_rvq<8>(h, a, (cudaStream_t)stream, nullptr);
+    const cudaError_t e = fwd ? launch_rvq_best<true>(h, a, (cudaStream_t)stream) : launch_rvq_best<false>(h, a, (cudaStream_t)stream);
     if (e != cudaSuccess) return h->fail(fmt("launch of rvq_kernel failed: %s", cudaGetErrorString(e)));
     ++h->launches;
+    return 0;
+}
+
+int adec_quantize_ex(adec_handle* h, const float* z, int B, int F, int64_t* idx, uint8_t* packed, float* zq, void* stream) {
+    return quantize_common(h, z, B, F, idx, packed, zq, false, stream);
+}
+
+int adec_quantize_forward(adec_handle* h, const float* z, int B, int F, int64_t* idx, float* zq_fwd, void* stream) {
+    if (h && !zq_fwd) return h->fail("quantize_forward: zq_fwd is NULL");
+    return quantize_common(h, z, B, F, idx, nullptr, zq_fwd, true, stream);
+}
+
+int adec_zq_moments(adec_handle* h, const float* zq, const int* frames, int B, double* sum, double* m2, void* stream) {
+    if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
+    if (h->cfg.model_type != ADEC_MODEL_SYMAD) return h->fail("zq_moments: not a symAD handle");
+    if (varlen_args(h, "zq_moments", frames, B)) return 1;
+    if (!zq || !sum || !m2) return h->fail("zq_moments: zq, sum and m2 must be given");
+    if ((uintptr_t)zq % 16) return h->fail("zq_moments: zq must be 16-byte aligned");
+    std::vector<int> off(B + 1, 0);
+    long long rows = 0;
+    for (int b = 0; b < B; ++b) {
+        rows += frames[b];
+        if (rows > INT32_MAX) return h->fail(fmt("zq_moments: the batch has more than 2^31 - 1 rows; split it"));
+        off[b + 1] = (int)rows;
+    }
+    DeviceGuard dg(h->device);
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (ensure(h, h->mom_tab, off.size())) return 1;
+    CK(h, cudaMemcpyAsync(h->mom_tab.p, off.data(), off.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    MomArgs a{zq, reinterpret_cast<const int*>(h->mom_tab.p), sum, m2};
+    zq_moments_kernel<false><<<B, MOM_THREADS, 0, s>>>(a);
+    CK(h, cudaGetLastError());
+    zq_moments_kernel<true><<<B, MOM_THREADS, 0, s>>>(a);
+    CK(h, cudaGetLastError());
+    h->launches += 2;
     return 0;
 }
 

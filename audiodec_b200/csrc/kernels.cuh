@@ -19,6 +19,7 @@
 //   rvq_kernel        - 8-stage residual VQ: fp32 distances in the reference's rounding order,
 //                       first-index arg-min by warp shuffles, int64 flat indices.
 //   lookup_kernel     - codebook gather-sum.
+//   zq_moments_kernel - per-utterance fp64 sums and centred second moments of zq (corpus statistics).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -695,7 +696,8 @@ struct RvqArgs {
     long long* idx;        // (nq, B, F) flat indices (+ N*i), or nullptr
     // fused outputs (SURVEY.md 8(f) rank 2; bin/stream.py:224 hand-off): either may be nullptr
     unsigned char* packed; // (B*F, bpf) index bitstream, same format as pack_kernel
-    float* zq;             // (B*F, D) = lookup(idx) (vq_module.py:159-161), so that quantize can hand zq straight to the decoder
+    float* zq;             // (B*F, D) = lookup(idx) (vq_module.py:159-161), so that quantize can hand zq straight to the decoder;
+                           //          with FWD the forward sum instead
     int bits, bpf, n_pass; // bits per index, bytes per packed frame, frame passes per block (frames per block = n_pass * FP)
 };
 
@@ -706,7 +708,9 @@ constexpr int RVQ_THREADS = 256;
 // what makes the indices bit-identical to torch-CPU), codeword elements streamed from L2 (the 256 KB stage table is shared by all
 // blocks), residuals broadcast from shared memory.  The host picks (FP, n_pass) so that the grid is one wave with the least idle
 // tail (adec_quantize), which alone took the 64 x 160-frame case from 0.58 ms (320 blocks of 32 frames = 1.08 waves) to one wave.
-template <int D, int NPT, int FP>   // codebook size N = RVQ_THREADS * NPT
+// FWD: zq accumulates ResidualVQ.forward's quantized_out, the sum of r + (e - r) from 0. (vq_module.py:136-143), instead of
+// lookup's sum of the codewords; shared memory, grid and every other output are the same.
+template <int D, int NPT, int FP, bool FWD>   // codebook size N = RVQ_THREADS * NPT
 __global__ void __launch_bounds__(RVQ_THREADS) rvq_kernel(const RvqArgs a) {
     constexpr int N = RVQ_THREADS * NPT, NW = RVQ_THREADS / 32;
     static_assert(D % 32 == 0 && FP % 4 == 0, "D must be a multiple of 32, FP of 4");
@@ -841,7 +845,8 @@ __global__ void __launch_bounds__(RVQ_THREADS) rvq_kernel(const RvqArgs a) {
             const float rn = __fsub_rn(rv, qq);
             r[i] = rn;
             r2[i] = 2.0f * rn;
-            zq[i] = st == 0 ? q : __fadd_rn(zq[i], q);
+            if (FWD) zq[i] = __fadd_rn(zq[i], qq);                 // stage 0 adds to the 0.f stored above: a -0 comes out +0
+            else zq[i] = st == 0 ? q : __fadd_rn(zq[i], q);
         }
         __syncthreads();
     }
@@ -909,6 +914,77 @@ __global__ void __launch_bounds__(256) lookup_kernel(const LookupArgs a) {
         else { s.x = __fadd_rn(s.x, v.x); s.y = __fadd_rn(s.y, v.y); s.z = __fadd_rn(s.z, v.z); s.w = __fadd_rn(s.w, v.w); }
     }
     *reinterpret_cast<float4*>(a.zq + fr * a.D + k4) = s;
+}
+
+// Per-utterance moments of the quantizer output (codecStatistic.py:104-105 calls StandardScaler.partial_fit once per file), fp64
+// throughout (fp32 values widen exactly).  Over utterance b's rows [off[b], off[b + 1]) of zq (rows, 64) channels-last:
+//   CENTRED = false:  sum[b][c] = sum_f x
+//   CENTRED = true:   with T = sum[b][c] / n,  m2[b][c] = sum_f (x - T)^2 - (sum_f (x - T))^2 / n   (sklearn's corrected two-pass term)
+// One block per utterance.  Its rows are cut into segments of MOM_SEG rows counted from the utterance's first row; thread (j, q) adds
+// rows j, j + 16, ... of a segment for channels 4q .. 4q + 3 in ascending order, the 16 row partials of a segment are added in row
+// order, and the segment totals in segment order.  No atomics: an utterance's result depends on its own rows only, not on where it
+// sits in the batch or what surrounds it.
+constexpr int MOM_THREADS = 256, MOM_D = 64, MOM_Q = MOM_D / 4, MOM_ROWS = MOM_THREADS / MOM_Q, MOM_SEG = 256;
+
+struct MomArgs {
+    const float* zq;   // (off[B], 64), 16-byte aligned
+    const int* off;    // (B + 1) row offsets
+    double* sum;       // (B, 64): written by the first launch, read by the second
+    double* m2;        // (B, 64)
+};
+
+template <bool CENTRED>
+__global__ void __launch_bounds__(MOM_THREADS) zq_moments_kernel(const MomArgs a) {
+    __shared__ double part[CENTRED ? 2 : 1][MOM_ROWS][MOM_D];
+    const int b = blockIdx.x, tid = threadIdx.x, q = tid % MOM_Q, j = tid / MOM_Q;
+    const int r0 = __ldg(a.off + b), n = __ldg(a.off + b + 1) - r0;
+    const float* x = a.zq + (long long)r0 * MOM_D + 4 * q;
+    double t[4] = {0.0, 0.0, 0.0, 0.0};
+    if (CENTRED)
+#pragma unroll
+        for (int k = 0; k < 4; ++k) t[k] = a.sum[(long long)b * MOM_D + 4 * q + k] / (double)n;
+    double tot1 = 0.0, tot2 = 0.0;            // threads c < 64: the running totals of channel c
+    for (int s0 = 0; s0 < n; s0 += MOM_SEG) {
+        double s1[4] = {0.0, 0.0, 0.0, 0.0}, s2[4] = {0.0, 0.0, 0.0, 0.0};
+#pragma unroll
+        for (int i = 0; i < MOM_SEG / MOM_ROWS; ++i) {
+            const int f = s0 + j + i * MOM_ROWS;
+            if (f < n) {
+                const float4 v = __ldg(reinterpret_cast<const float4*>(x + (long long)f * MOM_D));
+                const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    if (CENTRED) {
+                        const double d = __dsub_rn((double)vv[k], t[k]);
+                        s1[k] = __dadd_rn(s1[k], d);
+                        s2[k] = __dadd_rn(s2[k], __dmul_rn(d, d));     // the square rounded, then added (numpy's temp **= 2; sum)
+                    } else {
+                        s1[k] = __dadd_rn(s1[k], (double)vv[k]);
+                    }
+                }
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            part[0][j][4 * q + k] = s1[k];
+            if (CENTRED) part[CENTRED ? 1 : 0][j][4 * q + k] = s2[k];
+        }
+        __syncthreads();
+        if (tid < MOM_D) {
+            double p1 = part[0][0][tid], p2 = CENTRED ? part[CENTRED ? 1 : 0][0][tid] : 0.0;
+            for (int r = 1; r < MOM_ROWS; ++r) {
+                p1 = __dadd_rn(p1, part[0][r][tid]);
+                if (CENTRED) p2 = __dadd_rn(p2, part[CENTRED ? 1 : 0][r][tid]);
+            }
+            tot1 = __dadd_rn(tot1, p1);
+            tot2 = __dadd_rn(tot2, p2);
+        }
+        __syncthreads();
+    }
+    if (tid < MOM_D) {
+        if (CENTRED) a.m2[(long long)b * MOM_D + tid] = __dsub_rn(tot2, __ddiv_rn(__dmul_rn(tot1, tot1), (double)n));
+        else a.sum[(long long)b * MOM_D + tid] = tot1;
+    }
 }
 
 // Index bitstream (SURVEY.md 8(f) rank 2).  The reference has no wire format: it ships int64 (Nq,F) tensors through a queue

@@ -213,6 +213,31 @@ def write_checkpoint(root, kind, tag, steps, model_type, params, sd, sampling_ra
     return path
 
 
+def make_wav_corpus(root, seed, lengths, sr=48000):
+    """Write len(lengths) mono PCM16 wav files of lengths[i] samples under ``root``, spread over nested folders
+    (``spk<i % 3>/[sess<i % 2>/]utt_<i>.wav``), from nothing but the seed: band-limited noise with a per-file level and a
+    per-file DC offset, so that every code channel has a mean and a spread.  Returns the paths in the order of ``lengths``."""
+    import numpy as np
+    from scipy.io import wavfile
+    rng = np.random.default_rng(seed)
+    paths = []
+    for i, n in enumerate(lengths):
+        d = os.path.join(root, f"spk{i % 3}", f"sess{i % 2}") if i % 4 else os.path.join(root, f"spk{i % 3}")
+        os.makedirs(d, exist_ok=True)
+        level, dc = 0.05 + 0.25 * rng.random(), 0.02 * rng.standard_normal()
+        # brown noise minus its trailing 64-sample mean; cumulative sums and element-wise arithmetic only (no BLAS, whose
+        # summation order depends on the CPU), so the bytes are the same on every machine
+        x = np.cumsum(rng.standard_normal(int(n))) * 0.05
+        c = np.concatenate([np.zeros(64), np.cumsum(x)])
+        x = x - (c[64:] - c[:-64]) / 64.0
+        x = level * x / max(1e-9, np.abs(x).max()) + dc
+        pcm = np.clip(np.rint(x * 32767.0), -32768, 32767).astype(np.int16)
+        p = os.path.join(d, f"utt_{i:04d}.wav")
+        wavfile.write(p, int(sr), pcm)
+        paths.append(p)
+    return paths
+
+
 def make_model_zoo(root, model="vctk_sym", seed=0):
     """Create the synthetic checkpoint tree for one ``assign_model`` name under ``root``.
     Returns (sample_rate, encoder_checkpoint, decoder_checkpoint) as absolute paths."""

@@ -105,6 +105,17 @@ int adec_quantize(adec_handle *h, const float *z, int B, int F, int64_t *idx, vo
  * writes any of idx (Nq,B,F) int64, packed (B,F,adec_packed_frame_bytes) uint8 and zq (B,F,code_dim) = lookup(idx); pass NULL for
  * outputs that are not wanted (at least one must be given).  Same arithmetic, bit-identical to quantize + pack + lookup. */
 int adec_quantize_ex(adec_handle *h, const float *z, int B, int F, int64_t *idx, uint8_t *packed, float *zq, void *stream);
+/* Quantizer.forward's zq (quantizer.py:31-34, what codecStatistic.py:92-98 fits its statistics to): ONE launch writes
+ * zq_fwd (B,F,code_dim) channels-last = ResidualVQ.forward's quantized_out, the sum over stages of r + (e - r) starting from 0.
+ * (vq_module.py:136-143; a -0 comes out +0), and idx (Nq,B,F) int64 unless it is NULL.  The indices are those of adec_quantize;
+ * zq_fwd may differ from lookup's sum of the codewords in the last bits. */
+int adec_quantize_forward(adec_handle *h, const float *z, int B, int F, int64_t *idx, float *zq_fwd, void *stream);
+/* Per-utterance moments of a varlen zq (sum F_b, code_dim) channels-last fp32, 16-byte aligned, as adec_quantize_forward writes it
+ * for the varlen z: utterance b's rows are [sum_{i<b} F_i, +F_b).  frames: HOST array of B frame counts (>= 1), the row count must
+ * fit in 31 bits.  Writes, per utterance and channel, fp64 sum (B,code_dim) = sum_f x and m2 (B,code_dim) = sum_f (x - T)^2 -
+ * (sum_f (x - T))^2 / F_b with T = sum / F_b (the corrected two-pass term StandardScaler.partial_fit computes per call).  Two
+ * launches, no host synchronise; deterministic, and an utterance's result does not depend on its place in the batch. */
+int adec_zq_moments(adec_handle *h, const float *zq, const int *frames, int B, double *sum, double *m2, void *stream);
 /* StreamGenerator.lookup (AudioDec.py:242-243): idx (Nq,B,F) -> zq (B,F,code_dim). Stateless. */
 int adec_lookup(adec_handle *h, const int64_t *idx, int B, int F, float *zq, void *stream);
 /* StreamGenerator.decode (AudioDec.py:246-247 / HiFiGAN.py:268-273): zq (B,F,code_dim) -> y (B,1,F*hop). */
