@@ -42,6 +42,19 @@ class AdecConfig(ctypes.Structure):
 
 MODEL_SYMAD, MODEL_HIFIGAN = 0, 1
 
+
+class AdecTestOp(ctypes.Structure):
+    """struct adec_test_op (include/audiodec_b200.h)."""
+    _fields_ = [
+        ("kind", c_int), ("Cin", c_int), ("Cout", c_int), ("K", c_int), ("stride", c_int), ("dil", c_int), ("groups", c_int),
+        ("shared_in", c_int), ("pre_act", c_int), ("slope", c_float), ("out_nct", c_int), ("post_tanh", c_int),
+        ("w", c_void_p), ("w2", c_void_p), ("bias", c_void_p), ("mean", c_void_p), ("scale", c_void_p),
+    ]
+
+
+TEST_CONV, TEST_RU, TEST_CONVTR, TEST_STEM, TEST_HEAD = 0, 1, 2, 3, 4
+TEST_REC = 8
+
 # name -> (restype, argtypes); every symbol include/audiodec_b200.h declares
 SYMBOLS = {
     "adec_create": (c_int, [ctypes.POINTER(AdecConfig), c_int, ctypes.POINTER(c_void_p)]),
@@ -92,6 +105,11 @@ SYMBOLS = {
                                         c_void_p, c_void_p]),
     "adec_test_vocoder_layer": (c_int, [c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                         c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "adec_test_conv_op": (c_int, [c_int, ctypes.POINTER(AdecTestOp), c_int, c_int, c_int, c_int, ctypes.POINTER(c_int),
+                                  ctypes.POINTER(c_int), c_void_p, c_void_p, c_void_p, c_void_p, ctypes.POINTER(c_int), c_int,
+                                  ctypes.POINTER(c_int)]),
+    "adec_record_launches": (c_int, [c_void_p, c_int]),
+    "adec_launch_records": (c_int, [c_void_p, ctypes.POINTER(c_int), c_int]),
 }
 
 _lib = None

@@ -261,6 +261,8 @@ struct adec_handle {
     DevBuf slot_tab;              // stream pairs of the last state copy (ints)
     long long* hidx = nullptr;
     size_t hidx_cap = 0;
+    std::vector<int>* launch_log = nullptr;   // run_ops appends one ADEC_TEST_REC record per launch here (adec_record_launches)
+    std::vector<int> launch_rec;
 
     int fail(const std::string& m) { err = m; return 1; }
 };
@@ -850,12 +852,20 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
                 a.n_wbuf = op.tc->n_wbuf(wrows, op.fuse, pair);
                 if (a.n_wbuf < 1) return h->fail(fmt("%s: window of %d rows does not fit in shared memory", op.name.c_str(), wrows));
                 e = (vl ? op.tc->pfn_vl : pair ? op.tc->pfn_pair : op.tc->pfn)(a, (int)grid.x, (int)grid.y, (int)n_tiles, n_ctas, (int)psmem, rc.stream);
+                if (h->launch_log)
+                    h->launch_log->insert(h->launch_log->end(), {ADEC_TEST_LAUNCH_TC, op.tc->NT, op.tc->fuse, op.tc->pre, op.tc->prec, vl, pair,
+                                                                 a.stack_L > 0});
             } else {
                 const int TT = op.kc->TT;
                 dim3 grid((Tout + TT - 1) / TT, op.G * op.n_co_tiles, rc.B);
                 e = op.kc->fn(a, grid, TT + (op.Ktaps - 1) * op.dil, rc.stream);
+                if (h->launch_log)
+                    h->launch_log->insert(h->launch_log->end(), {ADEC_TEST_LAUNCH_FFMA, op.kc->CO, op.kc->fuse, op.pre_act, 0, 0, 0, 0});
             }
         }
+        if (h->launch_log && op.kind != OP_CONV)
+            h->launch_log->insert(h->launch_log->end(), {op.kind == OP_STEM ? ADEC_TEST_LAUNCH_STEM : ADEC_TEST_LAUNCH_HEAD, 0, 0, op.pre_act,
+                                                         0, vl, 0, 0});
         if (e != cudaSuccess) return h->fail(fmt("launch of %s failed: %s", op.name.c_str(), cudaGetErrorString(e)));
         ++h->launches;
         if (h->profiling) {
@@ -1853,6 +1863,20 @@ int adec_test_wgmma_columns(int device, const void* a, const void* b, float* d64
     return 0;
 }
 
+int adec_record_launches(adec_handle* h, int enable) {
+    if (!h) return 1;
+    h->launch_rec.clear();
+    h->launch_log = enable ? &h->launch_rec : nullptr;
+    return 0;
+}
+
+int adec_launch_records(const adec_handle* h, int* out, int max_records) {
+    if (!h || (max_records > 0 && !out)) return -1;
+    const int n = (int)h->launch_rec.size() / ADEC_TEST_REC;
+    std::copy(h->launch_rec.begin(), h->launch_rec.begin() + (size_t)std::min(n, std::max(max_records, 0)) * ADEC_TEST_REC, out);
+    return n;
+}
+
 int adec_profile(adec_handle* h, int enable) {
     if (!h) return 1;
     for (auto& ev : h->prof_events) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
@@ -1879,81 +1903,153 @@ int adec_profile_report(adec_handle* h, char* buf, int buf_len) {
 // -------------------------------------------------------------------------------------------------
 // single-layer entry points for the unit tests (HOST pointers, reference layouts)
 // -------------------------------------------------------------------------------------------------
-// Elements are h->act_bytes() wide: fp32, or bf16 words for a compute_dtype 2 handle.  x (B, Cin_real, T) and state (B, Cin_real, P_real)
-// channels-first (Cin_real: the channels x holds, i.e. those of one group when the op has shared_in); res (B, Cout_real_total, Tout) or
-// nullptr, added after the bias from a workspace buffer as the model wires it.  offline: Generator.forward (zero history, first-row
-// replication in transposed convs); state is neither read nor written and may be nullptr.
-static int run_single(adec_handle* h, Op& op, const void* x, int B, int Cin_real, int T, int Cout_real_total, void* state, int P_real,
-                      void* y, bool convtr, int stride, const void* res = nullptr, bool offline = false) {
+// One test's op list (one op, or the two launches of a split residual unit) and its host I/O.  Elements are h->act_bytes() wide: fp32,
+// or bf16 words for a compute_dtype 2 handle.  Layouts as adec_test_conv_op documents them.
+struct TestIO {
+    CallMode mode = CALL_STREAM;
+    int n_calls = 1, B = 1, n_streams = 1;
+    const int* lengths = nullptr;   // (n_calls, B)
+    const int* streams = nullptr;   // (n_calls, B), CALL_SLOTS
+    const void* x = nullptr;
+    const void* res = nullptr;
+    void* state = nullptr;
+    void* y = nullptr;
+    int Cin_x = 0;                  // channels of x and state
+    int Cout_total = 0;             // output channels (all groups; a transposed conv's per output row)
+};
+
+// Runs `ops` (built, not finalized) as the decoder list of `h`, through run_call: the codec's own call path, slot bits and state
+// buffers.  x and res go from channels-first to the channels-last row spaces the kernels read (utterance after utterance; uniform
+// calls are the same rows), and y and state come back the other way.
+static int run_test_ops(adec_handle* h, std::vector<Op> ops, const TestIO& io) {
     const size_t eb = h->act_bytes();
     auto put = [eb](void* dst, size_t i, const void* src, size_t j) { memcpy((char*)dst + i * eb, (const char*)src + j * eb, eb); };
-    // x (B, Cin_total, T) channels-first -> channels-last with per-group channel padding
-    const int G = op.shared_in ? 1 : op.G;
-    const int cin_g = Cin_real / G, ldx = G * op.Cin;
-    std::vector<char> xl((size_t)B * T * ldx * eb, 0);
-    for (int b = 0; b < B; ++b)
-        for (int g = 0; g < G; ++g)
-            for (int c = 0; c < cin_g; ++c)
-                for (int t = 0; t < T; ++t) put(xl.data(), ((size_t)b * T + t) * ldx + g * op.Cin + c, x, ((size_t)b * Cin_real + g * cin_g + c) * T + t);
-    const size_t per = (size_t)op.P * op.st_C;
-    std::vector<char> hs(per * B * eb, 0);
-    if (!offline)
-        for (int b = 0; b < B; ++b)
+    const bool vl = io.mode == CALL_VARLEN || io.mode == CALL_SLOTS;
+    const bool split = ops.size() == 2;
+    {   // wiring: x in EXT_IN (split unit: workspace 2, which is also its skip input), y to EXT_OUT, a conv's residual in workspace 0
+        Op& f = ops.front();
+        Op& l = ops.back();
+        const int ldx = (f.shared_in ? 1 : f.G) * f.Cin;
+        f.in_buf = split ? 2 : BUF_EXT_IN; f.ldx = ldx; f.x_goff = f.shared_in ? 0 : f.Cin;
+        if (split) {
+            f.out_buf = 1; f.ldy = f.Cout; f.y_goff = f.Cout;
+            l.in_buf = 1; l.ldx = f.Cout; l.x_goff = l.Cin;
+            l.res_buf = 2; l.ldr = ldx; l.r_goff = 0;
+        }
+        l.out_buf = BUF_EXT_OUT; l.ldy = l.G * l.Cout; l.y_goff = l.Cout;
+        if (io.res) { l.res_buf = 0; l.ldr = l.ldy; l.r_goff = l.Cout; }
+    }
+    for (Op& op : ops)
+        if (finalize_op(h, &op)) return 1;
+    h->dec_ops = std::move(ops);        // the handle owns the state buffers from here (adec_destroy)
+    for (Op& op : h->dec_ops)
+        if (alloc_state(h, &op, io.n_streams)) return 1;
+    h->n_streams = h->st_cap = io.n_streams;
+    h->dec_slots.bit.assign(io.n_streams, 0);
+    h->finalized = true;
+    const Op& f = h->dec_ops.front();
+    const Op& l = h->dec_ops.back();
+    const int G = f.shared_in ? 1 : f.G, cin_g = io.Cin_x / G;
+    const int cout_g = io.Cout_total / l.G, up = l.up;
+    const size_t per = (size_t)f.P * f.st_C;
+    if (per && io.state && io.mode != CALL_VARLEN) {
+        std::vector<char> hs(per * io.n_streams * eb, 0);
+        for (int s = 0; s < io.n_streams; ++s)
             for (int g = 0; g < G; ++g)
                 for (int c = 0; c < cin_g; ++c)
-                    for (int p = 0; p < P_real; ++p)
-                        put(hs.data(), ((size_t)b * op.P + p) * op.st_C + g * op.Cin + c, state, ((size_t)b * Cin_real + g * cin_g + c) * P_real + p);
-    op.in_buf = BUF_EXT_IN; op.ldx = ldx; op.x_goff = op.shared_in ? 0 : op.Cin;
-    op.out_buf = BUF_EXT_OUT; op.ldy = op.G * op.Cout; op.y_goff = op.Cout;
-    if (finalize_op(h, &op)) return 1;
-    for (int i = 0; i < 2; ++i) if (dev_alloc(h, &op.st[i], (per * B * eb + 3) / 4)) return 1;
-    CK(h, cudaMemcpy(op.st[0], hs.data(), hs.size(), cudaMemcpyHostToDevice));
-    h->n_streams = B;
-    const int Tout = (T - 1) / op.down + 1;
-    const int cout_g = Cout_real_total / op.G;
-    if (res) {      // (B, Cout_total, Tout) -> channels-last in workspace 0, as the model's residual operand
-        std::vector<char> rl((size_t)B * Tout * op.ldy * eb, 0);
-        for (int b = 0; b < B; ++b)
-            for (int g = 0; g < op.G; ++g)
-                for (int c = 0; c < cout_g; ++c)
-                    for (int t = 0; t < Tout; ++t)
-                        put(rl.data(), ((size_t)b * Tout + t) * op.ldy + g * op.Cout + c, res, ((size_t)b * Cout_real_total + g * cout_g + c) * Tout + t);
-        if (ensure(h, h->ws[0], (rl.size() + 3) / 4)) return 1;
-        CK(h, cudaMemcpy(h->ws[0].p, rl.data(), rl.size(), cudaMemcpyHostToDevice));
-        op.res_buf = 0; op.ldr = op.ldy; op.r_goff = op.Cout;
+                    for (int p = 0; p < f.P; ++p)
+                        put(hs.data(), ((size_t)s * f.P + p) * f.st_C + g * f.Cin + c, io.state, ((size_t)s * io.Cin_x + g * cin_g + c) * f.P + p);
+        CK(h, cudaMemcpy(f.st[0], hs.data(), hs.size(), cudaMemcpyHostToDevice));
     }
-    float *dx, *dy;
-    const size_t ybytes = (size_t)B * Tout * op.ldy * eb;
-    if (dev_alloc(h, &dx, (xl.size() + 3) / 4) || dev_alloc(h, &dy, (ybytes + 3) / 4)) return 1;
-    CK(h, cudaMemcpy(dx, xl.data(), xl.size(), cudaMemcpyHostToDevice));
-    std::vector<Op> ops;
-    ops.push_back(op);
-    RunCtx rc{B, dx, dy, 0, offline ? CALL_OFFLINE : CALL_STREAM};
-    if (run_ops(h, ops, rc, T, nullptr)) return 1;
-    CK(h, cudaDeviceSynchronize());
-    std::vector<char> yl(ybytes), sl(per * B * eb);
-    CK(h, cudaMemcpy(yl.data(), dy, yl.size(), cudaMemcpyDeviceToHost));
-    CK(h, cudaMemcpy(sl.data(), ops[0].st[ops[0].cur ^ 1], sl.size(), cudaMemcpyDeviceToHost));     // the new state (run_ops)
-    if (!convtr) {
-        for (int b = 0; b < B; ++b)
-            for (int g = 0; g < op.G; ++g)
-                for (int c = 0; c < cout_g; ++c)
-                    for (int t = 0; t < Tout; ++t)
-                        put(y, ((size_t)b * Cout_real_total + g * cout_g + c) * Tout + t, yl.data(), ((size_t)b * Tout + t) * op.ldy + g * op.Cout + c);
-    } else {
-        for (int b = 0; b < B; ++b)
-            for (int c = 0; c < Cout_real_total; ++c)
-                for (int j = 0; j < Tout; ++j)
-                    for (int r = 0; r < stride; ++r)
-                        put(y, ((size_t)b * Cout_real_total + c) * Tout * stride + j * stride + r, yl.data(), ((size_t)b * Tout + j) * op.ldy + r * Cout_real_total + c);
-    }
-    if (!offline)
-        for (int b = 0; b < B; ++b)
+    size_t x_at = 0, y_at = 0;          // elements of x / y (and res) consumed by the previous calls
+    for (int k = 0; k < io.n_calls; ++k) {
+        const int* len = io.lengths + (size_t)k * io.B;
+        std::vector<long long> in_off(io.B + 1, 0), out_off(io.B + 1, 0);
+        for (int b = 0; b < io.B; ++b) {
+            if (len[b] < 1 || (!vl && len[b] != len[0])) return h->fail("test_conv_op: lengths must be >= 1, and equal in modes 0 and 1");
+            in_off[b + 1] = in_off[b] + len[b];
+            out_off[b + 1] = out_off[b] + (len[b] - 1) / f.down + 1;
+        }
+        const long long rows_in = in_off[io.B], rows_out = out_off[io.B];
+        std::vector<char> xl((size_t)rows_in * f.ldx * eb, 0);
+        for (int b = 0; b < io.B; ++b)
             for (int g = 0; g < G; ++g)
                 for (int c = 0; c < cin_g; ++c)
-                    for (int p = 0; p < P_real; ++p)
-                        put(state, ((size_t)b * Cin_real + g * cin_g + c) * P_real + p, sl.data(), ((size_t)b * op.P + p) * op.st_C + g * op.Cin + c);
+                    for (int t = 0; t < len[b]; ++t)
+                        put(xl.data(), (size_t)(in_off[b] + t) * f.ldx + g * f.Cin + c, io.x,
+                            x_at + (size_t)io.Cin_x * in_off[b] + (size_t)(g * cin_g + c) * len[b] + t);
+        DevBuf& xb = split ? h->ws[2] : h->hx;
+        if (ensure(h, xb, (xl.size() + 3) / 4)) return 1;
+        CK(h, cudaMemcpy(xb.p, xl.data(), xl.size(), cudaMemcpyHostToDevice));
+        if (io.res) {
+            std::vector<char> rl((size_t)rows_out * l.ldy * eb, 0);
+            for (int b = 0; b < io.B; ++b)
+                for (int g = 0; g < l.G; ++g)
+                    for (int c = 0; c < cout_g; ++c)
+                        for (long long t = 0; t < out_off[b + 1] - out_off[b]; ++t)
+                            put(rl.data(), (size_t)(out_off[b] + t) * l.ldy + g * l.Cout + c, io.res,
+                                y_at + (size_t)io.Cout_total * out_off[b] + (size_t)(g * cout_g + c) * (out_off[b + 1] - out_off[b]) + t);
+            if (ensure(h, h->ws[0], (rl.size() + 3) / 4)) return 1;
+            CK(h, cudaMemcpy(h->ws[0].p, rl.data(), rl.size(), cudaMemcpyHostToDevice));
+        }
+        const size_t ybytes = (size_t)rows_out * l.ldy * eb;
+        if (ensure(h, h->hy, (ybytes + 3) / 4)) return 1;
+        const Call call{true, io.mode, h->act_bf16, vl ? len : nullptr, io.mode == CALL_SLOTS ? io.streams + (size_t)k * io.B : nullptr};
+        if (run_call(h, call, split ? nullptr : h->hx.p, io.B, len[0], h->hy.p, nullptr)) return 1;
+        CK(h, cudaDeviceSynchronize());
+        std::vector<char> yl(ybytes);
+        CK(h, cudaMemcpy(yl.data(), h->hy.p, yl.size(), cudaMemcpyDeviceToHost));
+        for (int b = 0; b < io.B; ++b) {
+            const long long to = out_off[b + 1] - out_off[b];
+            const size_t yo = y_at + (size_t)io.Cout_total * up * out_off[b];
+            if (up > 1) {       // (Tout, up * Cout) rows are (Tout * up, Cout)
+                for (int c = 0; c < io.Cout_total; ++c)
+                    for (long long j = 0; j < to; ++j)
+                        for (int r = 0; r < up; ++r)
+                            put(io.y, yo + (size_t)c * to * up + j * up + r, yl.data(), (size_t)(out_off[b] + j) * l.ldy + r * io.Cout_total + c);
+                continue;
+            }
+            // out_nct: uniform calls write (B, G * Cout, Tout), varlen calls one (G * Cout, rows) over all utterances
+            const long long nct_ld = vl ? rows_out : to, nct_b = vl ? out_off[b] : (long long)b * l.G * l.Cout * to;
+            for (int g = 0; g < l.G; ++g)
+                for (int c = 0; c < cout_g; ++c)
+                    for (long long t = 0; t < to; ++t)
+                        put(io.y, yo + (size_t)(g * cout_g + c) * to + t, yl.data(),
+                            l.out_nct ? (size_t)(nct_b + (long long)(g * l.Cout + c) * nct_ld + t) : (size_t)(out_off[b] + t) * l.ldy + g * l.Cout + c);
+        }
+        x_at += (size_t)io.Cin_x * rows_in;
+        y_at += (size_t)io.Cout_total * up * rows_out;
+    }
+    if (per && io.state && io.mode != CALL_VARLEN) {     // each stream's current state: st[cur], or the other buffer if its slot bit is set
+        std::vector<char> sl[2];
+        for (int i = 0; i < 2; ++i) {
+            sl[i].resize(per * io.n_streams * eb);
+            CK(h, cudaMemcpy(sl[i].data(), f.st[f.cur ^ i], sl[i].size(), cudaMemcpyDeviceToHost));
+        }
+        for (int s = 0; s < io.n_streams; ++s) {
+            const char* src = sl[h->dec_slots.bit[s]].data();
+            for (int g = 0; g < G; ++g)
+                for (int c = 0; c < cin_g; ++c)
+                    for (int p = 0; p < f.P; ++p)
+                        put(io.state, ((size_t)s * io.Cin_x + g * cin_g + c) * f.P + p, src, ((size_t)s * f.P + p) * f.st_C + g * f.Cin + c);
+        }
+    }
     return 0;
+}
+
+// The single-layer entry points below: B uniform streams of T rows, one call.  x (B, Cin_real, T), state (B, Cin_real, P), res
+// (B, Cout_real_total, Tout) or nullptr; offline: Generator.forward (zero history, first-row replication in transposed convs), state
+// is neither read nor written and may be nullptr.
+static int run_single(adec_handle* h, Op& op, const void* x, int B, int Cin_real, int T, int Cout_real_total, void* state, void* y,
+                      const void* res = nullptr, bool offline = false) {
+    TestIO io;
+    io.mode = offline ? CALL_OFFLINE : CALL_STREAM;
+    io.B = io.n_streams = B;
+    std::vector<int> len(B, T);
+    io.lengths = len.data();
+    io.x = x; io.res = res; io.state = offline ? nullptr : state; io.y = y;
+    io.Cin_x = Cin_real; io.Cout_total = Cout_real_total;
+    return run_test_ops(h, std::vector<Op>{op}, io);
 }
 
 int adec_test_causal_conv(int device, const float* x, int B, int Cin, int T, const float* w, const float* bias, int Cout,
@@ -1968,7 +2064,7 @@ int adec_test_causal_conv(int device, const float* x, int B, int Cin, int T, con
     if (bias) { Bt.shape = {Cout}; Bt.data.assign(bias, bias + Cout); }
     Op op;
     int rc = make_conv_op(h, &op, "test_conv", W, bias ? &Bt : nullptr, stride, dil, groups, pre_act, slope, false);
-    if (!rc) rc = run_single(h, op, x, B, Cin, T, Cout, state, (K - 1) * dil, y, false, 1);
+    if (!rc) rc = run_single(h, op, x, B, Cin, T, Cout, state, y);
     if (rc) g_create_error = h->err;
     adec_destroy(h);
     return rc;
@@ -1988,7 +2084,7 @@ int adec_test_residual_unit(int device, const float* x, int B, int C, int T, con
     Op op;
     int rc = make_ru_op(h, &op, "test_ru", W1, W2, dil, ACT_ELU);
     if (!rc && h->engine != 0 && op.Cout > h->tc_max_fuse) rc = h->fail("test_ru: C > 128 runs as two ops on the tensor-core path; test those separately");
-    if (!rc) rc = run_single(h, op, x, B, C, T, C, state, (K - 1) * dil, y, false, 1);
+    if (!rc) rc = run_single(h, op, x, B, C, T, C, state, y);
     if (rc) g_create_error = h->err;
     adec_destroy(h);
     return rc;
@@ -2006,7 +2102,7 @@ int adec_test_causal_convtr(int device, const float* x, int B, int Cin, int T, c
     if (bias) { Bt.shape = {Cout}; Bt.data.assign(bias, bias + Cout); }
     Op op;
     int rc = make_convtr_op(h, &op, "test_convtr", W, bias ? &Bt : nullptr, stride, ACT_NONE, 0.f);
-    if (!rc) rc = run_single(h, op, x, B, Cin, T, Cout, state, 1, y, true, stride);
+    if (!rc) rc = run_single(h, op, x, B, Cin, T, Cout, state, y);
     if (rc) g_create_error = h->err;
     adec_destroy(h);
     return rc;
@@ -2050,7 +2146,7 @@ int adec_test_vocoder_layer(int device, int compute_dtype, int kind, const void*
             op.mean = h->d_mean; op.scale = h->d_scale;
         }
         // shared_in: x and state hold the Cin / groups channels every group reads
-        if (!rc) rc = run_single(h, op, x, B, shared_in ? Cin / groups : Cin, T, Cout, state, (K - 1) * dil, y, false, 1, res, offline != 0);
+        if (!rc) rc = run_single(h, op, x, B, shared_in ? Cin / groups : Cin, T, Cout, state, y, res, offline != 0);
     } else if (res) {
         rc = h->fail("adec_test_vocoder_layer: a residual is built for kind 0 only");
     } else if (kind == 1) {
@@ -2059,7 +2155,7 @@ int adec_test_vocoder_layer(int device, int compute_dtype, int kind, const void*
         W.data.assign(w, w + (size_t)Cin * Cout * 2 * up);
         if (bias) { Bt.shape = {Cout}; Bt.data.assign(bias, bias + Cout); }
         rc = make_convtr_op(h, &op, "test_convtr", W, bias ? &Bt : nullptr, up, ACT_LRELU, slope);
-        if (!rc) rc = run_single(h, op, x, B, Cin, T, Cout, state, 1, y, true, up, nullptr, offline != 0);
+        if (!rc) rc = run_single(h, op, x, B, Cin, T, Cout, state, y, nullptr, offline != 0);
     } else if (kind == 2) {
         HostTensor W, Bt;      // through the state dict, as build_hifigan builds output_conv
         W.shape = {Cout, Cin, K};
@@ -2067,9 +2163,97 @@ int adec_test_vocoder_layer(int device, int compute_dtype, int kind, const void*
         h->tensors["test_head.conv.weight"] = W;
         if (bias) { Bt.shape = {1}; Bt.data.assign(bias, bias + 1); h->tensors["test_head.conv.bias"] = Bt; }
         rc = build_head(h, &op, "test_head", ACT_LRELU, slope, true);
-        if (!rc) rc = run_single(h, op, x, B, Cin, T, 1, state, op.P, y, false, 1, nullptr, offline != 0);
+        if (!rc) rc = run_single(h, op, x, B, Cin, T, 1, state, y, nullptr, offline != 0);
     } else {
         rc = h->fail("adec_test_vocoder_layer: kind must be 0 (conv), 1 (transposed conv) or 2 (head)");
+    }
+    if (rc) g_create_error = h->err;
+    adec_destroy(h);
+    return rc;
+}
+
+int adec_test_conv_op(int device, const adec_test_op* d, int mode, int n_calls, int B, int n_streams, const int* lengths,
+                      const int* streams, const float* x, const float* res, float* state, float* y, int* launched, int max_launched,
+                      int* range_flag) {
+    if (!d || !d->w || !x || !y || !lengths || mode < CALL_STREAM || mode > CALL_SLOTS || n_calls < 1 || B < 1 ||
+        (mode == CALL_SLOTS && (!streams || n_streams < B)) || (launched && max_launched < 0)) {
+        g_create_error = "adec_test_conv_op: bad argument";
+        return 1;
+    }
+    adec_config cfg{};      // a symAD handle: fp32 activations, the engine ADEC_CONV_PATH names
+    adec_handle* h = nullptr;
+    if (adec_create(&cfg, device, &h)) return 1;
+    DeviceGuard dg(device);
+    if (launched) adec_record_launches(h, 1);
+    auto tensor = [](std::vector<int64_t> shape, const float* p) {
+        HostTensor t;
+        t.shape = std::move(shape);
+        if (p) t.data.assign(p, p + t.numel());
+        return t;
+    };
+    std::vector<Op> ops(1);
+    int rc = 0, cin_x = d->Cin, cout_total = d->Cout;
+    const HostTensor Bt = tensor({d->kind == ADEC_TEST_CONV || d->kind == ADEC_TEST_CONVTR ? d->Cout : 0}, d->bias);   // conv biases
+    switch (d->kind) {
+    case ADEC_TEST_CONV:
+        if (d->groups < 1 || d->Cin % d->groups || d->Cout % d->groups) { rc = h->fail("test_conv_op: Cin and Cout must divide into groups"); break; }
+        if (d->pre_act == ACT_NORM && (d->groups != 1 || !d->mean || !d->scale)) { rc = h->fail("test_conv_op: norm needs groups = 1, mean and scale"); break; }
+        rc = make_conv_op(h, &ops[0], "test_conv", tensor({d->Cout, d->Cin / d->groups, d->K}, d->w), d->bias ? &Bt : nullptr, d->stride,
+                          d->dil, d->groups, d->pre_act, d->slope, d->shared_in != 0);
+        ops[0].out_nct = d->out_nct != 0;
+        if (d->shared_in) cin_x = d->Cin / d->groups;
+        if (!rc && d->pre_act == ACT_NORM) {      // padded like build_hifigan's stats
+            std::vector<float> mp(ops[0].Cin, 0.f), sp(ops[0].Cin, 1.f);
+            std::copy(d->mean, d->mean + d->Cin, mp.begin());
+            std::copy(d->scale, d->scale + d->Cin, sp.begin());
+            if (dev_upload(h, &h->d_mean, mp) || dev_upload(h, &h->d_scale, sp)) rc = 1;
+            ops[0].mean = h->d_mean; ops[0].scale = h->d_scale;
+        }
+        break;
+    case ADEC_TEST_RU:
+        if (!d->w2 || d->Cin != d->Cout) { rc = h->fail("test_conv_op: a residual unit needs w2 and Cin = Cout"); break; }
+        rc = make_ru_op(h, &ops[0], "test_ru", tensor({d->Cout, d->Cout, d->K}, d->w), tensor({d->Cout, d->Cout, 1}, d->w2), d->dil, ACT_ELU);
+        if (!rc && h->engine != 0 && ops[0].Cout > h->tc_max_fuse) {     // as push_ru builds it
+            Op conv, pw;
+            split_ru_op(ops[0], &conv, &pw);
+            ops = {conv, pw};
+        }
+        break;
+    case ADEC_TEST_CONVTR:
+        rc = make_convtr_op(h, &ops[0], "test_convtr", tensor({d->Cin, d->Cout, 2 * d->stride}, d->w), d->bias ? &Bt : nullptr, d->stride,
+                            d->pre_act, d->slope);
+        break;
+    case ADEC_TEST_STEM:     // through the state dict, as build_symad builds encoder.conv
+        h->tensors["test.conv.weight"] = tensor({32, 1, 7}, d->w);
+        if (d->bias) h->tensors["test.conv.bias"] = tensor({32}, d->bias);
+        rc = build_stem(h, &ops[0], "test", 32);
+        cin_x = 1; cout_total = 32;
+        break;
+    case ADEC_TEST_HEAD:     // as build_symad / build_hifigan build decoder.conv2 / output_conv
+        h->tensors["test.conv.weight"] = tensor({1, 32, 7}, d->w);
+        if (d->bias) h->tensors["test.conv.bias"] = tensor({1}, d->bias);
+        rc = build_head(h, &ops[0], "test", d->pre_act, d->slope, d->post_tanh != 0);
+        cin_x = 32; cout_total = 1;
+        break;
+    default:
+        rc = h->fail("test_conv_op: unknown kind");
+    }
+    if (!rc) {
+        TestIO io;
+        io.mode = (CallMode)mode;
+        io.n_calls = n_calls; io.B = B;
+        io.n_streams = mode == CALL_SLOTS ? n_streams : mode == CALL_VARLEN ? 1 : B;
+        io.lengths = lengths; io.streams = streams;
+        io.x = x; io.res = res; io.state = state; io.y = y;
+        io.Cin_x = cin_x; io.Cout_total = cout_total;
+        rc = run_test_ops(h, std::move(ops), io);
+    }
+    if (!rc && launched)
+        for (int i = 0; i < max_launched * ADEC_TEST_REC; ++i) launched[i] = i < (int)h->launch_rec.size() ? h->launch_rec[i] : -1;
+    if (!rc && range_flag) {
+        range_flag[0] = adec_range_error(h, nullptr);
+        range_flag[1] = adec_range_error(h, nullptr);
+        if (range_flag[0] < 0 || range_flag[1] < 0) rc = 1;
     }
     if (rc) g_create_error = h->err;
     adec_destroy(h);

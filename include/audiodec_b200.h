@@ -252,6 +252,43 @@ int adec_test_vocoder_layer(int device, int compute_dtype, int kind, const void 
                             int pre_act, float slope, const float *mean, const float *scale, const void *res, int offline,
                             void *state, void *y);
 
+/* One fp32-grade op (the engine ADEC_CONV_PATH names) built by the model builders and run through the codec call path in any call
+ * mode, so that tests can check every row space layer by layer.  HOST pointers, fp32, channels-first per utterance. */
+enum { ADEC_TEST_CONV = 0, ADEC_TEST_RU = 1, ADEC_TEST_CONVTR = 2, ADEC_TEST_STEM = 3, ADEC_TEST_HEAD = 4 };
+typedef struct adec_test_op {
+    int kind;          /* ADEC_TEST_*                                                                                              */
+    int Cin, Cout;     /* conv: w (Cout, Cin/groups, K); RU: w (C, C, K) and w2 (C, C, 1), C = Cin = Cout; transposed conv:
+                        * w (Cin, Cout, 2*stride); stem: w (32, 1, 7); head: w (1, 32, 7)                                           */
+    int K, stride, dil, groups, shared_in;   /* conv: stride s > 1 needs K = 2s (the encoder's strided convs)                      */
+    int pre_act;       /* the kernels' ACT_* codes: 0 none, 1 ELU, 2 LeakyReLU(slope), 3 norm ((x - mean) / scale, groups = 1)   */
+    float slope;
+    int out_nct;       /* conv: write channels-first, as the projector writes z                                                  */
+    int post_tanh;     /* head: tanh after the conv                                                                             */
+    const float *w, *w2, *bias, *mean, *scale;   /* bias, mean, scale may be NULL                                             */
+} adec_test_op;
+/* launch records: 8 ints {launch kind, NT (FFMA: output tile), fuse, pre_act, prec (wg_conv.cuh PREC_*), varlen, paired, stacked} */
+enum { ADEC_TEST_REC = 8, ADEC_TEST_LAUNCH_TC = 0, ADEC_TEST_LAUNCH_FFMA = 1, ADEC_TEST_LAUNCH_STEM = 2, ADEC_TEST_LAUNCH_HEAD = 3 };
+/* mode: 0 = stream (adec_encode: B = n_streams streams advanced by equal lengths, stacked rows unless ADEC_STACK_ROWS=0), 1 = offline
+ * (zero history, first-row replication in transposed convs), 2 = varlen offline, 3 = stream slots (`streams`: the B distinct streams of
+ * n_streams that each call advances).  n_calls consecutive calls on one handle: lengths (n_calls, B) are input rows per utterance
+ * (equal within a call in modes 0 and 1), streams (n_calls, B).  x: every call's utterances one after the other, each (Cin_x, L)
+ * where Cin_x = Cin (shared_in: Cin / groups; stem: 1).  y: the same for the outputs, each (Cout, Tout * stride) for a transposed conv,
+ * (Cout, (L - 1) / stride + 1) otherwise (head: 1 channel; stem: 32).  res: NULL, or a conv's residual, laid out like y, added after
+ * the bias.  state (n_streams, Cin_x, P): the initial history of every stream (modes 0 and 3; may be NULL in modes 1 and 2), and on
+ * return each stream's current state (not written in mode 2).  launched: NULL, or room for max_launched records; the launches of all
+ * calls are written in order and the rest of the array is set to -1.  A split residual unit (C above ADEC_TC_MAXFUSE on the tensor-core
+ * engines) runs as its two launches.  range_flag: NULL, or two ints: adec_range_error after the calls, then read once more (the
+ * flag's report-once protocol). */
+int adec_test_conv_op(int device, const adec_test_op *op, int mode, int n_calls, int B, int n_streams, const int *lengths,
+                      const int *streams, const float *x, const float *res, float *state, float *y, int *launched, int max_launched,
+                      int *range_flag);
+
+/* Launch records of a model handle, in the format above: adec_record_launches(h, 1) clears the record and starts appending one
+ * record per conv / stem / head launch of every later call, (h, 0) stops.  adec_launch_records copies up to max_records of them and
+ * returns how many there are (-1 on error).  Tests use it to list the kernel instantiations the shipped plans select. */
+int adec_record_launches(adec_handle *h, int enable);
+int adec_launch_records(const adec_handle *h, int *out, int max_records);
+
 #ifdef __cplusplus
 }
 #endif

@@ -101,9 +101,12 @@ def rvq_lookup(idx, codebook):
 class SymADOracle:
     """models/autoencoder/AudioDec.py:166-256 (StreamGenerator, codec='audiodec')."""
 
-    def __init__(self, params, state_dict):
+    def __init__(self, params, state_dict, dtype=torch.float32):
+        """dtype: the precision every weight, state and activation is computed in (float64: the exact reference of the tests'
+        precision checks; the default float32 is the reference's own arithmetic)."""
         self.p = dict(params)
-        self.sd = {k: v.detach().clone().float() for k, v in state_dict.items()}
+        self.dtype = dtype
+        self.sd = {k: v.detach().clone().to(dtype) for k, v in state_dict.items()}
         # use_weight_norm (symAAD, AudioDec.py:152-162): weight = g * v/||v||, recomputed per call in the reference
         for k in list(self.sd):
             if k.endswith("weight_g"):
@@ -176,7 +179,7 @@ class SymADOracle:
 
     def encode(self, x):                                 # AudioDec.py:228-234 -> encoder.py:137-142, :76-81
         self._ensure_batch(x.shape[0])
-        h = self._conv("encoder.conv", x)
+        h = self._conv("encoder.conv", x.to(self.dtype))
         for i, s in enumerate(self.p["enc_strides"]):
             for j, d in enumerate((1, 3, 9)):
                 h = self._res_unit(f"encoder.conv_blocks.{i}.res_units.{j}", h, d)
@@ -198,7 +201,7 @@ class SymADOracle:
 
     def decode(self, zq):                                # AudioDec.py:246-247 -> decoder.py:142-148, :76-81
         self._ensure_batch(zq.shape[0])
-        h = self._conv("decoder.conv1", zq.transpose(2, 1))
+        h = self._conv("decoder.conv1", zq.transpose(2, 1).to(self.dtype))
         for i, s in enumerate(self.p["dec_strides"]):
             n = f"decoder.conv_blocks.{i}.1" if self.activate else f"decoder.conv_blocks.{i}"
             if self.activate:
@@ -239,9 +242,11 @@ class HiFiGANOracle:
     """models/vocoder/HiFiGAN.py:222-305 (StreamGenerator) with MultiGroupConv1d blocks
     (models/vocoder/modules/multi_fusion.py:82-141, residual_block.py:23-105)."""
 
-    def __init__(self, params, state_dict):
+    def __init__(self, params, state_dict, dtype=torch.float32):
+        """dtype: as SymADOracle's"""
         self.p = dict(params)
-        sd = {k: v.detach().clone().float() for k, v in state_dict.items()}
+        self.dtype = dtype
+        sd = {k: v.detach().clone().to(dtype) for k, v in state_dict.items()}
         self.w = {}
         for k in list(sd):
             if k.endswith("weight_g"):
@@ -292,6 +297,7 @@ class HiFiGANOracle:
     def decode(self, c):                                 # HiFiGAN.py:268-296
         if next(iter(self.state.values())).shape[0] != c.shape[0]:
             self.set_batch(c.shape[0])
+        c = c.to(self.dtype)
         if self.mean is not None:
             c = (c - self.mean) / self.scale             # :276-279
         c = self._conv("input_conv", c.transpose(2, 1))  # :282-284
