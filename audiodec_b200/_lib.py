@@ -40,7 +40,7 @@ class AdecConfig(ctypes.Structure):
     ]
 
 
-MODEL_SYMAD, MODEL_HIFIGAN = 0, 1
+MODEL_SYMAD, MODEL_HIFIGAN, MODEL_SYMAD_DECODER = 0, 1, 2
 
 
 class AdecTestOp(ctypes.Structure):
@@ -49,11 +49,12 @@ class AdecTestOp(ctypes.Structure):
         ("kind", c_int), ("Cin", c_int), ("Cout", c_int), ("K", c_int), ("stride", c_int), ("dil", c_int), ("groups", c_int),
         ("shared_in", c_int), ("pre_act", c_int), ("slope", c_float), ("out_nct", c_int), ("post_tanh", c_int),
         ("w", c_void_p), ("w2", c_void_p), ("bias", c_void_p), ("mean", c_void_p), ("scale", c_void_p),
+        ("compute_dtype", c_int),
     ]
 
 
 TEST_CONV, TEST_RU, TEST_CONVTR, TEST_STEM, TEST_HEAD = 0, 1, 2, 3, 4
-TEST_REC = 8
+TEST_REC = 9
 
 # name -> (restype, argtypes); every symbol include/audiodec_b200.h declares
 SYMBOLS = {

@@ -15,13 +15,16 @@ Differences from the reference, all extensions:
     ``ResidualVQ.forward_index`` yields before its ``squeeze(1)``, vq_module.py:148-149) and ``lookup``
     returns (B,F,D).
   * there is no CPU path: ``.to('cpu')`` raises.
-  * ``HiFiGANStreamGenerator.set_activation_dtype(torch.bfloat16)`` keeps every activation, the causal state and the decode
-    input / output in bf16 (the data layout and dtype contract of the reference's ``decoder.to(torch.bfloat16)``); plain
-    ``.to(torch.bfloat16)`` rounds only the conv operands and keeps fp32 activations and fp32 I/O.
+  * ``set_activation_dtype(torch.bfloat16)`` on a decoder-only generator (``HiFiGANStreamGenerator``,
+    ``SymADDecoderStreamGenerator``) keeps every activation, the causal state and the decode input / output in bf16 (the data
+    layout and dtype contract of the reference's ``decoder.to(torch.bfloat16)``); plain ``.to(torch.bfloat16)`` rounds only the
+    conv operands and keeps fp32 activations and fp32 I/O.  ``SymADDecoderStreamGenerator`` is the symAD decoder alone, the
+    object the reference's receiver decodes with; a full ``SymADStreamGenerator`` stays fp32-grade.
 """
 from __future__ import annotations
 
 import ctypes
+import inspect
 
 import torch
 
@@ -72,7 +75,10 @@ class _StreamGeneratorBase:
         self._h = None
         self._device = None
         self._operand_mode = 0        # what .to(dtype) selected: 0 = fp32, 1 = bf16 conv operands
-        self._act_bf16 = False        # HiFi-GAN only (set_activation_dtype): bf16 activations, state and decode I/O = compute_dtype 2
+        self._act_bf16 = False        # decoders only (set_activation_dtype): bf16 activations, state and decode I/O = compute_dtype 2
+
+    # the decoder-only generators (HiFi-GAN vocoder, symAD decoder) have the bf16 modes; a full symAD generator does not
+    _bf16_modes = False
 
     # -- torch.nn.Module look-alikes ------------------------------------------------------------
     def load_state_dict(self, state_dict, strict=True):
@@ -109,14 +115,16 @@ class _StreamGeneratorBase:
         return self
 
     def _set_dtype(self, dtype):
-        """`module.to(torch.bfloat16)` of the reference: only the HiFi-GAN vocoder has a reduced-precision mode (bf16 conv operands,
-        fp32 accumulation and fp32 activations in HBM); the encoder / projector / RVQ must stay fp32-grade for bit-identical indices."""
+        """`module.to(torch.bfloat16)` of the reference: only the decoder-only generators (HiFi-GAN vocoder, symAD decoder) have a
+        reduced-precision mode (bf16 conv operands, fp32 accumulation and fp32 activations in HBM); the encoder / projector / RVQ must
+        stay fp32-grade for bit-identical indices."""
         if dtype == torch.float32:
             want = 0
-        elif dtype == torch.bfloat16 and self._cfg.model_type == _lib.MODEL_HIFIGAN:
+        elif dtype == torch.bfloat16 and self._bf16_modes:
             want = 1
         else:
-            raise NotImplementedError(f"{type(self).__name__} has no {dtype} mode (fp32 everywhere; bf16 for the HiFi-GAN vocoder only)")
+            raise NotImplementedError(f"{type(self).__name__} has no {dtype} mode (fp32 everywhere; bf16 for the decoder-only generators: "
+                                      "HiFiGANStreamGenerator, SymADDecoderStreamGenerator)")
         mode = 2 if self._act_bf16 else want
         if self._h is not None and mode != self._cfg.compute_dtype:
             raise RuntimeError("set the compute dtype before .to(device): the weights are packed when the handle is created")
@@ -125,8 +133,21 @@ class _StreamGeneratorBase:
         return self
 
     def set_activation_dtype(self, dtype):
-        raise NotImplementedError(f"{type(self).__name__} keeps fp32 activations: the encoder, projector and RVQ must stay fp32-grade "
-                                  "for bit-identical indices (bf16 activations are built for the HiFi-GAN vocoder only)")
+        """torch.bfloat16: every activation, the causal state, and decode's zq input and y output are bf16 (conv operands bf16, fp32
+        accumulation, one rounding per stored value) - what the reference's `decoder.to(torch.bfloat16)` stores and returns.
+        torch.float32: back to fp32 activations with the operand precision `.to(dtype)` chose.  Call before `.to(device)`; returns
+        self, so `d.set_activation_dtype(torch.bfloat16).to(dev)` chains.  Decoder-only generators only."""
+        if not self._bf16_modes:
+            raise NotImplementedError(f"{type(self).__name__} keeps fp32 activations: the encoder, projector and RVQ must stay fp32-grade "
+                                      "for bit-identical indices (bf16 activations are built for the decoder-only generators: "
+                                      "HiFiGANStreamGenerator, SymADDecoderStreamGenerator)")
+        if dtype not in (torch.float32, torch.bfloat16):
+            raise NotImplementedError(f"{type(self).__name__} has no {dtype} activation mode (float32 or bfloat16)")
+        if self._h is not None:
+            raise RuntimeError("set the activation dtype before .to(device): the state and workspaces are laid out when the handle is created")
+        self._act_bf16 = dtype == torch.bfloat16
+        self._cfg.compute_dtype = 2 if self._act_bf16 else self._operand_mode
+        return self
 
     def bfloat16(self):
         return self._set_dtype(torch.bfloat16)
@@ -288,36 +309,51 @@ class _StreamGeneratorBase:
         return self._decode_varlen("adec_decode_streams", zq, frames, sarr)
 
 
+def _symad_init(g, model_type, input_channels=1, output_channels=1, encode_channels=32, decode_channels=32, code_dim=64,
+                codebook_num=8, codebook_size=1024, bias=True, enc_ratios=(2, 4, 8, 16), dec_ratios=(16, 8, 4, 2),
+                enc_strides=(3, 4, 5, 5), dec_strides=(5, 5, 4, 3), mode="causal", codec="audiodec",
+                projector="conv1d", quantier="residual_vq", nonlinear_activation="ELU",
+                nonlinear_activation_params={}, use_weight_norm=False):
+    """The config of a symAD generator (AudioDec.py:31-51 keywords) into g's adec_config, as a handle of `model_type`."""
+    assert mode == "causal", f"Mode {mode} does not support streaming!"       # models/utils.py:13-15
+    if codec not in ("audiodec", "activate_audiodec"):
+        raise NotImplementedError(f"Codec ({codec}) is not supported!")          # AudioDec.py:53-60
+    if projector != "conv1d" or quantier != "residual_vq":
+        raise NotImplementedError("only projector='conv1d', quantier='residual_vq' are built")
+    if nonlinear_activation != "ELU" or nonlinear_activation_params:
+        raise NotImplementedError("only ELU(alpha=1) residual units are built")
+    c = g._cfg
+    c.model_type = model_type
+    c.input_channels, c.output_channels = input_channels, output_channels
+    c.encode_channels, c.decode_channels = encode_channels, decode_channels
+    c.code_dim, c.codebook_num, c.codebook_size = code_dim, codebook_num, codebook_size
+    c.bias = int(bias)
+    c.n_enc, c.n_dec = len(enc_strides), len(dec_strides)
+    _fill(c.enc_ratios, enc_ratios), _fill(c.enc_strides, enc_strides)
+    _fill(c.dec_ratios, dec_ratios), _fill(c.dec_strides, dec_strides)
+    c.use_weight_norm = int(use_weight_norm)
+    c.codec_activate = int(codec == "activate_audiodec")
+    g.input_channels = input_channels
+    g.code_dim, g.codebook_num = code_dim, codebook_num
+    g.enc_strides = tuple(enc_strides)
+
+
+def _symad_signature(init):
+    """Give a symAD generator's __init__(self, *args, **params) the explicit keywords of AudioDec.py's StreamGenerator (those of
+    _symad_init), for inspect.signature and help()."""
+    sig = inspect.signature(_symad_init)
+    self_p = inspect.Parameter("self", inspect.Parameter.POSITIONAL_OR_KEYWORD)
+    init.__signature__ = sig.replace(parameters=[self_p] + list(sig.parameters.values())[2:])
+    return init
+
+
 class SymADStreamGenerator(_StreamGeneratorBase):
     """models/autoencoder/AudioDec.py:166-256."""
 
-    def __init__(self, input_channels=1, output_channels=1, encode_channels=32, decode_channels=32, code_dim=64,
-                 codebook_num=8, codebook_size=1024, bias=True, enc_ratios=(2, 4, 8, 16), dec_ratios=(16, 8, 4, 2),
-                 enc_strides=(3, 4, 5, 5), dec_strides=(5, 5, 4, 3), mode="causal", codec="audiodec",
-                 projector="conv1d", quantier="residual_vq", nonlinear_activation="ELU",
-                 nonlinear_activation_params={}, use_weight_norm=False):
+    @_symad_signature
+    def __init__(self, *args, **params):
         super().__init__()
-        assert mode == "causal", f"Mode {mode} does not support streaming!"       # models/utils.py:13-15
-        if codec not in ("audiodec", "activate_audiodec"):
-            raise NotImplementedError(f"Codec ({codec}) is not supported!")          # AudioDec.py:53-60
-        if projector != "conv1d" or quantier != "residual_vq":
-            raise NotImplementedError("only projector='conv1d', quantier='residual_vq' are built")
-        if nonlinear_activation != "ELU" or nonlinear_activation_params:
-            raise NotImplementedError("only ELU(alpha=1) residual units are built")
-        c = self._cfg
-        c.model_type = _lib.MODEL_SYMAD
-        c.input_channels, c.output_channels = input_channels, output_channels
-        c.encode_channels, c.decode_channels = encode_channels, decode_channels
-        c.code_dim, c.codebook_num, c.codebook_size = code_dim, codebook_num, codebook_size
-        c.bias = int(bias)
-        c.n_enc, c.n_dec = len(enc_strides), len(dec_strides)
-        _fill(c.enc_ratios, enc_ratios), _fill(c.enc_strides, enc_strides)
-        _fill(c.dec_ratios, dec_ratios), _fill(c.dec_strides, dec_strides)
-        c.use_weight_norm = int(use_weight_norm)
-        c.codec_activate = int(codec == "activate_audiodec")
-        self.input_channels = input_channels
-        self.code_dim, self.codebook_num = code_dim, codebook_num
-        self.enc_strides = tuple(enc_strides)
+        _symad_init(self, _lib.MODEL_SYMAD, *args, **params)
 
     # -- streaming API ---------------------------------------------------------------------------------
     def initial_encoder(self, receptive_length, device):
@@ -557,8 +593,48 @@ class SymADStreamGenerator(_StreamGeneratorBase):
         return self._decode(zq)
 
 
+class SymADDecoderStreamGenerator(_StreamGeneratorBase):
+    """The decoder of a symAD StreamGenerator alone (models/autoencoder/AudioDec.py:224-256): what the reference's receiver runs as
+    its `decoder` object (initial_decoder / decode, utils/audiodec.py:104-106; rx_encoder does the lookup).  Same constructor
+    keywords as SymADStreamGenerator, and it loads the same state dict (the encoder, projector and quantizer keys are ignored).
+    Decoding in fp32 gives what SymADStreamGenerator.decode gives, bit for bit.  Unlike the full generator it has the vocoder's
+    bf16 modes: `.to(torch.bfloat16)` for bf16 conv operands with fp32 activations and I/O, `set_activation_dtype(torch.bfloat16)`
+    for bf16 activations, causal state and decode I/O."""
+    _bf16_modes = True
+
+    @_symad_signature
+    def __init__(self, *args, **params):
+        super().__init__()
+        _symad_init(self, _lib.MODEL_SYMAD_DECODER, *args, **params)
+
+    def initial_decoder(self, zq):
+        self.decode(zq)                                                              # AudioDec.py:224-225
+
+    def decode(self, zq):
+        """zq (B,F,code_dim) channels-last -> y (B,1,F*hop)   (AudioDec.py:246-247).  With bf16 activations zq may be bf16 or fp32
+        (cast on the device) and y is bf16."""
+        self._ready()
+        self._want(zq, "decode", 2, self.code_dim)
+        return self._decode(zq)
+
+    def decode_offline(self, zq):
+        """Decoder.forward (decoder.py:135-140): zq (B,code_dim,F) channels-first -> y (B,1,F*hop).  Discards the streaming state."""
+        return self._decode_offline(zq)
+
+    def decode_offline_varlen(self, zq, frames):
+        """decode_offline over utterances of different lengths in one launch sequence: zq (1, code_dim, sum F_b) channels-first ->
+        list of B waveforms (1, 1, F_b * hop), views of one output buffer, each equal to decode_offline of that utterance alone."""
+        return self._decode_offline_varlen(zq, frames)
+
+    def decode_streams(self, zq, frames, streams):
+        """Advance streams[b] by frames[b] frames of zq ((1, sum F_b, code_dim) or (sum F_b, code_dim) channels-last) in one launch
+        sequence -> list of B waveforms (1, 1, F_b * hop), each equal to a B = 1 streaming decode of those frames."""
+        return self._decode_streams(zq, frames, streams)
+
+
 class HiFiGANStreamGenerator(_StreamGeneratorBase):
     """models/vocoder/HiFiGAN.py:222-305 (AD v1: groups>1 and a single resblock kernel -> MultiGroupConv1d)."""
+    _bf16_modes = True
 
     def __init__(self, in_channels=80, out_channels=1, channels=512, kernel_size=7, upsample_scales=(8, 8, 2, 2),
                  upsample_kernel_sizes=(16, 16, 4, 4), resblock_kernel_sizes=(3, 7, 11),
@@ -591,19 +667,6 @@ class HiFiGANStreamGenerator(_StreamGeneratorBase):
         c.use_weight_norm = int(use_weight_norm)
         c.has_stats = int(stats is not None)       # mean/scale themselves come from the state dict (HiFiGAN.py:206-219)
         self.in_channels = in_channels
-
-    def set_activation_dtype(self, dtype):
-        """torch.bfloat16: every activation, the causal state, and decode's zq input and y output are bf16 (conv operands bf16, fp32
-        accumulation, one rounding per stored value) - what the reference's `decoder.to(torch.bfloat16)` stores and returns.
-        torch.float32: back to fp32 activations with the operand precision `.to(dtype)` chose.  Call before `.to(device)`; returns
-        self, so `d.set_activation_dtype(torch.bfloat16).to(dev)` chains."""
-        if dtype not in (torch.float32, torch.bfloat16):
-            raise NotImplementedError(f"HiFiGANStreamGenerator has no {dtype} activation mode (float32 or bfloat16)")
-        if self._h is not None:
-            raise RuntimeError("set the activation dtype before .to(device): the state and workspaces are laid out when the handle is created")
-        self._act_bf16 = dtype == torch.bfloat16
-        self._cfg.compute_dtype = 2 if self._act_bf16 else self._operand_mode
-        return self
 
     def initial_decoder(self, c):
         self.decode(c)                                                                # HiFiGAN.py:264-265

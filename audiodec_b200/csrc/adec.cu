@@ -93,7 +93,8 @@ const ConvKernelCfg* find_conv_kernel(int CW, int CO, bool fuse) {
 }
 
 // tensor-core engine (wg_conv.cuh): PREC_F16 = two fp16 pieces per operand, three products (fp32-grade, default); PREC_TF32 = 3xTF32
-// (ADEC_CONV_PATH=tf32); PREC_BF16 = bf16 operands, one product (the vocoder's bf16 modes; BST = bf16 activations in HBM as well).
+// (ADEC_CONV_PATH=tf32); PREC_BF16 = bf16 operands, one product (the bf16 modes of the vocoder and the symAD decoder-only handle;
+// BST = bf16 activations in HBM as well).
 // Persistent: one CTA per SM loops over (time tile, channel tile, stream) tiles.
 typedef cudaError_t (*TcPersistFn)(const ConvArgs&, int, int, int, int, int, cudaStream_t);
 template <int NT, bool F, int PRE, int PREC, bool BST, bool VL, bool PAIR = false>
@@ -141,8 +142,11 @@ struct TcKernelCfg { int NT; bool fuse; int pre, prec; bool bst; int tap_bytes; 
 #define ADEC_TC_FP32(NT, PREC) \
     ADEC_TC1(NT, true, ACT_ELU, PREC, false), ADEC_TC1(NT, false, ACT_NONE, PREC, false), ADEC_TC1(NT, false, ACT_ELU, PREC, false), \
     ADEC_TC1(NT, false, ACT_LRELU, PREC, false), ADEC_TC1(NT, false, ACT_NORM, PREC, false)
+// bf16: the vocoder's layers (none / LeakyReLU / norm) and the symAD decoder's (fused residual unit, ELU before the split unit's
+// launches and symAAD's transposed convs)
 #define ADEC_TC_BF16(NT, BST) \
-    ADEC_TC1(NT, false, ACT_NONE, PREC_BF16, BST), ADEC_TC1(NT, false, ACT_LRELU, PREC_BF16, BST), ADEC_TC1(NT, false, ACT_NORM, PREC_BF16, BST)
+    ADEC_TC1(NT, false, ACT_NONE, PREC_BF16, BST), ADEC_TC1(NT, false, ACT_LRELU, PREC_BF16, BST), ADEC_TC1(NT, false, ACT_NORM, PREC_BF16, BST), \
+    ADEC_TC1(NT, true, ACT_ELU, PREC_BF16, BST), ADEC_TC1(NT, false, ACT_ELU, PREC_BF16, BST)
 #define ADEC_TC(NT) ADEC_TC_FP32(NT, PREC_F16), ADEC_TC_FP32(NT, PREC_TF32), ADEC_TC_BF16(NT, false), ADEC_TC_BF16(NT, true)
 const TcKernelCfg kTcKernels[] = {ADEC_TC(128), ADEC_TC(64), ADEC_TC(32)};
 
@@ -235,7 +239,7 @@ struct adec_handle {
     int st_cap = 1;        // streams the state buffers were allocated for
     int engine = 2;               // ADEC_CONV_PATH: 2 = f16 (fp16-split wgmma, default), 1 = tf32 (3xTF32 wgmma), 0 = ffma (CUDA cores)
     int tc_max_fuse = 128;        // ADEC_TC_MAXFUSE: residual units wider than this run as two launches on the tensor-core engines
-    bool bf16 = false;            // cfg.compute_dtype >= 1: bf16 operands (HiFi-GAN vocoder, f16 engine only)
+    bool bf16 = false;            // cfg.compute_dtype >= 1: bf16 operands (HiFi-GAN vocoder and symAD decoder-only, f16 engine only)
     bool act_bf16 = false;        // cfg.compute_dtype == 2: bf16 activations, causal state and decode I/O as well
     int act_bytes() const { return act_bf16 ? 2 : 4; }   // bytes per stored activation / state element
     bool stack_rows = true;       // ADEC_STACK_ROWS=0: never stack several streams' rows into one tile (A/B)
@@ -497,7 +501,7 @@ int finalize_op_wg(adec_handle* h, Op* op) {
     // same activation window (the epilogue masks per column pair)
     const bool pad_tile = !op->fuse && NT == 32 && op->Cout > 64 && op->Cout < 128;
     if (pad_tile) NT = 128;
-    const int prec = h->engine == 1 ? PREC_TF32 : (h->bf16 && !op->fuse) ? PREC_BF16 : PREC_F16;
+    const int prec = h->engine == 1 ? PREC_TF32 : h->bf16 ? PREC_BF16 : PREC_F16;
     if (h->act_bf16 && op->RG > 1) return h->fail(op->name + ": bf16 activations are built for stride-1 and transposed convs only");
     op->tc = find_tc_kernel(NT, op->fuse, op->pre_act, prec, h->act_bf16);
     if (!op->tc || (op->fuse && (NT != op->Cout || op->mid_act != op->pre_act))) return h->fail(op->name + ": no tensor-core kernel");
@@ -854,18 +858,18 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
                 e = (vl ? op.tc->pfn_vl : pair ? op.tc->pfn_pair : op.tc->pfn)(a, (int)grid.x, (int)grid.y, (int)n_tiles, n_ctas, (int)psmem, rc.stream);
                 if (h->launch_log)
                     h->launch_log->insert(h->launch_log->end(), {ADEC_TEST_LAUNCH_TC, op.tc->NT, op.tc->fuse, op.tc->pre, op.tc->prec, vl, pair,
-                                                                 a.stack_L > 0});
+                                                                 a.stack_L > 0, op.tc->bst});
             } else {
                 const int TT = op.kc->TT;
                 dim3 grid((Tout + TT - 1) / TT, op.G * op.n_co_tiles, rc.B);
                 e = op.kc->fn(a, grid, TT + (op.Ktaps - 1) * op.dil, rc.stream);
                 if (h->launch_log)
-                    h->launch_log->insert(h->launch_log->end(), {ADEC_TEST_LAUNCH_FFMA, op.kc->CO, op.kc->fuse, op.pre_act, 0, 0, 0, 0});
+                    h->launch_log->insert(h->launch_log->end(), {ADEC_TEST_LAUNCH_FFMA, op.kc->CO, op.kc->fuse, op.pre_act, 0, 0, 0, 0, 0});
             }
         }
         if (h->launch_log && op.kind != OP_CONV)
             h->launch_log->insert(h->launch_log->end(), {op.kind == OP_STEM ? ADEC_TEST_LAUNCH_STEM : ADEC_TEST_LAUNCH_HEAD, 0, 0, op.pre_act,
-                                                         0, vl, 0, 0});
+                                                         0, vl, 0, 0, op.kind == OP_HEAD && h->act_bf16});
         if (e != cudaSuccess) return h->fail(fmt("launch of %s failed: %s", op.name.c_str(), cudaGetErrorString(e)));
         ++h->launches;
         if (h->profiling) {
@@ -975,48 +979,19 @@ int push_ru(adec_handle* h, std::vector<Op>* ops, Wire* w, const std::string& ru
     return 0;
 }
 
-int build_symad(adec_handle* h) {
+constexpr int kRuDils[3] = {1, 3, 9};     // encoder.py:33, decoder.py:30
+
+int check_symad_cfg(adec_handle* h) {
     const adec_config& c = h->cfg;
     if (c.input_channels != 1 || c.output_channels != 1) return h->fail("symAD: only mono (input/output_channels=1) is built");
     if (c.code_dim != 64) return h->fail("symAD: only code_dim=64 is built");
-    // ---- encoder (models/autoencoder/modules/encoder.py:84-142)
-    Wire w; w.cur = BUF_EXT_IN; w.cur_ld = 1;
-    {
-        Op op;
-        if (build_stem(h, &op, "encoder.conv", c.encode_channels)) return 1;
-        op.in_buf = BUF_EXT_IN; op.ldx = 1; op.out_buf = 0; op.ldy = 32;
-        w.cur = 0; w.cur_ld = 32;
-        h->enc_ops.push_back(std::move(op));
-    }
-    int ch = c.encode_channels;
-    static const int dils[3] = {1, 3, 9};   // encoder.py:33
-    for (int i = 0; i < c.n_enc; ++i) {
-        const std::string pre = fmt("encoder.conv_blocks.%d", i);
-        for (int j = 0; j < 3; ++j)
-            if (push_ru(h, &h->enc_ops, &w, pre + fmt(".res_units.%d", j), dils[j], ch)) return 1;
-        HostTensor W;
-        if (get_weight(h, pre + ".conv.conv", &W)) return 1;
-        const HostTensor* b = find(h, pre + ".conv.conv.bias");
-        Op op;
-        if (make_conv_op(h, &op, pre + ".conv", W, b, c.enc_strides[i], 1, 1, ACT_NONE, 0.f, false)) return 1;
-        load_pad_buffer(h, &op, pre + ".conv.pad_buffer", ch);
-        ch = c.encode_channels * c.enc_ratios[i];
-        chain(&op, &w, ch);
-        h->enc_ops.push_back(std::move(op));
-    }
-    {   // projector (projector.py:40,52-54): k=3, no bias; writes z channels-first (B,64,F)
-        HostTensor W;
-        if (get_weight(h, "projector.project.conv", &W)) return 1;
-        Op op;   // symAAD: the encoder's trailing ELU (encoder.py:174-175) is this conv's pre-activation
-        if (make_conv_op(h, &op, "projector.project", W, find(h, "projector.project.conv.bias"), 1, 1, 1,
-                         c.codec_activate ? ACT_ELU : ACT_NONE, 0.f, false)) return 1;
-        load_pad_buffer(h, &op, "projector.project.pad_buffer", ch);
-        op.in_buf = w.cur; op.ldx = w.cur_ld; op.x_goff = op.Cin;
-        op.out_buf = BUF_EXT_OUT; op.out_nct = true; op.ldy = op.Cout; op.y_goff = op.Cout;
-        if (op.Cout != c.code_dim) return h->fail("projector: code_dim must be a multiple of 32");
-        h->enc_ops.push_back(std::move(op));
-    }
-    // ---- decoder (models/autoencoder/modules/decoder.py:84-148)
+    return 0;
+}
+
+// ---- decoder (models/autoencoder/modules/decoder.py:84-148): what a full symAD handle and a decoder-only one (ADEC_MODEL_SYMAD_DECODER)
+// both decode with
+int build_symad_decoder(adec_handle* h) {
+    const adec_config& c = h->cfg;
     Wire d; d.cur = BUF_EXT_IN; d.cur_ld = c.code_dim;
     {
         HostTensor W;
@@ -1043,7 +1018,7 @@ int build_symad(adec_handle* h) {
         d.cur_ld = cout;   // (T, s*Cout) is (T*s, Cout)
         h->dec_ops.push_back(std::move(op));
         for (int j = 0; j < 3; ++j)
-            if (push_ru(h, &h->dec_ops, &d, pre + fmt(".res_units.%d", j), dils[j], cout)) return 1;
+            if (push_ru(h, &h->dec_ops, &d, pre + fmt(".res_units.%d", j), kRuDils[j], cout)) return 1;
     }
     {
         Op op;
@@ -1051,6 +1026,58 @@ int build_symad(adec_handle* h) {
         op.in_buf = d.cur; op.ldx = d.cur_ld; op.out_buf = BUF_EXT_OUT; op.ldy = 1;
         h->dec_ops.push_back(std::move(op));
     }
+    return 0;
+}
+
+// The decoder-only handle loads a full generator state dict: the encoder, projector and RVQ keys are accepted and ignored.
+int build_symad_decoder_only(adec_handle* h) {
+    if (check_symad_cfg(h) || build_symad_decoder(h)) return 1;
+    for (const auto& kv : h->tensors)
+        for (const char* pre : {"encoder.", "projector.", "quantizer."})
+            if (kv.first.compare(0, strlen(pre), pre) == 0) h->consumed.insert(kv.first);
+    return 0;
+}
+
+int build_symad(adec_handle* h) {
+    const adec_config& c = h->cfg;
+    if (check_symad_cfg(h)) return 1;
+    // ---- encoder (models/autoencoder/modules/encoder.py:84-142)
+    Wire w; w.cur = BUF_EXT_IN; w.cur_ld = 1;
+    {
+        Op op;
+        if (build_stem(h, &op, "encoder.conv", c.encode_channels)) return 1;
+        op.in_buf = BUF_EXT_IN; op.ldx = 1; op.out_buf = 0; op.ldy = 32;
+        w.cur = 0; w.cur_ld = 32;
+        h->enc_ops.push_back(std::move(op));
+    }
+    int ch = c.encode_channels;
+    for (int i = 0; i < c.n_enc; ++i) {
+        const std::string pre = fmt("encoder.conv_blocks.%d", i);
+        for (int j = 0; j < 3; ++j)
+            if (push_ru(h, &h->enc_ops, &w, pre + fmt(".res_units.%d", j), kRuDils[j], ch)) return 1;
+        HostTensor W;
+        if (get_weight(h, pre + ".conv.conv", &W)) return 1;
+        const HostTensor* b = find(h, pre + ".conv.conv.bias");
+        Op op;
+        if (make_conv_op(h, &op, pre + ".conv", W, b, c.enc_strides[i], 1, 1, ACT_NONE, 0.f, false)) return 1;
+        load_pad_buffer(h, &op, pre + ".conv.pad_buffer", ch);
+        ch = c.encode_channels * c.enc_ratios[i];
+        chain(&op, &w, ch);
+        h->enc_ops.push_back(std::move(op));
+    }
+    {   // projector (projector.py:40,52-54): k=3, no bias; writes z channels-first (B,64,F)
+        HostTensor W;
+        if (get_weight(h, "projector.project.conv", &W)) return 1;
+        Op op;   // symAAD: the encoder's trailing ELU (encoder.py:174-175) is this conv's pre-activation
+        if (make_conv_op(h, &op, "projector.project", W, find(h, "projector.project.conv.bias"), 1, 1, 1,
+                         c.codec_activate ? ACT_ELU : ACT_NONE, 0.f, false)) return 1;
+        load_pad_buffer(h, &op, "projector.project.pad_buffer", ch);
+        op.in_buf = w.cur; op.ldx = w.cur_ld; op.x_goff = op.Cin;
+        op.out_buf = BUF_EXT_OUT; op.out_nct = true; op.ldy = op.Cout; op.y_goff = op.Cout;
+        if (op.Cout != c.code_dim) return h->fail("projector: code_dim must be a multiple of 32");
+        h->enc_ops.push_back(std::move(op));
+    }
+    if (build_symad_decoder(h)) return 1;
     // ---- residual VQ (layers/vq_module.py)
     const int nq = c.codebook_num, D = c.code_dim, N = c.codebook_size;
     if (N != 1024) return h->fail("RVQ: only codebook_size=1024 is built");
@@ -1220,8 +1247,18 @@ int build_hifigan(adec_handle* h) {
 int hop_of(const adec_handle* h) {
     int hop = 1;
     if (h->cfg.model_type == ADEC_MODEL_SYMAD) for (int i = 0; i < h->cfg.n_enc; ++i) hop *= h->cfg.enc_strides[i];
+    else if (h->cfg.model_type == ADEC_MODEL_SYMAD_DECODER) for (int i = 0; i < h->cfg.n_dec; ++i) hop *= h->cfg.dec_strides[i];
     else for (int i = 0; i < h->cfg.n_up; ++i) hop *= h->cfg.upsample_scales[i];
     return hop;
+}
+
+// The entry points that need the encoder, projector or RVQ: a full symAD handle only
+int need_full_symad(adec_handle* h, const std::string& what) {
+    if (h->cfg.model_type == ADEC_MODEL_SYMAD) return 0;
+    if (h->cfg.model_type == ADEC_MODEL_SYMAD_DECODER)
+        return h->fail(what + ": a symAD decoder-only handle (ADEC_MODEL_SYMAD_DECODER) has no encoder, projector or RVQ; use a full symAD "
+                              "handle (ADEC_MODEL_SYMAD)");
+    return h->fail(what + ": not a symAD handle");
 }
 
 struct DeviceGuard {
@@ -1275,14 +1312,17 @@ int adec_create(const adec_config* cfg, int device, adec_handle** out) {
         delete h;
         return 1;
     }
-    if (h->bf16 && (cfg->model_type != ADEC_MODEL_HIFIGAN || h->engine != 2)) {
-        g_create_error = "compute_dtype = bf16 is built for the HiFi-GAN vocoder on the f16 tensor-core engine only (the encoder, projector and RVQ "
-                         "must stay fp32-grade for bit-identical indices)";
+    if (h->bf16 && ((cfg->model_type != ADEC_MODEL_HIFIGAN && cfg->model_type != ADEC_MODEL_SYMAD_DECODER) || h->engine != 2)) {
+        g_create_error = "compute_dtype = bf16 is built for the decoder handles - the HiFi-GAN vocoder and the symAD decoder-only handle "
+                         "(ADEC_MODEL_SYMAD_DECODER) - on the f16 tensor-core engine only (the encoder, projector and RVQ of a full symAD "
+                         "handle must stay fp32-grade for bit-identical indices)";
         delete h;
         return 1;
     }
-    if (h->act_bf16 && cfg->in_channels % 8) {      // a bf16 zq row must be whole 16-byte vectors
-        g_create_error = "compute_dtype = 2 needs in_channels to be a multiple of 8";
+    const int zq_dim = cfg->model_type == ADEC_MODEL_SYMAD_DECODER ? cfg->code_dim : cfg->in_channels;
+    if (h->act_bf16 && zq_dim % 8) {      // a bf16 zq row must be whole 16-byte vectors
+        g_create_error = cfg->model_type == ADEC_MODEL_SYMAD_DECODER ? "compute_dtype = 2 needs code_dim to be a multiple of 8"
+                                                                     : "compute_dtype = 2 needs in_channels to be a multiple of 8";
         delete h;
         return 1;
     }
@@ -1330,6 +1370,7 @@ int adec_finalize(adec_handle* h) {
     DeviceGuard dg(h->device);
     int rc = h->cfg.model_type == ADEC_MODEL_SYMAD ? build_symad(h)
            : h->cfg.model_type == ADEC_MODEL_HIFIGAN ? build_hifigan(h)
+           : h->cfg.model_type == ADEC_MODEL_SYMAD_DECODER ? build_symad_decoder_only(h)
            : h->fail("unknown model_type");
     if (rc) return rc;
     for (const auto& kv : h->tensors)   // load_state_dict(strict=True): unexpected keys are an error
@@ -1415,7 +1456,7 @@ int adec_reset(adec_handle* h, void* stream) {
 }
 
 int adec_frames_for(const adec_handle* h, int T) {
-    if (!h || h->cfg.model_type != ADEC_MODEL_SYMAD) return -1;
+    if (!h || (h->cfg.model_type != ADEC_MODEL_SYMAD && h->cfg.model_type != ADEC_MODEL_SYMAD_DECODER)) return -1;
     int t = T;
     for (int i = 0; i < h->cfg.n_enc; ++i) t = (t - 1) / h->cfg.enc_strides[i] + 1;
     return t;
@@ -1461,7 +1502,7 @@ static int run_call(adec_handle* h, const Call& c, const void* in, int B, int T,
     static const char* const kModeName[] = {"", "_offline", "_offline_varlen", "_streams"};
     const std::string base = std::string(c.decode ? "decode" : "encode") + kModeName[c.mode];
     const std::string name = base + (c.bf16_io ? "_bf16" : "");
-    if (!c.decode && h->cfg.model_type != ADEC_MODEL_SYMAD) return h->fail(name + ": not a symAD handle");
+    if (!c.decode && need_full_symad(h, name)) return 1;
     if (h->act_bf16 && !c.bf16_io)
         return h->fail(fmt("%s: this handle has bf16 activations (compute_dtype 2); call adec_%s_bf16 with bf16 zq / y", name.c_str(),
                            base.c_str()));
@@ -1627,7 +1668,7 @@ cudaError_t launch_rvq_best(const adec_handle* h, const RvqArgs& a, cudaStream_t
 static int quantize_common(adec_handle* h, const float* z, int B, int F, int64_t* idx, uint8_t* packed, float* zq, bool fwd,
                            void* stream) {
     if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    if (h->cfg.model_type != ADEC_MODEL_SYMAD) return h->fail("quantize: not a symAD handle");
+    if (need_full_symad(h, "quantize")) return 1;
     if (B < 1 || F < 1) return h->fail("quantize: empty input");
     if (!idx && !packed && !zq) return h->fail("quantize: no output requested");
     DeviceGuard dg(h->device);
@@ -1651,7 +1692,7 @@ int adec_quantize_forward(adec_handle* h, const float* z, int B, int F, int64_t*
 
 int adec_zq_moments(adec_handle* h, const float* zq, const int* frames, int B, double* sum, double* m2, void* stream) {
     if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    if (h->cfg.model_type != ADEC_MODEL_SYMAD) return h->fail("zq_moments: not a symAD handle");
+    if (need_full_symad(h, "zq_moments")) return 1;
     if (varlen_args(h, "zq_moments", frames, B)) return 1;
     if (!zq || !sum || !m2) return h->fail("zq_moments: zq, sum and m2 must be given");
     if ((uintptr_t)zq % 16) return h->fail("zq_moments: zq must be 16-byte aligned");
@@ -1681,7 +1722,7 @@ int adec_quantize(adec_handle* h, const float* z, int B, int F, int64_t* idx, vo
 
 static int lookup_common(adec_handle* h, const int64_t* idx, const uint8_t* packed, int B, int F, float* zq, void* stream) {
     if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    if (h->cfg.model_type != ADEC_MODEL_SYMAD) return h->fail("lookup: not a symAD handle");
+    if (need_full_symad(h, "lookup")) return 1;
     if (B < 1 || F < 1) return h->fail("lookup: empty input");
     DeviceGuard dg(h->device);
     LookupArgs a{};
@@ -1709,6 +1750,7 @@ int adec_codec_host(adec_handle* enc, adec_handle* dec, const float* x_host, int
     if (enc->device != dec->device) return enc->fail("codec_host: handles on different devices");
     if (dec->act_bf16) return enc->fail("codec_host: the decoder has bf16 activations (compute_dtype 2), which the host path does not carry; "
                                         "use compute_dtype 0 or 1, or adec_decode_bf16 on device buffers");
+    if (need_full_symad(enc, "codec_host (enc)")) return 1;
     DeviceGuard dg(enc->device);
     cudaStream_t s = (cudaStream_t)stream;
     const int F = adec_frames_for(enc, T);
@@ -1744,7 +1786,7 @@ int adec_codec_host(adec_handle* enc, adec_handle* dec, const float* x_host, int
 
 static int pack_common(adec_handle* h, const char* what, int64_t* idx, int B, int F, uint8_t* packed, void* stream, bool pack) {
     if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    if (h->cfg.model_type != ADEC_MODEL_SYMAD) return h->fail(std::string(what) + ": not a symAD handle");
+    if (need_full_symad(h, what)) return 1;
     if (B < 1 || F < 1) return h->fail(std::string(what) + ": empty input");
     if (h->cfg.codebook_size < 2 || h->cfg.codebook_size > 65536) return h->fail(std::string(what) + ": codebook_size must be in [2, 65536]");
     DeviceGuard dg(h->device);
@@ -2180,7 +2222,10 @@ int adec_test_conv_op(int device, const adec_test_op* d, int mode, int n_calls, 
         g_create_error = "adec_test_conv_op: bad argument";
         return 1;
     }
-    adec_config cfg{};      // a symAD handle: fp32 activations, the engine ADEC_CONV_PATH names
+    // fp32: a symAD handle, the engine ADEC_CONV_PATH names; bf16: a symAD decoder-only handle with that compute_dtype (f16 engine)
+    adec_config cfg{};
+    cfg.model_type = d->compute_dtype ? ADEC_MODEL_SYMAD_DECODER : ADEC_MODEL_SYMAD;
+    cfg.compute_dtype = d->compute_dtype;
     adec_handle* h = nullptr;
     if (adec_create(&cfg, device, &h)) return 1;
     DeviceGuard dg(device);
@@ -2224,6 +2269,7 @@ int adec_test_conv_op(int device, const adec_test_op* d, int mode, int n_calls, 
                             d->pre_act, d->slope);
         break;
     case ADEC_TEST_STEM:     // through the state dict, as build_symad builds encoder.conv
+        if (h->bf16) { rc = h->fail("test_conv_op: the stem is fp32-grade only (compute_dtype 0)"); break; }
         h->tensors["test.conv.weight"] = tensor({32, 1, 7}, d->w);
         if (d->bias) h->tensors["test.conv.bias"] = tensor({32}, d->bias);
         rc = build_stem(h, &ops[0], "test", 32);

@@ -14,7 +14,8 @@
 //     fp16 and tf32 both carry 11 significand bits, so this is as accurate as 3xTF32, at half the operand bytes per MAC.
 //     Range: |a| < 65504 (checked in the epilogue, ConvArgs::err).
 //   PREC_TF32 (ADEC_CONV_PATH=tf32): a = A_hi + A_lo, w = W_hi + W_lo in tf32; A_lo W_hi + A_hi W_lo + A_hi W_hi.  No range limit.
-//   PREC_BF16 (the HiFi-GAN vocoder's bf16 mode): bf16 operands, one product.
+//   PREC_BF16 (the bf16 modes of the HiFi-GAN vocoder and the symAD decoder-only handle): bf16 operands, one product.  In the fused
+//     residual unit the intermediate operand is bf16_rne(ELU(fp32 sum of the dilated conv)), rounded once by split2.
 //
 // The tensor core's fp32 accumulation truncates at every step, which over the hundreds of steps of a long-K conv becomes a 1e-5-level
 // systematic shrink - enough to flip nearest-codeword decisions.  So accumulation is GROUPED: one group = one 32-channel piece x up to
@@ -274,7 +275,8 @@ __device__ __forceinline__ const XT* slot_hist(const ConvArgs& a, int u, int i, 
     return base + (((e >> 1) * a.P + i) * a.st_ld + c);
 }
 
-// BST: activations, causal state, residual and output stored as bf16 in HBM (bf16 operands only; no 4-channel strided convs)
+// BST: activations, causal state, residual and output stored as bf16 in HBM (bf16 operands only; no 4-channel strided convs).  The
+// fused residual unit reads its skip, its own input, as stored.
 // VL: utterances of different lengths in one stacked row space (ConvArgs::vl_in / vl_out), zero history, no state written; a separate
 // instantiation, so that the uniform kernels keep their code.  With ConvArgs::vl_slot set (a runtime branch, not another instantiation)
 // each utterance is a chunk of one stream slot: history from the slot, new state written back to it.
@@ -282,7 +284,7 @@ __device__ __forceinline__ const XT* slot_hist(const ConvArgs& a, int u, int i, 
 // (no VL, no stacked rows), which the host guarantees.
 template <int NT, bool FUSE, int PRE, int PREC, bool BST, bool VL = false, bool PAIR = false>
 __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(const ConvArgs a, int n_xtiles, int n_ytiles, int n_tiles) {
-    static_assert(!BST || (PREC == PREC_BF16 && !FUSE), "bf16 storage is built for the non-fused bf16-operand kernels");
+    static_assert(!BST || PREC == PREC_BF16, "bf16 storage is built for the bf16-operand kernels");
     static_assert(!PAIR || (NT == 32 && FUSE && PREC == PREC_F16 && !BST && !VL), "the paired kernel is built for the fused fp16-split RU(32)");
     using Cfg = WgCfg<NT, PREC>;
     using XT = typename std::conditional<BST, __nv_bfloat16, float>::type;

@@ -14,7 +14,8 @@
  *     (adec_last_error() gives the message).  Nothing throws, nothing falls back to CPU.
  *   - all data pointers of the *_dev entry points are DEVICE pointers on the handle's GPU;
  *     `stream` is a cudaStream_t passed as void* (NULL = legacy default stream).
- *   - activations are fp32, except on HiFi-GAN handles with compute_dtype 2 (the *_bf16 decode entry points).  Layouts at
+ *   - activations are fp32, except on decoder handles (HiFi-GAN, symAD decoder-only) with compute_dtype 2 (the *_bf16 decode entry
+ *     points).  Layouts at
  *     the boundary are the reference's own
  *     (SURVEY.md A.3):  x (B,1,T)   z (B,64,F) channels-first   idx (Nq,B,F) int64 flat
  *     (+1024*i already added)   zq (B,F,64) channels-last   y (B,1,F*hop).
@@ -38,7 +39,13 @@ typedef struct adec_handle adec_handle;
 
 enum adec_model_type {
     ADEC_MODEL_SYMAD = 0,      /* models/autoencoder/AudioDec.py:166 StreamGenerator (codec='audiodec') */
-    ADEC_MODEL_HIFIGAN = 1     /* models/vocoder/HiFiGAN.py:222 StreamGenerator, MultiGroupConv1d fusion (AD v1) */
+    ADEC_MODEL_HIFIGAN = 1,    /* models/vocoder/HiFiGAN.py:222 StreamGenerator, MultiGroupConv1d fusion (AD v1) */
+    ADEC_MODEL_SYMAD_DECODER = 2   /* the decoder of a symAD StreamGenerator alone: what the receiver's `decoder` object runs
+                                      (initial_decoder / decode, utils/audiodec.py:104-106).  Same config as ADEC_MODEL_SYMAD; loads a
+                                      full generator state dict (decoder.* strict, encoder.* / projector.* / quantizer.* ignored).  The
+                                      decode entry points, the state calls, adec_hop_length / adec_frames_for and the diagnostics work on
+                                      it; encode, quantize*, lookup*, pack / unpack and adec_zq_moments fail.  compute_dtype 1 and 2 on
+                                      the f16 engine, as for HiFi-GAN. */
 };
 
 /* POD mirror of config.yml `generator_params` (exp/.../config.yml:102-134 resp. :102-130). */
@@ -64,7 +71,8 @@ typedef struct adec_config {
     int n_resblocks;  int resblock_kernel_sizes[ADEC_MAX_STAGES];   /* AD v0: MultiReceptiveField, one residual block per kernel size */
     /* appended in round 2 */
     int compute_dtype;                                     /* 0 = fp32-grade (default); 1 = bf16 conv operands with fp32 accumulation, HiFi-GAN vocoder
-                                                              only: what `decoder.to(torch.bfloat16)` asks of the reference (BASELINE configs[2]);
+                                                              and symAD decoder-only handles: what `decoder.to(torch.bfloat16)` asks of the
+                                                              reference (BASELINE configs[2]);
                                                               2 = as 1, and every activation, the causal state and the decode input / output are
                                                               bf16 in memory (the reference's bf16 data layout and dtype contract): decode with
                                                               adec_decode_bf16 / adec_decode_offline_bf16.  1 and 2 need the f16 engine. */
@@ -121,7 +129,8 @@ int adec_lookup(adec_handle *h, const int64_t *idx, int B, int F, float *zq, voi
 /* StreamGenerator.decode (AudioDec.py:246-247 / HiFiGAN.py:268-273): zq (B,F,code_dim) -> y (B,1,F*hop). */
 int adec_decode(adec_handle *h, const float *zq, int B, int F, float *y, void *stream);
 
-/* Same, for a HiFi-GAN handle with compute_dtype 2: zq (B,F,in_channels) and y (B,1,F*hop) are bf16 (raw 16-bit words), both
+/* Same, for a HiFi-GAN or symAD decoder-only handle with compute_dtype 2: zq (B,F,in_channels resp. code_dim) and y (B,1,F*hop) are
+ * bf16 (raw 16-bit words), both
  * 16-byte aligned.  adec_decode on such a handle fails, and so does adec_decode_bf16 on any other handle. */
 int adec_decode_bf16(adec_handle *h, const uint16_t *zq, int B, int F, uint16_t *y, void *stream);
 
@@ -173,7 +182,8 @@ int adec_hop_length(const adec_handle *h);
 /* -- whole path with HOST buffers (what demoFile.py:55-62 does around the four calls) ------- */
 /* x_host (B,1,T) -> idx_host (Nq,B,F) (may be NULL) and y_host (B,1,F*hop).  Copies H2D, runs
  * enc.encode -> enc.quantize -> enc.lookup -> dec.decode on `stream`, copies D2H and synchronises.
- * `enc` must be a symAD handle; `dec` a symAD or HiFi-GAN handle (may equal enc) with fp32 activations (compute_dtype 0 or 1). */
+ * `enc` must be a full symAD handle; `dec` a symAD, symAD decoder-only or HiFi-GAN handle (may equal enc) with fp32 activations
+ * (compute_dtype 0 or 1). */
 int adec_codec_host(adec_handle *enc, adec_handle *dec, const float *x_host, int B, int T,
                     int64_t *idx_host, float *y_host, void *stream);
 
@@ -182,7 +192,7 @@ int adec_codec_host(adec_handle *enc, adec_handle *dec, const float *x_host, int
  * (bin/stream.py:224).  Packed frame = Nq local indices (idx - i*codebook_size) of ceil(log2 codebook_size) bits each,
  * stage 0 first, little-endian bit order, zero-padded to whole bytes: 8 x 10 bit = 10 bytes / frame = 12.8 kbit/s at
  * hop 300 / 48 kHz.  idx (Nq,B,F) int64 flat <-> packed (B,F,adec_packed_frame_bytes) uint8, device pointers. */
-int adec_packed_frame_bytes(const adec_handle *h);       /* -1 if h is not a symAD handle */
+int adec_packed_frame_bytes(const adec_handle *h);       /* -1 if h is not a full symAD handle (ADEC_MODEL_SYMAD) */
 int adec_pack_indices(adec_handle *h, const int64_t *idx, int B, int F, uint8_t *packed, void *stream);
 int adec_unpack_indices(adec_handle *h, const uint8_t *packed, int B, int F, int64_t *idx, void *stream);
 /* lookup straight from the packed bitstream (unpack fused into lookup): packed (B,F,bytes) -> zq (B,F,code_dim) */
@@ -252,8 +262,9 @@ int adec_test_vocoder_layer(int device, int compute_dtype, int kind, const void 
                             int pre_act, float slope, const float *mean, const float *scale, const void *res, int offline,
                             void *state, void *y);
 
-/* One fp32-grade op (the engine ADEC_CONV_PATH names) built by the model builders and run through the codec call path in any call
- * mode, so that tests can check every row space layer by layer.  HOST pointers, fp32, channels-first per utterance. */
+/* One op built by the model builders and run through the codec call path in any call mode, so that tests can check every row space
+ * layer by layer: fp32-grade (the engine ADEC_CONV_PATH names) or, with compute_dtype 1 / 2, bf16.  HOST pointers, channels-first per
+ * utterance. */
 enum { ADEC_TEST_CONV = 0, ADEC_TEST_RU = 1, ADEC_TEST_CONVTR = 2, ADEC_TEST_STEM = 3, ADEC_TEST_HEAD = 4 };
 typedef struct adec_test_op {
     int kind;          /* ADEC_TEST_*                                                                                              */
@@ -265,9 +276,13 @@ typedef struct adec_test_op {
     int out_nct;       /* conv: write channels-first, as the projector writes z                                                  */
     int post_tanh;     /* head: tanh after the conv                                                                             */
     const float *w, *w2, *bias, *mean, *scale;   /* bias, mean, scale may be NULL                                             */
+    int compute_dtype; /* 0: the fp32-grade engine ADEC_CONV_PATH names; 1 / 2: the op as a symAD decoder-only handle with that
+                        * compute_dtype builds it (f16 engine; no stem, no strided conv): x, res, state and y are fp32 for 0 and 1 and
+                        * bf16 words for 2                                                                                          */
 } adec_test_op;
-/* launch records: 8 ints {launch kind, NT (FFMA: output tile), fuse, pre_act, prec (wg_conv.cuh PREC_*), varlen, paired, stacked} */
-enum { ADEC_TEST_REC = 8, ADEC_TEST_LAUNCH_TC = 0, ADEC_TEST_LAUNCH_FFMA = 1, ADEC_TEST_LAUNCH_STEM = 2, ADEC_TEST_LAUNCH_HEAD = 3 };
+/* launch records: 9 ints {launch kind, NT (FFMA: output tile), fuse, pre_act, prec (wg_conv.cuh PREC_*), varlen, paired, stacked,
+ * bf16 storage (BST)} */
+enum { ADEC_TEST_REC = 9, ADEC_TEST_LAUNCH_TC = 0, ADEC_TEST_LAUNCH_FFMA = 1, ADEC_TEST_LAUNCH_STEM = 2, ADEC_TEST_LAUNCH_HEAD = 3 };
 /* mode: 0 = stream (adec_encode: B = n_streams streams advanced by equal lengths, stacked rows unless ADEC_STACK_ROWS=0), 1 = offline
  * (zero history, first-row replication in transposed convs), 2 = varlen offline, 3 = stream slots (`streams`: the B distinct streams of
  * n_streams that each call advances).  n_calls consecutive calls on one handle: lengths (n_calls, B) are input rows per utterance
