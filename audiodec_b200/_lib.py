@@ -85,6 +85,11 @@ SYMBOLS = {
     "adec_decode_streams": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),
     "adec_decode_streams_bf16": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),
     "adec_copy_stream_state": (c_int, [c_void_p, c_int, ctypes.POINTER(c_int), c_int, c_void_p]),
+    "adec_state_entries": (c_int, [c_void_p]),
+    "adec_state_entry": (c_int, [c_void_p, c_int, ctypes.POINTER(c_char_p), ctypes.POINTER(c_int), ctypes.POINTER(c_int)]),
+    "adec_stream_state_elems": (c_int64, [c_void_p]),
+    "adec_get_stream_state": (c_int, [c_void_p, ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),
+    "adec_set_stream_state": (c_int, [c_void_p, ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),
     "adec_frames_for": (c_int, [c_void_p, c_int]),
     "adec_hop_length": (c_int, [c_void_p]),
     "adec_codec_host": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),

@@ -15,6 +15,8 @@ Differences from the reference, all extensions:
     ``ResidualVQ.forward_index`` yields before its ``squeeze(1)``, vq_module.py:148-149) and ``lookup``
     returns (B,F,D).
   * there is no CPU path: ``.to('cpu')`` raises.
+  * ``stream_state`` / ``load_stream_state`` move one stream's causal state out of and into any stream of a handle (of the same
+    config and dtype, on any GPU); ``state_dict()`` returns the live state of every stream as the reference's pad_buffers.
   * ``set_activation_dtype(torch.bfloat16)`` on a decoder-only generator (``HiFiGANStreamGenerator``,
     ``SymADDecoderStreamGenerator``) keeps every activation, the causal state and the decode input / output in bf16 (the data
     layout and dtype contract of the reference's ``decoder.to(torch.bfloat16)``); plain ``.to(torch.bfloat16)`` rounds only the
@@ -64,6 +66,31 @@ def _int_array(values):
     return (ctypes.c_int * max(1, len(values)))(*values), len(values)
 
 
+def _stream_ids(streams):
+    """An int or an iterable of ints -> list of ints (the handle checks that they are distinct and in range)."""
+    if isinstance(streams, int):
+        return [streams]
+    ids = list(streams)
+    for s in ids:
+        if isinstance(s, bool) or not isinstance(s, int):
+            raise TypeError(f"audiodec_b200: stream ids must be ints, got {type(s).__name__}")
+    return ids
+
+
+def _check_state(state, n, elems, dtype, device):
+    """An imported state: a (n, elems) tensor of the handle's state dtype on the handle's device, returned contiguous and 16-byte aligned."""
+    if not isinstance(state, torch.Tensor):
+        raise TypeError(f"audiodec_b200: load_stream_state: expected a tensor, got {type(state).__name__}")
+    if state.device != device:
+        raise RuntimeError(f"audiodec_b200: load_stream_state: the state is on {state.device}, the codec on {device}; move it with .to()")
+    if state.dtype != dtype:
+        raise ValueError(f"audiodec_b200: load_stream_state: the state is {state.dtype}, this handle's state is {dtype}")
+    if tuple(state.shape) != (n, elems):
+        raise ValueError(f"audiodec_b200: load_stream_state: expected ({n}, {elems}) for {n} streams, got {tuple(state.shape)}")
+    state = state.contiguous()
+    return state.clone() if state.data_ptr() % 16 else state
+
+
 class _StreamGeneratorBase:
     """Common plumbing: deferred handle creation (weights arrive before the device is known, exactly
     like ``Generator(**params)`` -> ``load_state_dict`` -> ``.to(device)`` in the reference)."""
@@ -76,14 +103,36 @@ class _StreamGeneratorBase:
         self._device = None
         self._operand_mode = 0        # what .to(dtype) selected: 0 = fp32, 1 = bf16 conv operands
         self._act_bf16 = False        # decoders only (set_activation_dtype): bf16 activations, state and decode I/O = compute_dtype 2
+        self._layout = None           # state_layout, read from the handle once
 
     # the decoder-only generators (HiFi-GAN vocoder, symAD decoder) have the bf16 modes; a full symAD generator does not
     _bf16_modes = False
 
     # -- torch.nn.Module look-alikes ------------------------------------------------------------
     def load_state_dict(self, state_dict, strict=True):
+        """Weights, stats, codebooks and pad_buffers as the reference's state dict names them.  A pad_buffer (1, C, P) is every stream's
+        initial state; a batched one (B, C, P) with B > 1 (what state_dict() returns for B streams) gives stream b its row b: the handle
+        gets B streams in `.to(device)`."""
         self._sd = {k: v.detach().to(torch.float32).cpu().contiguous() for k, v in state_dict.items()}
         return self
+
+    def state_dict(self):
+        """Every key as loaded, except the pad_buffers of the layers the handle runs: those are the live causal state of every stream,
+        (n_streams, C, P) device tensors (fp32; bf16 with bf16 activations, as `.to(torch.bfloat16)` stores them in the reference), read
+        in one launch.  `load_state_dict` of the result into a fresh generator resumes every stream exactly."""
+        if self._sd is None:
+            raise RuntimeError("load_state_dict must be called before state_dict")
+        live = {}
+        if self._h is not None and self.state_layout:
+            n = self.n_streams
+            st = self.stream_state(range(n))
+            off = 0
+            for key, c, p in self.state_layout:
+                live[key] = st[:, off:off + c * p].view(n, c, p)
+                off += c * p
+        out = {k: live.pop(k, v) for k, v in self._sd.items()}
+        out.update(live)
+        return out
 
     def eval(self):
         return self
@@ -111,8 +160,30 @@ class _StreamGeneratorBase:
             shape = (ctypes.c_int64 * t.dim())(*t.shape)
             _check(self._lib.adec_set_tensor(h, key.encode(), _ptr(t), shape, t.dim()), h)
         _check(self._lib.adec_finalize(h), h)
-        self._sd = None
+        self._load_batched_pad_buffers()
         return self
+
+    def _load_batched_pad_buffers(self):
+        """(B, C, P) pad_buffers with B > 1: the handle (which started every stream from row 0) gets B streams, and stream b row b of
+        each such buffer, in one import."""
+        names = {key for key, _, _ in self.state_layout}
+        rows = {k: v for k, v in self._sd.items() if k in names and v.dim() == 3 and v.size(0) > 1}
+        if not rows:
+            return
+        sizes = {v.size(0) for v in rows.values()}
+        if len(sizes) != 1:
+            raise ValueError(f"audiodec_b200: load_state_dict: batched pad_buffers disagree on the number of streams {sorted(sizes)}")
+        b = sizes.pop()
+        self._batch(b)
+        st = self.stream_state(range(b))
+        off = 0
+        for key, c, p in self.state_layout:
+            if key in rows:
+                if tuple(rows[key].shape) != (b, c, p):
+                    raise ValueError(f"audiodec_b200: load_state_dict: {key} has shape {tuple(rows[key].shape)}, the handle runs {(b, c, p)}")
+                st[:, off:off + c * p] = rows[key].reshape(b, c * p).to(self._device, st.dtype)
+            off += c * p
+        self.load_stream_state(range(b), st)
 
     def _set_dtype(self, dtype):
         """`module.to(torch.bfloat16)` of the reference: only the decoder-only generators (HiFi-GAN vocoder, symAD decoder) have a
@@ -237,6 +308,49 @@ class _StreamGeneratorBase:
         dst = [dst] if isinstance(dst, int) else list(dst)
         arr, n = _int_array(dst)
         _check(self._lib.adec_copy_stream_state(self._h, int(src), arr, n, self._stream()), self._h)
+
+    # ---- stream state out of and into the handle (adec_get_stream_state / adec_set_stream_state)
+    @property
+    def state_layout(self):
+        """[(key, C, P)]: the reference pad_buffers the handle runs, in the order a stream's state vector holds them, each (C, P)
+        channels-first."""
+        self._ready()
+        if self._layout is None:
+            key, c, p = ctypes.c_char_p(), ctypes.c_int(), ctypes.c_int()
+            out = []
+            for i in range(self._lib.adec_state_entries(self._h)):
+                _check(self._lib.adec_state_entry(self._h, i, ctypes.byref(key), ctypes.byref(c), ctypes.byref(p)), self._h)
+                out.append((key.value.decode(), c.value, p.value))
+            self._layout = out
+        return self._layout
+
+    @property
+    def state_dtype(self):
+        """dtype of the exported state: bf16 with bf16 activations, fp32 otherwise."""
+        return torch.bfloat16 if self._act_bf16 else torch.float32
+
+    def stream_state(self, streams):
+        """The current causal state of `streams` (an int or a list of distinct ids) -> (n, S) device tensor, row i stream streams[i]'s
+        state_layout entries one after the other.  Asynchronous on the current stream; the streams' state is left as it is."""
+        self._ready()
+        ids = _stream_ids(streams)
+        arr, n = _int_array(ids)
+        out = torch.empty(n, int(self._lib.adec_stream_state_elems(self._h)), device=self._device, dtype=self.state_dtype)
+        _check(self._lib.adec_get_stream_state(self._h, arr, n, _ptr(out), self._stream()), self._h)
+        return out
+
+    def load_stream_state(self, streams, state, layout=None):
+        """Import `state` (n, S), as stream_state returns it, into `streams`: stream streams[i] continues exactly as the exported stream
+        would have.  `layout` (optional): the exporting handle's state_layout, checked against this handle's.  Streams not listed keep
+        their state."""
+        self._ready()
+        ids = _stream_ids(streams)
+        if layout is not None and [tuple(e) for e in layout] != [tuple(e) for e in self.state_layout]:
+            raise ValueError(f"audiodec_b200: load_stream_state: the state was exported by a handle with another state layout "
+                             f"({len(layout)} entries; this handle has {len(self.state_layout)})")
+        state = _check_state(state, len(ids), int(self._lib.adec_stream_state_elems(self._h)), self.state_dtype, self._device)
+        arr, n = _int_array(ids)
+        _check(self._lib.adec_set_stream_state(self._h, arr, n, _ptr(state), self._stream()), self._h)
 
     # ---- decode plumbing shared by both generators
     def _fn(self, name):

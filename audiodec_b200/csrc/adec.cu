@@ -176,6 +176,20 @@ float tf32_round_host(float x) {   // cvt.rna.tf32.f32: round to nearest (ties a
 enum OpKind { OP_STEM, OP_CONV, OP_HEAD };
 enum { BUF_EXT_IN = -10, BUF_EXT_OUT = -11, BUF_NONE = -1 };
 
+// One reference pad_buffer an op's causal state holds (the state map, adec_state_entry): the key (1, C, P) channels-first is rows
+// [zrows, zrows + P) of the op's (P_op, st_C) channels-last state, its channel g * cg + c at column col0 + g * gstride + c.
+//   plain layers:       groups 1, col0 0, zrows 0
+//   MultiGroupConv1d:   groups G; convs1.0 reads one shared input, so its key holds G copies of it (x.repeat, multi_fusion.py:134):
+//                       gstride 0, export writes every copy, import reads copy 0
+//   AD v0 (synthesize_mrf_as_groups): one key per block b with kernel k_b; the op keeps (K - 1) dil rows, the key the last
+//                       (k_b - 1) dil of them (zrows = (K - k_b) dil) in group b (col0 = b Cin).  Import zeroes the older rows, which
+//                       only meet zero taps.  convs1.0's blocks share one input: only the block with the largest kernel is imported.
+struct StKey {
+    std::string key;
+    int C = 0, P = 0, groups = 1, cg = 0, col0 = 0, gstride = 0, zrows = 0;
+    bool import = true;
+};
+
 struct Op {
     OpKind kind = OP_CONV;
     std::string name;
@@ -206,6 +220,7 @@ struct Op {
     int st_C = 0, st_groups = 1;
     float* st[2] = {nullptr, nullptr};
     int cur = 0;
+    std::vector<StKey> keys;    // the reference pad_buffers this op's state holds
     // wiring
     int in_buf = BUF_NONE, out_buf = BUF_NONE, res_buf = BUF_NONE;
     int ldx = 0, x_goff = 0, ldy = 0, y_goff = 0, ldr = 0, r_goff = 0;
@@ -263,6 +278,13 @@ struct adec_handle {
     DevBuf mom_tab;               // row offsets of the last adec_zq_moments call (ints)
     SlotBits enc_slots, dec_slots;
     DevBuf slot_tab;              // stream pairs of the last state copy (ints)
+    // the state map: every reference pad_buffer the handle runs, in plan order (encoder ops, then decoder ops), one stream's exported
+    // vector holding them one after the other; st_tiles: the 32 x 32 tiles of the export / import kernels (adec_get_stream_state)
+    struct StMapEntry { int list, op, k; long long off; };
+    std::vector<StMapEntry> st_map;
+    std::vector<int4> st_tiles;
+    long long st_elems = 0;
+    DevBuf st_tab;                // entries, tiles and streams of the last export / import
     long long* hidx = nullptr;
     size_t hidx_cap = 0;
     std::vector<int>* launch_log = nullptr;   // run_ops appends one ADEC_TEST_REC record per launch here (adec_record_launches)
@@ -604,23 +626,37 @@ int alloc_state(adec_handle* h, Op* op, int n_streams) {
     return 0;
 }
 
-// pad_buffer (1, C, P) from the state dict -> (P, st_C) channels-last initial state.  The reference stores in pad_buffer the tail of
-// what it feeds to conv.inference, i.e. values AFTER the pre-activation / normalisation (residual_unit.py:79 `conv1.inference(
-// self.activation(x))`, HiFiGAN.py:276-284,288), and the kernels keep exactly that: state rows are never activated again (only chunk
-// rows are, while the window is written), so checkpoint values are copied as they are.
-void load_pad_buffer(adec_handle* h, Op* op, const std::string& key, int c_real) {
-    const HostTensor* pb = find(h, key);
-    if (!pb || pb->shape.size() != 3 || op->P == 0) return;
+// Register reference key `key` of op `op` (see StKey; the key's reference shape is (1, groups * cg, P)) and load it from the state dict
+// as the op's initial state.  The reference stores in pad_buffer the tail of what it feeds to conv.inference, i.e. values AFTER the
+// pre-activation / normalisation (residual_unit.py:79 `conv1.inference(self.activation(x))`, HiFiGAN.py:276-284,288), and the kernels keep
+// exactly that: state rows are never activated again (only chunk rows are, while the window is written), so checkpoint values are copied as
+// they are.  A batched (B, C, P) buffer loads its row 0 here; the Python layer imports every row per stream (load_state_dict).
+void add_pad_buffer(adec_handle* h, Op* op, StKey k) {
+    if (!k.P) k.P = op->P - k.zrows;
+    if (!k.C) k.C = k.groups * k.cg;
+    const HostTensor* pb = find(h, k.key);
+    op->keys.push_back(k);
+    if (!k.import || !pb || pb->shape.size() != 3 || op->P == 0) return;
     const int C = (int)pb->shape[1], P = (int)pb->shape[2];
-    if (P != op->P) return;
+    if (P != k.P) return;
     bool any = false;
-    for (float v : pb->data) any |= (v != 0.f);
+    for (int64_t i = 0; i < (int64_t)C * P && i < pb->numel(); ++i) any |= (pb->data[i] != 0.f);
     if (!any) return;
-    op->hstate.assign((size_t)op->P * op->st_C, 0.f);
-    const int groups = op->st_groups, cg = c_real;   // real channels per group
+    if (op->hstate.empty()) op->hstate.assign((size_t)op->P * op->st_C, 0.f);
+    const int groups = k.gstride ? k.groups : 1;      // a shared input: copy 0
     for (int g = 0; g < groups; ++g)
-        for (int c = 0; c < cg && g * cg + c < C; ++c)
-            for (int p = 0; p < P; ++p) op->hstate[(size_t)p * op->st_C + g * op->Cin + c] = pb->data[((size_t)(g * cg + c)) * P + p];
+        for (int c = 0; c < k.cg && g * k.cg + c < C; ++c)
+            for (int p = 0; p < P; ++p)
+                op->hstate[(size_t)(k.zrows + p) * op->st_C + k.col0 + g * k.gstride + c] = pb->data[((size_t)(g * k.cg + c)) * P + p];
+}
+
+// a plain layer, or a MultiGroupConv1d conv (op->G groups of c_real channels; shared_in: copies of one input)
+void load_pad_buffer(adec_handle* h, Op* op, const std::string& key, int c_real) {
+    StKey k;
+    k.key = key; k.cg = c_real;
+    k.groups = op->kind == OP_CONV ? op->G : 1;
+    k.gstride = op->shared_in ? 0 : op->Cin;
+    add_pad_buffer(h, op, k);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -913,10 +949,7 @@ int build_stem(adec_handle* h, Op* op, const std::string& prefix, int cout) {
         for (int k = 0; k < 7; ++k) w[k * 32 + co] = W->data[co * 7 + k];
     if (dev_upload(h, &op->w, w)) return 1;
     if (const HostTensor* b = find(h, prefix + ".conv.bias")) { if (dev_upload(h, &op->bias, b->data)) return 1; }
-    if (const HostTensor* pb = find(h, prefix + ".pad_buffer")) {
-        bool any = false; for (float v : pb->data) any |= v != 0.f;
-        if (any && pb->numel() == 6) op->hstate = pb->data;
-    }
+    load_pad_buffer(h, op, prefix + ".pad_buffer", 1);
     return 0;
 }
 
@@ -1138,7 +1171,6 @@ int synthesize_mrf_as_groups(adec_handle* h, int stage, int C, HostTensor W1[], 
                             W.data[((size_t)(b * C + co) * C + ci) * K + (K - kb) + k] = w.data[((size_t)co * C + ci) * kb + k];
                 if (const HostTensor* bb = find(h, pre + ".conv.bias"))
                     for (int co = 0; co < C; ++co) Bt.data[b * C + co] = bb->data[co];
-                find(h, pre + ".pad_buffer");   // zeros in every released checkpoint; the longer zero-tap history starts at zero too
             }
         }
     Wout->shape = {C, nb * C, 1};
@@ -1213,6 +1245,23 @@ int build_hifigan(adec_handle* h) {
             if (!mrf) {
                 load_pad_buffer(h, &o1, p1 + ".pad_buffer", cout);
                 load_pad_buffer(h, &o2, p2 + ".pad_buffer", cout);
+            } else {
+                // one key per block: the tail of the block's group (convs1.0: of the shared input, read from the largest kernel's block)
+                int kmax = 0;
+                for (int b = 1; b < G; ++b) if (c.resblock_kernel_sizes[b] > c.resblock_kernel_sizes[kmax]) kmax = b;
+                for (int which = 0; which < 2; ++which) {
+                    Op& o = which ? o2 : o1;
+                    for (int b = 0; b < G; ++b) {
+                        StKey k;
+                        k.key = fmt("blocks.%d.blocks.%d.convs%d.%d.pad_buffer", i, b, which + 1, j);
+                        k.cg = cout;
+                        k.P = (c.resblock_kernel_sizes[b] - 1) * o.dil;
+                        k.zrows = o.P - k.P;
+                        k.col0 = o.shared_in ? 0 : b * o.Cin;
+                        k.import = !o.shared_in || b == kmax;
+                        add_pad_buffer(h, &o, k);
+                    }
+                }
             }
             o1.in_buf = j == 0 ? A : Cc; o1.ldx = j == 0 ? cout : C3; o1.x_goff = j == 0 ? 0 : cout;
             o1.out_buf = Bb; o1.ldy = C3; o1.y_goff = cout;
@@ -1259,6 +1308,25 @@ int need_full_symad(adec_handle* h, const std::string& what) {
         return h->fail(what + ": a symAD decoder-only handle (ADEC_MODEL_SYMAD_DECODER) has no encoder, projector or RVQ; use a full symAD "
                               "handle (ADEC_MODEL_SYMAD)");
     return h->fail(what + ": not a symAD handle");
+}
+
+// The state map from the ops' keys, and the 32 x 32 (channel, row) tiles the export / import kernels run over
+void build_state_map(adec_handle* h) {
+    h->st_map.clear();
+    h->st_tiles.clear();
+    h->st_elems = 0;
+    for (int list = 0; list < 2; ++list) {
+        const std::vector<Op>& ops = list ? h->dec_ops : h->enc_ops;
+        for (int o = 0; o < (int)ops.size(); ++o)
+            for (int k = 0; k < (int)ops[o].keys.size(); ++k) {
+                const StKey& key = ops[o].keys[k];
+                const int e = (int)h->st_map.size();
+                h->st_map.push_back({list, o, k, h->st_elems});
+                h->st_elems += (long long)key.C * key.P;
+                for (int c0 = 0; c0 < key.C; c0 += 32)
+                    for (int r0 = 0; r0 < key.zrows + key.P; r0 += 32) h->st_tiles.push_back(make_int4(e, c0, r0, 0));
+            }
+    }
 }
 
 struct DeviceGuard {
@@ -1345,7 +1413,7 @@ void adec_destroy(adec_handle* h) {
         for (Op& op : *ops)
             for (int i = 0; i < 2; ++i) if (op.st[i]) cudaFree(op.st[i]);
     for (auto& b : h->ws) if (b.p) cudaFree(b.p);
-    for (DevBuf* b : {&h->hx, &h->hz, &h->hzq, &h->hy, &h->vl_tab, &h->mom_tab, &h->slot_tab}) if (b->p) cudaFree(b->p);
+    for (DevBuf* b : {&h->hx, &h->hz, &h->hzq, &h->hy, &h->vl_tab, &h->mom_tab, &h->slot_tab, &h->st_tab}) if (b->p) cudaFree(b->p);
     if (h->hidx) cudaFree(h->hidx);
     if (h->d_err) cudaFree(h->d_err);
     if (h->d_ktrace) cudaFree(h->d_ktrace);
@@ -1383,6 +1451,7 @@ int adec_finalize(adec_handle* h) {
     h->n_streams = 1;
     h->enc_slots.bit.assign(1, 0);
     h->dec_slots.bit.assign(1, 0);
+    build_state_map(h);
     h->tensors.clear();
     h->finalized = true;
     return 0;
@@ -1623,6 +1692,86 @@ int adec_copy_stream_state(adec_handle* h, int src, const int* dst, int n, void*
         if (sel) sb->dirty = true;
     }
     return 0;
+}
+
+// ---- stream state export / import: the state map (build_state_map) over the streams' current buffers
+int adec_state_entries(const adec_handle* h) { return h && h->finalized ? (int)h->st_map.size() : -1; }
+
+int adec_state_entry(const adec_handle* h, int i, const char** key, int* C, int* P) {
+    if (!h || !h->finalized || i < 0 || i >= (int)h->st_map.size()) return 1;
+    const auto& m = h->st_map[i];
+    const StKey& k = (m.list ? h->dec_ops : h->enc_ops)[m.op].keys[m.k];
+    if (key) *key = k.key.c_str();
+    if (C) *C = k.C;
+    if (P) *P = k.P;
+    return 0;
+}
+
+int64_t adec_stream_state_elems(const adec_handle* h) { return h && h->finalized ? h->st_elems : -1; }
+
+// One launch over every entry and every requested stream.  Each stream's state is read from / written to the buffer its slot bit names
+// (st[cur ^ bit]); neither cur nor the slot bits change, so an export sees exactly what the next call of any kind would read.
+static int stream_state_io(adec_handle* h, const char* name, const int* streams, int n, void* ext, bool import, void* stream) {
+    if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
+    if (n < 0) return h->fail(fmt("%s: n must be >= 0, got %d", name, n));
+    if (n == 0) return 0;
+    if (stream_args(h, name, streams, n)) return 1;
+    if (!ext) return h->fail(fmt("%s: the state buffer is NULL", name));
+    if ((uintptr_t)ext & 15) return h->fail(fmt("%s: the state buffer must be 16-byte aligned", name));
+    if (h->st_map.empty()) return 0;
+    std::vector<StateEntry> ents;
+    for (const auto& m : h->st_map) {
+        const Op& op = (m.list ? h->dec_ops : h->enc_ops)[m.op];
+        const StKey& k = op.keys[m.k];
+        StateEntry e{};
+        e.st[0] = op.st[op.cur]; e.st[1] = op.st[op.cur ^ 1];
+        e.per = (long long)op.P * op.st_C; e.off = m.off;
+        e.C = k.C; e.P = k.P; e.zrows = k.zrows; e.st_C = op.st_C; e.cg = k.cg; e.col0 = k.col0; e.gstride = k.gstride;
+        e.list = m.list;
+        e.wc = !k.import ? 0 : k.gstride == 0 ? k.cg : k.C;
+        ents.push_back(e);
+    }
+    std::vector<int> sv(3 * (size_t)n);
+    for (int i = 0; i < n; ++i) {
+        sv[3 * i] = streams[i];
+        sv[3 * i + 1] = h->enc_slots.bit.empty() ? 0 : h->enc_slots.bit[streams[i]];
+        sv[3 * i + 2] = h->dec_slots.bit.empty() ? 0 : h->dec_slots.bit[streams[i]];
+    }
+    // one upload: entries | tiles | streams (each part 16-byte aligned)
+    const size_t eb = ents.size() * sizeof(StateEntry), tb = h->st_tiles.size() * sizeof(int4), sb = sv.size() * sizeof(int);
+    std::vector<char> tab(eb + tb + sb);
+    memcpy(tab.data(), ents.data(), eb);
+    memcpy(tab.data() + eb, h->st_tiles.data(), tb);
+    memcpy(tab.data() + eb + tb, sv.data(), sb);
+    DeviceGuard dg(h->device);
+    if (ensure(h, h->st_tab, (tab.size() + 3) / 4)) return 1;
+    CK(h, cudaMemcpyAsync(h->st_tab.p, tab.data(), tab.size(), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    const char* d = reinterpret_cast<const char*>(h->st_tab.p);
+    StateArgs a{};
+    a.ent = reinterpret_cast<const StateEntry*>(d);
+    a.tiles = reinterpret_cast<const int4*>(d + eb);
+    a.streams = reinterpret_cast<const int*>(d + eb + tb);
+    a.n = n; a.ext = ext; a.S = h->st_elems;
+    a.err = import && h->engine == 2 && !h->bf16 ? h->d_err : nullptr;    // the fp16-split engine's range flag
+    const dim3 grid((unsigned)h->st_tiles.size(), (unsigned)std::min(n, 65535));
+    if (h->act_bf16) {
+        if (import) stream_state_kernel<uint16_t, true><<<grid, 256, 0, (cudaStream_t)stream>>>(a);
+        else stream_state_kernel<uint16_t, false><<<grid, 256, 0, (cudaStream_t)stream>>>(a);
+    } else {
+        if (import) stream_state_kernel<float, true><<<grid, 256, 0, (cudaStream_t)stream>>>(a);
+        else stream_state_kernel<float, false><<<grid, 256, 0, (cudaStream_t)stream>>>(a);
+    }
+    CK(h, cudaGetLastError());
+    ++h->launches;
+    return 0;
+}
+
+int adec_get_stream_state(adec_handle* h, const int* streams, int n, void* out, void* stream) {
+    return stream_state_io(h, "get_stream_state", streams, n, out, false, stream);
+}
+
+int adec_set_stream_state(adec_handle* h, const int* streams, int n, const void* in, void* stream) {
+    return stream_state_io(h, "set_stream_state", streams, n, const_cast<void*>(in), true, stream);
 }
 
 static int index_bits(int n) { int b = 1; while ((1 << b) < n) ++b; return b; }

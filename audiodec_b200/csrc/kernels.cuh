@@ -1046,4 +1046,75 @@ __global__ void replicate_kernel(float* dst, const float* src, long long per_str
     if (i < per_stream * n) dst[i] = src[i % per_stream];
 }
 
+// ---- stream state export / import (adec_get_stream_state / adec_set_stream_state) ----------------------------------------------------
+// One entry of the handle's state map as the kernels see it: a reference pad_buffer (C, P) channels-first <-> rows [zrows, zrows + P) of
+// its op's (P_op, st_C) channels-last state.  Key channel c = g * cg + cc sits at column col0 + g * gstride + cc (gstride 0: the groups
+// are copies of one shared input).  On import the rows [0, zrows) of the key's columns are zeroed (AD v0: they only meet zero taps).
+struct alignas(16) StateEntry {      // 16-byte aligned: the tile table follows the entries in one upload
+    const void* st[2];        // the op's state buffer for a stream whose slot bit is 0 (st[cur]) and 1 (st[cur ^ 1])
+    long long per;            // elements per stream of the op's state (P_op * st_C)
+    long long off;            // the entry's first element in a stream's exported vector
+    int C, P, zrows, st_C, cg, col0, gstride;
+    int list;                 // 0 = encoder ops, 1 = decoder ops: which slot bits name the stream's buffer
+    int wc;                   // channels an import writes (shared input: cg, copy 0; 0: the entry is not imported)
+};
+
+struct StateArgs {
+    const StateEntry* ent;
+    const int4* tiles;        // {entry, c0, r0, 0}: a 32 x 32 tile of key channels [c0, +32) x handle rows [r0, +32)
+    const int* streams;       // per requested stream: {stream id, encoder slot bit, decoder slot bit}
+    int n;                    // requested streams
+    void* ext;                // (n, S) stream-major vectors
+    long long S;              // elements per stream
+    int* err;                 // import on the fp16-split engine: bit 1 for a value outside its range (|v| >= 6e4 or non-finite)
+};
+
+template <typename T, bool IMPORT>
+__global__ void __launch_bounds__(256) stream_state_kernel(StateArgs a) {
+    __shared__ T tile[32][33];
+    const int4 tl = a.tiles[blockIdx.x];
+    const StateEntry& e = a.ent[tl.x];
+    const int c0 = tl.y, r0 = tl.z;
+    const int nc = min(32, (IMPORT ? e.wc : e.C) - c0), nr = min(32, e.zrows + e.P - r0);
+    if (nc <= 0) return;
+    const int tid = threadIdx.x;
+    bool bad = false;
+    for (int i = blockIdx.y; i < a.n; i += gridDim.y) {
+        const int s = a.streams[3 * i], sel = a.streams[3 * i + 1 + e.list];
+        T* st = (T*)e.st[sel] + (long long)s * e.per;
+        T* ext = (T*)a.ext + (long long)i * a.S + e.off;
+        if (!IMPORT) {
+            // channels-last rows (consecutive threads: consecutive channels) -> tile[row][channel] -> channels-first (consecutive rows)
+            for (int k = tid; k < nc * nr; k += 256) {
+                const int r = k / nc, c = k - r * nc, row = r0 + r, kc = c0 + c, g = kc / e.cg;
+                if (row >= e.zrows) tile[r][c] = st[(long long)row * e.st_C + e.col0 + g * e.gstride + (kc - g * e.cg)];
+            }
+            __syncthreads();
+            for (int k = tid; k < nc * nr; k += 256) {
+                const int c = k / nr, r = k - c * nr, row = r0 + r;
+                if (row >= e.zrows) ext[(long long)(c0 + c) * e.P + row - e.zrows] = tile[r][c];
+            }
+        } else {
+            for (int k = tid; k < nc * nr; k += 256) {
+                const int c = k / nr, r = k - c * nr, row = r0 + r;
+                T v;
+                if (row >= e.zrows) {
+                    v = ext[(long long)(c0 + c) * e.P + row - e.zrows];
+                    if constexpr (std::is_same<T, float>::value) bad |= a.err && !(fabsf(v) < 60000.f);
+                } else {
+                    v = T(0);
+                }
+                tile[r][c] = v;
+            }
+            __syncthreads();
+            for (int k = tid; k < nc * nr; k += 256) {
+                const int r = k / nc, c = k - r * nc, row = r0 + r, kc = c0 + c, g = kc / e.cg;
+                st[(long long)row * e.st_C + e.col0 + g * e.gstride + (kc - g * e.cg)] = tile[r][c];
+            }
+        }
+        __syncthreads();
+    }
+    if (bad) atomicOr(a.err, 2);
+}
+
 }  // namespace adec

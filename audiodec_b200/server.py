@@ -228,6 +228,22 @@ class MultiStreamCodecServer:
         }
 
 
+class SessionState:
+    """What a detached session needs to continue on another SessionCodecServer (of the same config and dtypes, on any device):
+    per stateful generator of the server its state_layout and its (1, S) device state, the queued input frames with their capture
+    stamps, and the decoded frames it has not polled yet."""
+
+    def __init__(self, layouts, states, inputs, outputs):
+        self.layouts: List[list] = layouts
+        self.states: List[torch.Tensor] = states
+        self.inputs: List[Tuple[np.ndarray, float]] = inputs
+        self.outputs: List[np.ndarray] = outputs
+
+    def to(self, device) -> "SessionState":
+        """A copy with the states on `device` (the frames are host arrays and are shared)."""
+        return SessionState(self.layouts, [t.to(device) for t in self.states], list(self.inputs), list(self.outputs))
+
+
 class SessionCodecServer(MultiStreamCodecServer):
     """Duplex streams that open and close while others run, each advanced only when it has audio.
 
@@ -237,7 +253,8 @@ class SessionCodecServer(MultiStreamCodecServer):
     caller.  ``step()`` runs ONE slot call per codec stage (``encode_streams`` -> quantize -> ``decode_streams``) over the open
     streams that have a frame queued: idle streams are not fed silence, their causal state stays as it is, and a step costs what
     its streams cost, not what the capacity costs.  ``submit`` / ``poll`` / the drop policy / ``start`` / ``stop`` are the lock-step
-    server's; the per-stream counters in ``statistics()`` are per slot.  The generators must hold ONE warmed stream when the server is
+    server's; the per-stream counters in ``statistics()`` are per slot.  ``detach()`` closes a stream and returns its causal state and its
+    queued and undelivered frames; ``attach()`` continues it in a free slot of this or another server, on any device.  The generators must hold ONE warmed stream when the server is
     built (what load_transmitter / load_receiver leave), since only that stream is replicated into the slots.
     """
 
@@ -258,6 +275,7 @@ class SessionCodecServer(MultiStreamCodecServer):
         self._open: set = set()
         self._session = [0] * capacity                # per slot: bumped by every open(), so a step hands out only its own session's frames
         self._codec_lock = threading.Lock()           # the codec handles are driven by step() and open() from different threads
+        self._step_lock = threading.Lock()            # held for a whole step, output hand-off included: detach() waits for it
 
     # ------------------------------------------------------------------ sessions
     def open(self) -> int:
@@ -287,6 +305,57 @@ class SessionCodecServer(MultiStreamCodecServer):
             self._out[stream].clear()
             self._free.append(stream)
 
+    def detach(self, stream: int) -> SessionState:
+        """Close stream `stream` and return what it needs to continue elsewhere (attach(), on this or another server): its causal state
+        in every stateful generator, its queued input frames and its undelivered output frames.  Waits for a step in progress to finish
+        and hand off its frames, so no frame in flight is lost.  Raises KeyError if the stream is not open."""
+        with self._step_lock:
+            with self._lock:
+                if stream not in self._open:
+                    raise KeyError(f"stream {stream} is not open")
+                self._open.remove(stream)
+                inputs, outputs = list(self._in[stream]), list(self._out[stream])
+                self._in[stream].clear()
+                self._out[stream].clear()
+            with self._codec_lock:       # the slot stays taken until its state is out
+                states = [g.stream_state([stream]) for g in self._stateful]
+            layouts = [list(g.state_layout) for g in self._stateful]
+            with self._lock:
+                self._free.append(stream)
+        return SessionState(layouts, states, inputs, outputs)
+
+    def attach(self, state: SessionState) -> int:
+        """Open a stream in a free slot from a detached session instead of the template: it continues exactly where it left off, with
+        its queued and undelivered frames, and fresh per-stream counters.  The state must be on this server's device (SessionState.to).
+        Raises ValueError if the session comes from codecs of another layout, RuntimeError when every slot is taken."""
+        if len(state.states) != len(self._stateful) or len(state.layouts) != len(self._stateful):
+            raise ValueError(f"the session holds the state of {len(state.states)} generators; this server has {len(self._stateful)}")
+        for g, layout in zip(self._stateful, state.layouts):
+            if [tuple(e) for e in layout] != [tuple(e) for e in g.state_layout]:
+                raise ValueError(f"the session's state layout does not match this server's {type(g).__name__}")
+        with self._lock:
+            if not self._free:
+                raise RuntimeError(f"server is full: all {self.capacity} streams are open")
+            s = min(self._free)
+            self._free.remove(s)
+            self._session[s] += 1
+        try:
+            with self._codec_lock:
+                for g, layout, t in zip(self._stateful, state.layouts, state.states):
+                    g.load_stream_state([s], t, layout)
+        except Exception:
+            with self._lock:
+                self._free.append(s)
+            raise
+        with self._lock:
+            self._in[s].clear()
+            self._in[s].extend(state.inputs)
+            self._out[s].clear()
+            self._out[s].extend(state.outputs)
+            self.stats[s] = StreamStats()
+            self._open.add(s)
+        return s
+
     @property
     def open_streams(self) -> List[int]:
         with self._lock:
@@ -300,6 +369,10 @@ class SessionCodecServer(MultiStreamCodecServer):
     # ------------------------------------------------------------------ one step over the streams that have audio
     def step(self) -> int:
         """Advance every open stream that has a frame queued by that frame.  Returns the number of streams advanced."""
+        with self._step_lock:
+            return self._step()
+
+    def _step(self) -> int:
         t0 = self._clock()
         dev = self.device if self.device is not None else torch.device("cpu")
         x_host = self._staging(dev)

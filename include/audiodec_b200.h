@@ -171,8 +171,28 @@ int adec_decode_streams(adec_handle *h, const float *zq, const int *frames, cons
 int adec_decode_streams_bf16(adec_handle *h, const uint16_t *zq, const int *frames, const int *streams, int B, uint16_t *y, void *stream);
 /* Copy stream src's current causal state (all layers of the handle) into each dst[i]: a joining stream starts warm. */
 int adec_copy_stream_state(adec_handle *h, int src, const int *dst, int n, void *stream);
+
 /* The uniform streaming calls, adec_set_streams and adec_reset see every stream's latest state after slot calls (a handle that made slot
  * calls copies the streams whose state sits in the other ping-pong buffer back once, before its next uniform call or resize). */
+
+/* -- stream state out of and into a handle: save, resume, and move a stream to another handle (another server, another GPU) ---------
+ * The state map lists every reference pad_buffer the handle runs (layers/conv_layer.py:146,187), with the reference's key as a state dict
+ * names it and its shape (C, P); buffers of layers the handle does not run (the encoder of a decoder-only handle) are not in it.  One
+ * stream's state is S = adec_stream_state_elems(h) elements: the entries in map order, each (C, P) channels-first.  A MultiGroupConv1d
+ * convs1.0 buffer holds `groups` copies of its shared input: export writes every copy, import reads copy 0.  AD v0's per-block buffers are
+ * the tails of the handle's longer per-group history: import zeroes the older rows (they only meet zero taps) and takes convs1.0's shared
+ * input from the block with the largest kernel. */
+int     adec_state_entries(const adec_handle *h);                 /* entries of the state map, -1 before adec_finalize */
+/* entry i: *key (valid for the handle's life), *C, *P; any of them may be NULL.  Returns non-zero for an i out of range. */
+int     adec_state_entry(const adec_handle *h, int i, const char **key, int *C, int *P);
+int64_t adec_stream_state_elems(const adec_handle *h);            /* S = sum C * P, elements per stream; -1 before adec_finalize */
+/* Export / import the current state of streams[0..n) (HOST array of distinct ids in [0, n_streams)) to / from a device buffer of (n, S)
+ * elements, 16-byte aligned: fp32, or bf16 words on a compute_dtype 2 handle, copied as they are.  One launch on `stream`, no host
+ * synchronise; neither call changes which buffer a stream's next call reads, so an export between any two calls sees what the next one
+ * would read.  Streams not listed keep their state bit for bit.  On the fp16-split engine an import sets the range flag
+ * (adec_range_error) for a value that is non-finite or has |v| >= 6e4. */
+int adec_get_stream_state(adec_handle *h, const int *streams, int n, void *out, void *stream);
+int adec_set_stream_state(adec_handle *h, const int *streams, int n, const void *in, void *stream);
 
 /* output frames of encode for T input samples: floor((T-1)/s)+1 applied per stride (conv_layer.py:153-156) */
 int adec_frames_for(const adec_handle *h, int T);
