@@ -41,6 +41,7 @@ class AdecConfig(ctypes.Structure):
 
 
 MODEL_SYMAD, MODEL_HIFIGAN, MODEL_SYMAD_DECODER = 0, 1, 2
+GRAPH_TX, GRAPH_RX = 0, 1
 
 
 class AdecTestOp(ctypes.Structure):
@@ -73,6 +74,12 @@ SYMBOLS = {
     "adec_zq_moments": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), c_int, c_void_p, c_void_p, c_void_p]),
     "adec_lookup": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "adec_lookup_packed": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "adec_lookup_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "adec_lookup_packed_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "adec_graph_create": (c_int, [c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, ctypes.POINTER(c_void_p)]),
+    "adec_graph_launch": (c_int, [c_void_p, c_void_p]),
+    "adec_graph_info": (c_int, [c_void_p, ctypes.POINTER(c_int), ctypes.POINTER(c_int), ctypes.POINTER(c_int)]),
+    "adec_graph_destroy": (c_int, [c_void_p]),
     "adec_decode": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "adec_encode_offline": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "adec_decode_offline": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),

@@ -521,8 +521,9 @@ class SymADStreamGenerator(_StreamGeneratorBase):
             packed = packed.squeeze(0) if packed is not None else None
         return idx, packed, zq
 
-    def lookup_packed(self, packed):
-        """uint8 (F,bytes) -> zq (1,F,D); (B,F,bytes) -> (B,F,D): lookup straight from the bitstream (unpack fused into lookup)."""
+    def lookup_packed(self, packed, dtype=torch.float32):
+        """uint8 (F,bytes) -> zq (1,F,D); (B,F,bytes) -> (B,F,D): lookup straight from the bitstream (unpack fused into lookup).
+        dtype=torch.bfloat16: bf16 zq, the fp32 sum rounded once, equal to lookup_packed(packed).to(torch.bfloat16)."""
         self._ready()
         packed = self._in(packed, torch.uint8)
         if packed.dim() == 2:
@@ -530,12 +531,19 @@ class SymADStreamGenerator(_StreamGeneratorBase):
         b, f, nb = packed.shape
         if nb != self.packed_frame_bytes():
             raise RuntimeError(f"audiodec_b200: lookup_packed: expected {self.packed_frame_bytes()} bytes per frame, got {nb}")
-        zq = torch.empty(b, f, self.code_dim, device=self._device, dtype=torch.float32)
-        _check(self._lib.adec_lookup_packed(self._h, _ptr(packed), b, f, _ptr(zq), self._stream()), self._h)
+        fn = self._lookup_fn("adec_lookup_packed", dtype)
+        zq = torch.empty(b, f, self.code_dim, device=self._device, dtype=dtype)
+        _check(fn(self._h, _ptr(packed), b, f, _ptr(zq), self._stream()), self._h)
         return zq
 
-    def lookup(self, idx):
-        """idx (Nq,F) -> zq (1,F,D); (Nq,B,F) -> (B,F,D)   (AudioDec.py:242-243)"""
+    def _lookup_fn(self, name, dtype):
+        if dtype not in (torch.float32, torch.bfloat16):
+            raise NotImplementedError(f"audiodec_b200: {name[5:]}: zq is float32 or bfloat16, not {dtype}")
+        return getattr(self._lib, name + "_bf16" if dtype == torch.bfloat16 else name)
+
+    def lookup(self, idx, dtype=torch.float32):
+        """idx (Nq,F) -> zq (1,F,D); (Nq,B,F) -> (B,F,D)   (AudioDec.py:242-243).  dtype=torch.bfloat16: bf16 zq, the fp32 sum
+        rounded once, equal to lookup(idx).to(torch.bfloat16) (what a decoder with bf16 activations takes)."""
         self._ready()
         idx = self._in(idx, torch.int64)
         if idx.dim() == 2:
@@ -543,8 +551,9 @@ class SymADStreamGenerator(_StreamGeneratorBase):
         if idx.dim() != 3 or idx.size(0) != self.codebook_num:
             raise RuntimeError(f"audiodec_b200: lookup: expected ({self.codebook_num},F) or ({self.codebook_num},B,F) indices, got {tuple(idx.shape)}")
         _, b, f = idx.shape
-        zq = torch.empty(b, f, self.code_dim, device=self._device, dtype=torch.float32)
-        _check(self._lib.adec_lookup(self._h, _ptr(idx), b, f, _ptr(zq), self._stream()), self._h)
+        fn = self._lookup_fn("adec_lookup", dtype)
+        zq = torch.empty(b, f, self.code_dim, device=self._device, dtype=dtype)
+        _check(fn(self._h, _ptr(idx), b, f, _ptr(zq), self._stream()), self._h)
         return zq
 
     # ---- non-streaming batch forward (SURVEY.md 8(f) rank 4; codecTest.py:78-95).  These calls discard the streaming state.
@@ -810,6 +819,124 @@ class HiFiGANStreamGenerator(_StreamGeneratorBase):
         launch sequence -> list of B waveforms (1, 1, F_b * hop), views of one output buffer (bf16 with bf16 activations), each equal to
         a B = 1 streaming decode of those frames.  Streams not listed keep their state untouched."""
         return self._decode_streams(c, frames, streams)
+
+class _StepGraph:
+    """One graphed streaming step (adec_graph_*): static `input` / `output` tensors and the generators it runs.  Launching it is the
+    eager call sequence it replaces, bit for bit: outputs, causal state, range / index flags and launch_count."""
+
+    def __init__(self, kind, gens, state_gen, n_streams, size, wire, input, output):
+        self._gens = gens
+        for g in gens:
+            g._ready()
+        dev = gens[0]._device
+        if any(g._device != dev for g in gens):
+            raise RuntimeError(f"audiodec_b200: graph: the generators are on {[str(g._device) for g in gens]}; they must share one device")
+        self._handles = [g._h.value for g in gens]
+        self._state_gen, self._B = state_gen, n_streams
+        self._kind, self._size, self._wire = kind, size, bool(wire)
+        self._lib, self._device = gens[0]._lib, dev
+        self._raw_in, self._raw_out = input, output
+        self._g = None
+        self._create()
+
+    def _create(self):
+        self._state_gen._batch(self._B)
+        g = ctypes.c_void_p()
+        a = self._gens[0]._h
+        b = self._gens[1]._h if len(self._gens) > 1 else None
+        _check(self._lib.adec_graph_create(self._kind, a, b, self._B, self._size, int(self._wire), _ptr(self._raw_in), _ptr(self._raw_out),
+                                           ctypes.byref(g)), a)
+        self._g = g
+
+    def handles_current(self):
+        """False once a generator's handle was replaced (.to() again) since the graph was made."""
+        return [g._h.value if g._h is not None else None for g in self._gens] == self._handles
+
+    def _check_handles(self):
+        if not self.handles_current():
+            raise RuntimeError("audiodec_b200: graph: a generator's handle was replaced (.to() again) since the graph was made; make a new graph")
+
+    def __call__(self, x):
+        """Copy x into `input` (unless x is `input`), launch the step on the current stream, return `output`.  Like torch.cuda.CUDAGraph,
+        the output is a static tensor that the next call overwrites: clone it to keep it."""
+        self._check_handles()
+        if x is not self.input:
+            if tuple(x.shape) != tuple(self.input.shape):
+                raise RuntimeError(f"audiodec_b200: graph: expected input of shape {tuple(self.input.shape)}, got {tuple(x.shape)}")
+            self.input.copy_(x)
+        if self._state_gen.n_streams != self._B:         # what the eager call's _batch does; the launch re-captures if buffers moved
+            self._state_gen._batch(self._B)
+        a = self._gens[0]
+        _check(self._lib.adec_graph_launch(self._g, a._stream()), a._h)
+        return self.output
+
+    def info(self):
+        """{'kernels': kernels per step, 'programmatic_edges': PDL edges in the captured graph, 'instantiations': executables built}"""
+        k, e, i = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+        _check(self._lib.adec_graph_info(self._g, ctypes.byref(k), ctypes.byref(e), ctypes.byref(i)), self._gens[0]._h)
+        return {"kernels": k.value, "programmatic_edges": e.value, "instantiations": i.value}
+
+    def __del__(self):
+        try:
+            if self._g is not None:
+                self._lib.adec_graph_destroy(self._g)
+                self._g = None
+        except Exception:
+            pass
+
+
+class TransmitterGraph(_StepGraph):
+    """tx_encoder.encode(x) -> tx_encoder.quantize(z) for n_streams streams of `chunk` samples as one CUDA graph launch; with wire,
+    quantize_fused(z, want_idx=False, want_packed=True, want_zq=False) instead.  `input` is x (n_streams, 1, chunk) float32; `output`
+    is what the eager calls return: indices (Nq, F) for one stream, (Nq, n_streams, F) otherwise, or with wire the packed bytes
+    (F, bytes) / (n_streams, F, bytes).  The output is overwritten by the next call."""
+
+    def __init__(self, tx_encoder, n_streams, chunk, wire=False):
+        if not isinstance(tx_encoder, SymADStreamGenerator):
+            raise TypeError(f"audiodec_b200: TransmitterGraph needs a SymADStreamGenerator (encoder, projector and RVQ), got "
+                            f"{type(tx_encoder).__name__}")
+        tx_encoder._ready()
+        dev, b = tx_encoder._device, int(n_streams)
+        f = tx_encoder._lib.adec_frames_for(tx_encoder._h, int(chunk))
+        self.input = torch.zeros(b, tx_encoder.input_channels, int(chunk), device=dev, dtype=torch.float32)
+        if wire:
+            raw = torch.empty(b, f, tx_encoder.packed_frame_bytes(), device=dev, dtype=torch.uint8)
+            self.output = raw.squeeze(0) if b == 1 else raw
+        else:
+            raw = torch.empty(tx_encoder.codebook_num, b, f, device=dev, dtype=torch.int64)
+            self.output = raw.squeeze(1) if b == 1 else raw
+        super().__init__(_lib.GRAPH_TX, [tx_encoder], tx_encoder, b, int(chunk), wire, self.input, raw)
+
+
+class ReceiverGraph(_StepGraph):
+    """rx_encoder.lookup(idx) -> decoder.decode(zq) for n_streams streams of `frames` frames as one CUDA graph launch; with wire,
+    rx_encoder.lookup_packed(packed) instead of lookup.  `decoder` is any decoder generator (symAD, symAD decoder-only or HiFi-GAN, fp32 or
+    bf16).  `input` has the shape the transmitter's output has (indices or packed bytes); `output` is y (n_streams, 1, frames * hop),
+    bf16 for a decoder with bf16 activations.  The output is overwritten by the next call."""
+
+    def __init__(self, rx_encoder, decoder, n_streams, frames, wire=False):
+        if not isinstance(rx_encoder, SymADStreamGenerator):
+            raise TypeError(f"audiodec_b200: ReceiverGraph needs a SymADStreamGenerator as rx_encoder (its codebooks), got "
+                            f"{type(rx_encoder).__name__}")
+        if not isinstance(decoder, _StreamGeneratorBase):
+            raise TypeError(f"audiodec_b200: ReceiverGraph needs a library decoder generator, got {type(decoder).__name__}")
+        rx_encoder._ready(), decoder._ready()
+        dev, b, f = rx_encoder._device, int(n_streams), int(frames)
+        if wire:
+            raw = torch.zeros(b, f, rx_encoder.packed_frame_bytes(), device=dev, dtype=torch.uint8)
+            self.input = raw.squeeze(0) if b == 1 else raw
+        else:
+            raw = torch.zeros(rx_encoder.codebook_num, b, f, device=dev, dtype=torch.int64)
+            self.input = raw.squeeze(1) if b == 1 else raw
+        hop = decoder._lib.adec_hop_length(decoder._h)
+        self.output = torch.empty(b, 1, f * hop, device=decoder._device, dtype=torch.bfloat16 if decoder._act_bf16 else torch.float32)
+        super().__init__(_lib.GRAPH_RX, [rx_encoder, decoder], decoder, b, f, wire, raw, self.output)
+
+
+def is_library_codec(tx_encoder, rx_encoder, decoder):
+    """True when the three codec objects are this library's generators on a CUDA device, so a stream step can run as graphs."""
+    return (isinstance(tx_encoder, SymADStreamGenerator) and isinstance(rx_encoder, SymADStreamGenerator)
+            and isinstance(decoder, _StreamGeneratorBase) and all(g._h is not None for g in (tx_encoder, rx_encoder, decoder)))
 
 
 class OfflineCodec:

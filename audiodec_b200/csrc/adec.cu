@@ -262,6 +262,9 @@ struct adec_handle {
     int ktrace_n = 0;
     int n_sms = 132;
     DevBuf ws[3];
+    // bumped by every reallocation a captured stream step bakes in (ws[*] growth, state buffers in resize_state): a graph captured
+    // at another generation re-captures before its next launch (adec_graph_launch)
+    uint64_t gen = 0;
     std::vector<void*> owned;     // device allocations freed in destroy
     // rvq
     float *d_embed = nullptr, *d_e2 = nullptr, *d_codebook = nullptr;
@@ -320,6 +323,7 @@ int ensure(adec_handle* h, DevBuf& b, size_t n_floats) {
     b.cap = 0;
     CK(h, cudaMalloc((void**)&b.p, n_floats * sizeof(float)));
     b.cap = n_floats;
+    if (&b >= h->ws && &b < h->ws + 3) ++h->gen;
     return 0;
 }
 
@@ -755,6 +759,22 @@ int plan_varlen(adec_handle* h, const std::vector<Op>& ops, const RunCtx& rc, Vl
     return 0;
 }
 
+// Grow the activation workspaces to what `ops` need over B uniform streams of T_in rows, or over the varlen row tables `pl`
+int size_ws(adec_handle* h, const std::vector<Op>& ops, int B, int T_in, const VlPlan* pl) {
+    size_t need[3] = {0, 0, 0};
+    int T = T_in;
+    for (size_t k = 0; k < ops.size(); ++k) {
+        const Op& op = ops[k];
+        const int Tout = (T - 1) / op.down + 1;
+        const size_t rows = pl ? (size_t)pl->Tout[k] : (size_t)B * Tout;
+        if (op.out_buf >= 0) need[op.out_buf] = std::max(need[op.out_buf], rows * op.ldy);
+        T = Tout * op.up;
+    }
+    for (int i = 0; i < 3; ++i)     // need[] counts elements; the buffers are sized in floats
+        if (need[i] && ensure(h, h->ws[i], (need[i] * h->act_bytes() + 3) / 4)) return 1;
+    return 0;
+}
+
 // The launches of one call.  Reads each stateful op's history from st[cur] (slot calls: from the buffer the stream's slot bit names)
 // and writes the new state to the other buffer; what that does to `cur` and the slot bits is the caller's (run_call).
 int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, int* T_out_final) {
@@ -768,19 +788,7 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
                 return h->fail(fmt("%s: the FFMA engine (ADEC_CONV_PATH=ffma) has no varlen kernels; use the f16 or tf32 tensor-core engine",
                                    rc.what));
     }
-    size_t need[3] = {0, 0, 0};
-    {
-        int T = T_in;
-        for (size_t k = 0; k < ops.size(); ++k) {
-            const Op& op = ops[k];
-            const int Tout = (T - 1) / op.down + 1;
-            const size_t rows = vl ? (size_t)pl.Tout[k] : (size_t)rc.B * Tout;
-            if (op.out_buf >= 0) need[op.out_buf] = std::max(need[op.out_buf], rows * op.ldy);
-            T = Tout * op.up;
-        }
-    }
-    for (int i = 0; i < 3; ++i)     // need[] counts elements; the buffers are sized in floats
-        if (need[i] && ensure(h, h->ws[i], (need[i] * h->act_bytes() + 3) / 4)) return 1;
+    if (size_ws(h, ops, rc.B, T_in, vl ? &pl : nullptr)) return 1;
     if (!vl && rc.B != h->n_streams) return h->fail(fmt("batch %d != n_streams %d (call adec_set_streams)", rc.B, h->n_streams));
     const int* vl_tab = nullptr;
     const int* vl_slot = nullptr;
@@ -1493,6 +1501,7 @@ static int resize_state(adec_handle* h, int n, bool replicate) {
             }
         }
     CK(h, cudaDeviceSynchronize());
+    if (n > h->st_cap) ++h->gen;
     h->st_cap = std::max(h->st_cap, n);
     h->n_streams = n;
     h->enc_slots.bit.assign(n, 0);
@@ -1869,28 +1878,41 @@ int adec_quantize(adec_handle* h, const float* z, int B, int F, int64_t* idx, vo
     return adec_quantize_ex(h, z, B, F, idx, nullptr, nullptr, stream);
 }
 
-static int lookup_common(adec_handle* h, const int64_t* idx, const uint8_t* packed, int B, int F, float* zq, void* stream) {
+// bf16: zq is bf16 (lookup_kernel<true>), 16-byte aligned
+static int lookup_common(adec_handle* h, const int64_t* idx, const uint8_t* packed, int B, int F, void* zq, bool bf16, void* stream) {
     if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    if (need_full_symad(h, "lookup")) return 1;
-    if (B < 1 || F < 1) return h->fail("lookup: empty input");
+    const char* what = bf16 ? "lookup_bf16" : "lookup";
+    if (need_full_symad(h, what)) return 1;
+    if (B < 1 || F < 1) return h->fail(std::string(what) + ": empty input");
+    if (bf16 && (h->cfg.code_dim % 8 || (uintptr_t)zq % 16))
+        return h->fail("lookup_bf16: needs code_dim % 8 == 0 and a 16-byte aligned zq");
     DeviceGuard dg(h->device);
     LookupArgs a{};
     a.idx = (const long long*)idx; a.packed = packed; a.nfr = (long long)B * F; a.nq = h->cfg.codebook_num; a.D = h->cfg.code_dim;
     a.N = h->cfg.codebook_size; a.bits = index_bits(a.N); a.bpf = adec_packed_frame_bytes(h);
-    a.codebook = h->d_codebook; a.n_rows = (long long)h->cfg.codebook_num * h->cfg.codebook_size; a.zq = zq; a.err = h->d_err;
+    a.codebook = h->d_codebook; a.n_rows = (long long)h->cfg.codebook_num * h->cfg.codebook_size; a.zq = (float*)zq; a.err = h->d_err;
     const long long nth = a.nfr * (a.D / 4);
-    lookup_kernel<<<(unsigned)((nth + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a);
+    if (bf16) lookup_kernel<true><<<(unsigned)((nth + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a);
+    else lookup_kernel<false><<<(unsigned)((nth + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a);
     CK(h, cudaGetLastError());
     ++h->launches;
     return 0;
 }
 
 int adec_lookup(adec_handle* h, const int64_t* idx, int B, int F, float* zq, void* stream) {
-    return lookup_common(h, idx, nullptr, B, F, zq, stream);
+    return lookup_common(h, idx, nullptr, B, F, zq, false, stream);
+}
+
+int adec_lookup_bf16(adec_handle* h, const int64_t* idx, int B, int F, uint16_t* zq, void* stream) {
+    return lookup_common(h, idx, nullptr, B, F, zq, true, stream);
 }
 
 int adec_lookup_packed(adec_handle* h, const uint8_t* packed, int B, int F, float* zq, void* stream) {
-    return lookup_common(h, nullptr, packed, B, F, zq, stream);
+    return lookup_common(h, nullptr, packed, B, F, zq, false, stream);
+}
+
+int adec_lookup_packed_bf16(adec_handle* h, const uint8_t* packed, int B, int F, uint16_t* zq, void* stream) {
+    return lookup_common(h, nullptr, packed, B, F, zq, true, stream);
 }
 
 int adec_codec_host(adec_handle* enc, adec_handle* dec, const float* x_host, int B, int T, int64_t* idx_host,
@@ -2093,6 +2115,262 @@ int adec_profile_report(adec_handle* h, char* buf, int buf_len) {
 
 // -------------------------------------------------------------------------------------------------
 // single-layer entry points for the unit tests (HOST pointers, reference layouts)
+// ---- graphed stream steps: the eager call sequence of a transmitter or receiver step, captured once per state parity
+struct adec_graph {
+    int kind = ADEC_GRAPH_TX;
+    adec_handle* a = nullptr;     // the tx handle (ADEC_GRAPH_TX) or the rx handle (ADEC_GRAPH_RX); errors are reported on it
+    adec_handle* b = nullptr;     // the decoder (ADEC_GRAPH_RX), may equal a
+    int device = 0;
+    int B = 0, T = 0, F = 0;      // streams, input samples (TX), frames
+    bool wire = false;
+    const void* in = nullptr;
+    void* out = nullptr;
+    void* mid = nullptr;          // TX: z (B, code_dim, F) fp32; RX: zq (B, F, code_dim), bf16 when the decoder has bf16 activations
+    cudaStream_t cs = nullptr;    // private capture stream
+    // by the parity (op.cur) of the stateful op list: both captured together, each instantiated the first time it is launched
+    cudaGraph_t graph[2] = {nullptr, nullptr};
+    cudaGraphExec_t exec[2] = {nullptr, nullptr};
+    uint64_t gen_a = 0, gen_b = 0;                    // the handles' generations the graphs were captured at
+    int64_t da = 0, db = 0;       // launches one step counts on a and on b (b != a), as the eager calls count them
+    int kernels = 0, edges = 0, instantiations = 0;
+};
+
+static adec_handle* graph_state_handle(const adec_graph* g) { return g->kind == ADEC_GRAPH_TX ? g->a : g->b; }
+static std::vector<Op>& graph_state_ops(adec_graph* g) { return g->kind == ADEC_GRAPH_TX ? g->a->enc_ops : g->b->dec_ops; }
+
+// which state buffer the stateful ops of a list read next (op.cur); -1 if they disagree
+static int list_parity(const std::vector<Op>& ops) {
+    int p = -1;
+    for (const Op& op : ops)
+        if (op.P > 0) {
+            if (p < 0) p = op.cur;
+            else if (p != op.cur) return -1;
+        }
+    return p < 0 ? 0 : p;
+}
+
+// The eager sequence a step stands for: encode + quantize (TX), lookup + decode (RX), on stream s
+static int graph_body(adec_graph* g, cudaStream_t s) {
+    adec_handle *a = g->a, *b = g->b;
+    if (g->kind == ADEC_GRAPH_TX) {
+        if (run_call(a, {false, CALL_STREAM, false}, g->in, g->B, g->T, g->mid, s)) return 1;
+        return quantize_common(a, (const float*)g->mid, g->B, g->F, g->wire ? nullptr : (int64_t*)g->out,
+                               g->wire ? (uint8_t*)g->out : nullptr, nullptr, false, s);
+    }
+    if (lookup_common(a, g->wire ? nullptr : (const int64_t*)g->in, g->wire ? (const uint8_t*)g->in : nullptr, g->B, g->F, g->mid,
+                      b->act_bf16, s))
+        return 1;
+    if (run_call(b, {true, CALL_STREAM, b->act_bf16}, g->mid, g->B, g->F, g->out, s)) { a->err = b->err; return 1; }
+    return 0;
+}
+
+// A handle's host state as a capture finds it: the capture runs the eager code, which advances it, and puts it back afterwards.
+// The diagnostics (profiling events, launch records, the kernel trace) are switched off for the capture, so that none of their
+// records or trace slots is baked into the graph or left behind for launches that never ran.
+struct HostSnap {
+    adec_handle* h;
+    int64_t launches;
+    SlotBits enc, dec;
+    std::vector<int> cur;
+    bool profiling;
+    std::vector<int>* launch_log;
+    unsigned long long* d_ktrace;
+    int ktrace_n;
+    explicit HostSnap(adec_handle* h_)
+        : h(h_), launches(h_->launches), enc(h_->enc_slots), dec(h_->dec_slots), profiling(h_->profiling), launch_log(h_->launch_log),
+          d_ktrace(h_->d_ktrace), ktrace_n(h_->ktrace_n) {
+        for (auto* ops : {&h->enc_ops, &h->dec_ops})
+            for (const Op& op : *ops) cur.push_back(op.cur);
+        h->profiling = false;
+        h->launch_log = nullptr;
+        h->d_ktrace = nullptr;
+    }
+    void restore() const {
+        h->launches = launches;
+        h->enc_slots = enc;
+        h->dec_slots = dec;
+        h->profiling = profiling;
+        h->launch_log = launch_log;
+        h->d_ktrace = d_ktrace;
+        h->ktrace_n = ktrace_n;
+        size_t i = 0;
+        for (auto* ops : {&h->enc_ops, &h->dec_ops})
+            for (Op& op : *ops) op.cur = cur[i++];
+    }
+};
+
+static void graph_drop(adec_graph* g) {
+    for (int p = 0; p < 2; ++p) {
+        if (g->exec[p]) { cudaGraphExecDestroy(g->exec[p]); g->exec[p] = nullptr; }
+        if (g->graph[p]) { cudaGraphDestroy(g->graph[p]); g->graph[p] = nullptr; }
+    }
+}
+
+// Capture the step at parity p (the stateful ops' cur set to p for the capture) into *out; counts its kernels and programmatic edges
+// and the launches the eager step counts on a and on b.
+static int graph_capture_one(adec_graph* g, int p, cudaGraph_t* out, int* kernels, int* edges, int64_t* da, int64_t* db) {
+    adec_handle *a = g->a, *b = g->b;
+    std::vector<HostSnap> snaps{HostSnap(a)};
+    if (b && b != a) snaps.emplace_back(b);
+    for (const HostSnap& sn : snaps) sn.h->enc_slots.dirty = sn.h->dec_slots.dirty = false;
+    for (Op& op : graph_state_ops(g))
+        if (op.P > 0) op.cur = p;
+    cudaGraph_t graph = nullptr;
+    cudaError_t ec = cudaStreamBeginCapture(g->cs, cudaStreamCaptureModeThreadLocal);
+    if (ec != cudaSuccess) {
+        for (const HostSnap& sn : snaps) sn.restore();
+        return a->fail(fmt("graph: cudaStreamBeginCapture failed: %s", cudaGetErrorString(ec)));
+    }
+    const int rc = graph_body(g, g->cs);
+    ec = cudaStreamEndCapture(g->cs, &graph);
+    *da = a->launches - snaps[0].launches;
+    *db = snaps.size() > 1 ? b->launches - snaps[1].launches : 0;
+    for (const HostSnap& sn : snaps) sn.restore();
+    if (rc || ec != cudaSuccess || !graph) {
+        if (graph) cudaGraphDestroy(graph);
+        cudaGetLastError();
+        return rc ? 1 : a->fail(fmt("graph: stream capture failed: %s", cudaGetErrorString(ec)));
+    }
+    size_t n = 0, ne = 0;
+    std::vector<cudaGraphNode_t> nodes, from, to;
+    std::vector<cudaGraphEdgeData> ed;
+    cudaError_t e = cudaGraphGetNodes(graph, nullptr, &n);
+    if (e == cudaSuccess) { nodes.resize(n); e = cudaGraphGetNodes(graph, nodes.data(), &n); }
+    if (e == cudaSuccess) e = cudaGraphGetEdges_v2(graph, nullptr, nullptr, nullptr, &ne);
+    if (e == cudaSuccess) { from.resize(ne); to.resize(ne); ed.resize(ne); e = cudaGraphGetEdges_v2(graph, from.data(), to.data(), ed.data(), &ne); }
+    *kernels = *edges = 0;
+    for (size_t i = 0; e == cudaSuccess && i < n; ++i) {
+        cudaGraphNodeType t;
+        e = cudaGraphNodeGetType(nodes[i], &t);
+        *kernels += t == cudaGraphNodeTypeKernel;
+    }
+    for (size_t i = 0; i < ne; ++i) *edges += ed[i].type == cudaGraphDependencyTypeProgrammatic;
+    if (e != cudaSuccess) { cudaGraphDestroy(graph); return a->fail(fmt("graph: %s", cudaGetErrorString(e))); }
+    if (*kernels != *da + *db) {
+        cudaGraphDestroy(graph);
+        return a->fail(fmt("graph: %d kernels captured, the eager step counts %lld launches", *kernels, (long long)(*da + *db)));
+    }
+    *out = graph;
+    return 0;
+}
+
+// Capture the step at both parities.  Every workspace is sized first, so nothing is allocated during a capture; the slot bits are
+// taken as clean (adec_graph_launch copies dirty streams back eagerly before each launch).  Capturing both here keeps stream capture
+// out of the launches that alternate parity: a launch only instantiates, and captures again only after a reallocation.
+static int graph_capture(adec_graph* g) {
+    adec_handle *a = g->a, *b = g->b, *sh = graph_state_handle(g);
+    graph_drop(g);
+    if (size_ws(sh, graph_state_ops(g), g->B, g->kind == ADEC_GRAPH_TX ? g->T : g->F, nullptr)) {
+        if (sh != a) a->err = sh->err;
+        return 1;
+    }
+    const uint64_t ga = a->gen, gb = b ? b->gen : 0;
+    for (int p = 0; p < 2; ++p)
+        if (graph_capture_one(g, p, &g->graph[p], &g->kernels, &g->edges, &g->da, &g->db)) { graph_drop(g); return 1; }
+    if (a->gen != ga || (b && b->gen != gb)) {
+        graph_drop(g);
+        return a->fail("graph: a workspace was reallocated during the capture");
+    }
+    g->gen_a = ga;
+    g->gen_b = gb;
+    return 0;
+}
+
+static int graph_instantiate(adec_graph* g, int p) {
+    const cudaError_t e = cudaGraphInstantiateWithFlags(&g->exec[p], g->graph[p], 0);
+    if (e != cudaSuccess) { g->exec[p] = nullptr; return g->a->fail(fmt("graph: cudaGraphInstantiate failed: %s", cudaGetErrorString(e))); }
+    ++g->instantiations;
+    return 0;
+}
+
+int adec_graph_destroy(adec_graph* g) {
+    if (!g) return 0;
+    DeviceGuard dg(g->device);
+    graph_drop(g);
+    if (g->mid) cudaFree(g->mid);
+    if (g->cs) cudaStreamDestroy(g->cs);
+    delete g;
+    return 0;
+}
+
+int adec_graph_create(int kind, adec_handle* a, adec_handle* b, int B, int T_or_F, int wire, const void* in, void* out, adec_graph** out_g) {
+    if (!a || !out_g) { g_create_error = "graph_create: null argument"; return 1; }
+    *out_g = nullptr;
+    if (!a->finalized) return a->fail("graph_create: the handle is not finalized");
+    if (kind != ADEC_GRAPH_TX && kind != ADEC_GRAPH_RX) return a->fail("graph_create: kind must be ADEC_GRAPH_TX or ADEC_GRAPH_RX");
+    const bool tx = kind == ADEC_GRAPH_TX;
+    if (tx && b) return a->fail("graph_create: a transmitter graph takes no decoder handle");
+    if (!tx && (!b || !b->finalized)) return a->fail("graph_create: a receiver graph needs a finalized decoder handle");
+    if (need_full_symad(a, tx ? "graph_create (transmitter: encode, quantize)" : "graph_create (receiver: lookup)")) return 1;
+    if (b && b->device != a->device)
+        return a->fail(fmt("graph_create: the rx handle is on device %d, the decoder on device %d", a->device, b->device));
+    if (!in || !out) return a->fail("graph_create: in and out must be device buffers");
+    if (B < 1 || T_or_F < 1) return a->fail("graph_create: empty input");
+    adec_handle* sh = tx ? a : b;
+    if (B != sh->n_streams)
+        return a->fail(fmt("graph_create: batch %d != n_streams %d of the %s handle (call adec_set_streams)", B, sh->n_streams,
+                           tx ? "tx" : "decoder"));
+    if (!tx) {
+        const int zq_dim = b->cfg.model_type == ADEC_MODEL_HIFIGAN ? b->cfg.in_channels : b->cfg.code_dim;
+        if (zq_dim != a->cfg.code_dim)
+            return a->fail(fmt("graph_create: the decoder takes %d channels, the rx handle's codewords have %d", zq_dim, a->cfg.code_dim));
+    }
+    DeviceGuard dg(a->device);
+    auto* g = new adec_graph();
+    g->kind = kind; g->a = a; g->b = b; g->device = a->device; g->B = B; g->wire = wire != 0; g->in = in; g->out = out;
+    g->T = tx ? T_or_F : 0;
+    g->F = tx ? adec_frames_for(a, T_or_F) : T_or_F;
+    const size_t mid_bytes = (size_t)B * g->F * a->cfg.code_dim * (!tx && b->act_bf16 ? 2 : 4);
+    cudaError_t e = cudaStreamCreateWithFlags(&g->cs, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaMalloc(&g->mid, mid_bytes);
+    if (e != cudaSuccess) {
+        a->fail(fmt("graph_create: %s", cudaGetErrorString(e)));
+        adec_graph_destroy(g);
+        return 1;
+    }
+    const int p = list_parity(graph_state_ops(g));
+    if (p < 0) {
+        a->fail("graph_create: the stateful ops of the handle disagree on which state buffer is current");
+        adec_graph_destroy(g);
+        return 1;
+    }
+    if (graph_capture(g) || graph_instantiate(g, p)) { adec_graph_destroy(g); return 1; }
+    *out_g = g;
+    return 0;
+}
+
+int adec_graph_launch(adec_graph* g, void* stream) {
+    if (!g) return 1;
+    adec_handle *a = g->a, *b = g->b, *sh = graph_state_handle(g);
+    const cudaStream_t s = (cudaStream_t)stream;
+    DeviceGuard dg(a->device);
+    for (adec_handle* h : {a, b})     // profiling, the kernel trace and launch records see every launch: run the eager sequence
+        if (h && (h->profiling || h->d_ktrace || h->launch_log)) return graph_body(g, s);
+    if (sh->n_streams != g->B)
+        return a->fail(fmt("graph_launch: the %s handle has %d streams, the graph was made for %d (call adec_set_streams)",
+                           g->kind == ADEC_GRAPH_TX ? "tx" : "decoder", sh->n_streams, g->B));
+    std::vector<Op>& ops = graph_state_ops(g);
+    if (slot_fixup(sh, ops, s)) { if (sh != a) a->err = sh->err; return 1; }
+    const int p = list_parity(ops);
+    if (p < 0) return a->fail("graph_launch: the stateful ops of the handle disagree on which state buffer is current");
+    if ((a->gen != g->gen_a || (b && b->gen != g->gen_b)) && graph_capture(g)) return 1;
+    if (!g->exec[p] && graph_instantiate(g, p)) return 1;
+    CK(a, cudaGraphLaunch(g->exec[p], s));
+    for (Op& op : ops)
+        if (op.P > 0) op.cur ^= 1;
+    a->launches += g->da;
+    if (b && b != a) b->launches += g->db;
+    return 0;
+}
+
+int adec_graph_info(const adec_graph* g, int* kernels, int* programmatic_edges, int* instantiations) {
+    if (!g) return 1;
+    if (kernels) *kernels = g->kernels;
+    if (programmatic_edges) *programmatic_edges = g->edges;
+    if (instantiations) *instantiations = g->instantiations;
+    return 0;
+}
+
 // -------------------------------------------------------------------------------------------------
 // One test's op list (one op, or the two launches of a split residual unit) and its host I/O.  Elements are h->act_bytes() wide: fp32,
 // or bf16 words for a compute_dtype 2 handle.  Layouts as adec_test_conv_op documents them.

@@ -18,7 +18,7 @@
 //   head_kernel       - Cout = 1 last conv (+ LeakyReLU / bias / tanh for the vocoder).
 //   rvq_kernel        - 8-stage residual VQ: fp32 distances in the reference's rounding order,
 //                       first-index arg-min by warp shuffles, int64 flat indices.
-//   lookup_kernel     - codebook gather-sum.
+//   lookup_kernel     - codebook gather-sum (fp32 zq, or bf16 zq rounded once).
 //   zq_moments_kernel - per-utterance fp64 sums and centred second moments of zq (corpus statistics).
 #pragma once
 #include <cuda_bf16.h>
@@ -887,6 +887,9 @@ struct LookupArgs {
     int* err;               // bit 0 set on an out-of-range index
 };
 
+// BF16: zq is bf16 words, each value the fp32 sum rounded once to nearest even, so it equals torch's .to(torch.bfloat16) of the fp32
+// zq (the input of a decoder with bf16 activations); D % 8 == 0 keeps its rows 16-byte aligned.
+template <bool BF16>
 __global__ void __launch_bounds__(256) lookup_kernel(const LookupArgs a) {
     const int vpf = a.D / 4;    // float4 per frame
     const long long gid = (long long)blockIdx.x * 256 + threadIdx.x;
@@ -913,7 +916,10 @@ __global__ void __launch_bounds__(256) lookup_kernel(const LookupArgs a) {
         if (i == 0) s = v;
         else { s.x = __fadd_rn(s.x, v.x); s.y = __fadd_rn(s.y, v.y); s.z = __fadd_rn(s.z, v.z); s.w = __fadd_rn(s.w, v.w); }
     }
-    *reinterpret_cast<float4*>(a.zq + fr * a.D + k4) = s;
+    if constexpr (BF16)
+        *reinterpret_cast<uint2*>(reinterpret_cast<uint16_t*>(a.zq) + fr * a.D + k4) = make_uint2(bf2_bits(s.x, s.y), bf2_bits(s.z, s.w));
+    else
+        *reinterpret_cast<float4*>(a.zq + fr * a.D + k4) = s;
 }
 
 // Per-utterance moments of the quantizer output (codecStatistic.py:104-105 calls StandardScaler.partial_fit once per file), fp64

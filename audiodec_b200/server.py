@@ -29,6 +29,8 @@ from typing import Deque, Dict, List, Optional, Tuple
 import numpy as np
 import torch
 
+from .codec import ReceiverGraph, TransmitterGraph, is_library_codec
+
 
 class StreamStats:
     """Per-stream counters, same quantities as AudioCodecStreamer._exit prints (bin/stream.py:296-312)."""
@@ -77,6 +79,7 @@ class MultiStreamCodecServer:
         self._x_host = None                    # pinned staging buffers, allocated on the first step
         self._x_np = None
         self._y_host = None
+        self._graphs = None                    # (key, TransmitterGraph, ReceiverGraph) of the lock-step pass on library generators
 
     # ------------------------------------------------------------------ producer / consumer side (audio callbacks)
     def submit(self, stream: int, frame, t_capture: Optional[float] = None) -> None:
@@ -147,26 +150,10 @@ class MultiStreamCodecServer:
         held while the codec runs.  Returns (decoded frames (n, frame_size) float32, the clock when they reached the host)."""
         n = x_host.shape[0]
         with torch.no_grad(), codec_lock or contextlib.nullcontext():
-            x = x_host.to(dev, non_blocking=True)
-            if streams is None:
-                z = self.tx_encoder.encode(x)                                   # utils/audiodec.py:100-102
+            if streams is None and dev.type == "cuda" and is_library_codec(self.tx_encoder, self.rx_encoder, self.decoder):
+                y = self._graph_pass(x_host, dev)
             else:
-                z, frames = self.tx_encoder.encode_streams(list(x.view(n, -1)), streams)
-            if self.wire and hasattr(self.tx_encoder, "quantize_fused") and hasattr(self.rx_encoder, "lookup_packed"):
-                # the RVQ kernel writes the bitstream itself; the receiver looks the codewords up straight from the packed bytes
-                _, packed, _ = self.tx_encoder.quantize_fused(z, want_idx=False, want_packed=True, want_zq=False)
-                self.wire_bytes += packed.numel()
-                zq = self.rx_encoder.lookup_packed(packed)
-            elif self.wire:
-                packed = self.tx_encoder.pack(self.tx_encoder.quantize(z))
-                self.wire_bytes += packed.numel()
-                zq = self.rx_encoder.lookup(self.rx_encoder.unpack(packed))
-            else:
-                zq = self.rx_encoder.lookup(self.tx_encoder.quantize(z))
-            if streams is None:
-                y = self.decoder.decode(zq).detach()                            # utils/audiodec.py:104-106
-            else:                           # every chunk is frame_size samples: equal frame counts
-                y = torch.cat([v.reshape(1, -1) for v in self.decoder.decode_streams(zq, frames, streams)]).detach()
+                y = self._eager_pass(x_host, dev, streams)
             if y.device.type == "cuda":
                 # device -> PINNED host buffer (a pageable destination is staged through a driver bounce buffer), then one synchronise
                 if self._y_host is None or self._y_host.shape != y.shape or self._y_host.dtype != y.dtype:
@@ -180,6 +167,49 @@ class MultiStreamCodecServer:
         if y_host.dtype == torch.bfloat16:
             y_host = y_host.float()             # a bf16-activation decoder: half the D2H bytes, widened here; frames out stay float32
         return y_host.numpy().reshape(n, -1)[:, :self.frame_size].copy(), now    # one copy; the queues hold row views of it
+
+    def _eager_pass(self, x_host, dev, streams):
+        """The codec calls one by one (duck-typed codec objects, and the slot calls of SessionCodecServer) -> decoded frames."""
+        n = x_host.shape[0]
+        x = x_host.to(dev, non_blocking=True)
+        if streams is None:
+            z = self.tx_encoder.encode(x)                                   # utils/audiodec.py:100-102
+        else:
+            z, frames = self.tx_encoder.encode_streams(list(x.view(n, -1)), streams)
+        if self.wire and hasattr(self.tx_encoder, "quantize_fused") and hasattr(self.rx_encoder, "lookup_packed"):
+            # the RVQ kernel writes the bitstream itself; the receiver looks the codewords up straight from the packed bytes
+            _, packed, _ = self.tx_encoder.quantize_fused(z, want_idx=False, want_packed=True, want_zq=False)
+            self.wire_bytes += packed.numel()
+            zq = self.rx_encoder.lookup_packed(packed)
+        elif self.wire:
+            packed = self.tx_encoder.pack(self.tx_encoder.quantize(z))
+            self.wire_bytes += packed.numel()
+            zq = self.rx_encoder.lookup(self.rx_encoder.unpack(packed))
+        else:
+            zq = self.rx_encoder.lookup(self.tx_encoder.quantize(z))
+        if streams is None:
+            return self.decoder.decode(zq).detach()                         # utils/audiodec.py:104-106
+        # every chunk is frame_size samples: equal frame counts
+        return torch.cat([v.reshape(1, -1) for v in self.decoder.decode_streams(zq, frames, streams)]).detach()
+
+    def _graph_pass(self, x_host, dev):
+        """The lock-step pass on the library's generators as two graph launches (TransmitterGraph, ReceiverGraph), bit for bit the eager
+        calls.  The graphs are built on the first step and again when the shape or a generator's handle changes.  Returns the decoded
+        frames on the device (the ReceiverGraph's static output, read before the next step)."""
+        n, t = x_host.shape[0], x_host.shape[-1]
+        wire = bool(self.wire)
+        key = (n, t, wire, dev, tuple(g._h.value for g in (self.tx_encoder, self.rx_encoder, self.decoder)))
+        if self._graphs is None or self._graphs[0] != key:
+            self._graphs = None
+            frames = self.tx_encoder._lib.adec_frames_for(self.tx_encoder._h, t)
+            self._graphs = (key, TransmitterGraph(self.tx_encoder, n, t, wire=wire),
+                            ReceiverGraph(self.rx_encoder, self.decoder, n, frames, wire=wire))
+        _, txg, rxg = self._graphs
+        txg.input.copy_(x_host, non_blocking=True)
+        out = txg(txg.input)
+        if wire:
+            self.wire_bytes += out.numel()
+        return rxg(out)
 
     # ------------------------------------------------------------------ real-time loop (the two worker threads of the reference, merged)
     def start(self, period: Optional[float] = None) -> None:

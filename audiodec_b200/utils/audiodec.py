@@ -11,7 +11,7 @@ from typing import Union
 import torch
 
 from audiodec_b200.bin.stream import AudioCodec, AudioCodecStreamer
-from audiodec_b200.codec import HiFiGANStreamGenerator, SymADStreamGenerator
+from audiodec_b200.codec import HiFiGANStreamGenerator, ReceiverGraph, SymADStreamGenerator, TransmitterGraph, is_library_codec
 
 _AUTOENCODER_TYPES = ("symAudioDec", "symAudioDecUniv")      # utils/audiodec.py:36,48
 _VOCODER_TYPES = ("HiFiGAN", "UnivNet")                      # utils/audiodec.py:50
@@ -57,10 +57,37 @@ class AudioDecStreamer(AudioCodecStreamer):
                          max_latency=max_latency, tx_encoder=tx_encoder, tx_device=tx_device, rx_encoder=rx_encoder,
                          decoder=decoder, rx_device=rx_device)
 
+    # On the library's generators each worker's step is one graph launch (TransmitterGraph / ReceiverGraph).  Both graphs are made
+    # in _start_threads, on the calling thread, before the workers run: a capture must not overlap the other worker's device
+    # synchronise.  A frame of another shape, or a generator whose handle was replaced, takes the eager calls.  The static output is
+    # cloned before it goes into the queue: the other thread reads it after this thread's next launch.
+    def _start_threads(self):
+        if not self._threads_started:
+            self._tx_graph = self._rx_graph = None
+            if is_library_codec(self.tx_encoder, self.rx_encoder, self.decoder) and torch.device(self.tx_device).type == "cuda" \
+                    and torch.device(self.rx_device).type == "cuda":
+                frames = self.tx_encoder._lib.adec_frames_for(self.tx_encoder._h, self.frame_size)
+                self._tx_graph = TransmitterGraph(self.tx_encoder, 1, self.frame_size)
+                self._rx_graph = ReceiverGraph(self.rx_encoder, self.decoder, 1, frames)
+        super()._start_threads()
+
+    @staticmethod
+    def _graph_for(graph, x):
+        """the graph when x is its input's shape on its device and its generators keep their handles, else None"""
+        if graph is None or tuple(x.shape) != tuple(graph.input.shape) or x.device != graph.input.device:
+            return None
+        return graph if graph.handles_current() else None
+
     def _encode(self, x):                       # utils/audiodec.py:100-102
+        g = self._graph_for(getattr(self, "_tx_graph", None), x)
+        if g is not None:
+            return g(x).clone()
         return self.tx_encoder.quantize(self.tx_encoder.encode(x))
 
     def _decode(self, x):                       # utils/audiodec.py:104-106
+        g = self._graph_for(getattr(self, "_rx_graph", None), x)
+        if g is not None:
+            return g(x).clone()
         return self.decoder.decode(self.rx_encoder.lookup(x))
 
 

@@ -225,8 +225,39 @@ int adec_index_error(adec_handle *h, void *stream);
  * bound, so a model that gets there must run with ADEC_CONV_PATH=tf32.  adec_codec_host checks both flags itself. */
 int adec_range_error(adec_handle *h, void *stream);
 
+/* lookup / lookup_packed with bf16 zq (what a decoder with bf16 activations, compute_dtype 2, takes): the fp32 codeword sum rounded once
+ * to nearest even, equal to the fp32 zq converted to bf16.  zq 16-byte aligned; needs code_dim % 8 == 0. */
+int adec_lookup_bf16(adec_handle *h, const int64_t *idx, int B, int F, uint16_t *zq, void *stream);
+int adec_lookup_packed_bf16(adec_handle *h, const uint8_t *packed, int B, int F, uint16_t *zq, void *stream);
+
 /* number of kernel launches issued by this handle since creation (bench.py's gpu_launches) */
 int64_t adec_launch_count(const adec_handle *h);
+
+/* -- graphed stream steps: one CUDA graph launch for the launches of a transmitter or receiver step ------------------------------
+ * ADEC_GRAPH_TX (a = full symAD tx handle, b = NULL, T_or_F = samples per chunk):
+ *   in x (B, 1, T) fp32 -> adec_encode -> adec_quantize_ex -> out idx (Nq, B, F) int64, or with `wire` packed (B, F, bytes) uint8.
+ * ADEC_GRAPH_RX (a = full symAD rx handle, b = any decoder handle, may equal a; T_or_F = frames per chunk):
+ *   in idx (Nq, B, F) int64, or with `wire` packed (B, F, bytes) -> adec_lookup[_packed] -> adec_decode -> out y (B, F * hop), fp32, or
+ *   bf16 when b has bf16 activations (compute_dtype 2; the lookup then writes bf16 zq itself, adec_lookup_bf16).
+ * in and out are the caller's device buffers, fixed for the graph's life; the intermediate z / zq belongs to the graph.  B must equal
+ * n_streams of the stateful handle (a for TX, b for RX).  Creating a graph sizes the workspaces and captures the step at both parities of
+ * the double-buffered causal state on a private stream (thread-local capture mode); it runs nothing and leaves the handles' state, slot
+ * bits, launch counts and diagnostics as they were (profiling, launch records and the kernel trace are off during the capture).
+ * adec_graph_launch(g, stream) is the eager call sequence, bit for bit: outputs, causal state, flags and launch counts.  It launches the
+ * executable of the current parity, instantiated the first time that parity is launched.  A launch first copies streams that slot calls
+ * left in the other buffer back (as the uniform calls do), and captures again when a workspace or the state buffers were reallocated
+ * since the capture.  While profiling, the kernel trace or launch records are on, it runs the eager sequence instead.
+ * Stream capture happens only in adec_graph_create and in such a re-capturing launch.  CUDA forbids synchronising the device while a
+ * stream is captured, so a program whose other threads synchronise creates its graphs before those threads run.
+ * Errors are reported by adec_last_error(a) (create with a == NULL: adec_last_error(NULL)).  The handles must outlive the graph. */
+enum { ADEC_GRAPH_TX = 0, ADEC_GRAPH_RX = 1 };
+typedef struct adec_graph adec_graph;
+int adec_graph_create(int kind, adec_handle *a, adec_handle *b, int B, int T_or_F, int wire, const void *in, void *out,
+                      adec_graph **g);
+int adec_graph_launch(adec_graph *g, void *stream);
+/* kernels per step and programmatic (PDL) edges of the last capture, and the executables instantiated since creation */
+int adec_graph_info(const adec_graph *g, int *kernels, int *programmatic_edges, int *instantiations);
+int adec_graph_destroy(adec_graph *g);
 
 /* Diagnostics (handles created with ADEC_KTRACE=1 in the environment): copies up to max_records {start ns, end ns, SM cycles} records
  * of the tensor-core conv launches issued since the last call (CTA 0's globaltimer / clock64) and resets the trace; returns the
