@@ -126,8 +126,8 @@ cudaError_t launch_wg(const ConvArgs& a, int n_xtiles, int n_ytiles, int n_tiles
     cfg.numAttrs = pdl ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, kern, a, n_xtiles, n_ytiles, n_tiles);
 }
-typedef size_t (*TcSmemFn)(int, bool, bool);
-typedef int (*TcWbufFn)(int, bool, bool);
+typedef size_t (*TcSmemFn)(int, bool, bool, int);
+typedef int (*TcWbufFn)(int, bool, bool, int);
 // the paired instantiation (two output rows per MMA row): built for the fused fp16-split RU(32) only
 template <int NT, bool F, int PRE, int PREC, bool BST>
 constexpr TcPersistFn pair_fn() {
@@ -209,10 +209,10 @@ struct Op {
     // kernel config
     const ConvKernelCfg* kc = nullptr;
     const TcKernelCfg* tc = nullptr;   // tensor-core path; kc = FFMA path
-    float w_scale = 1.f, w2_scale = 1.f;
     int n_pieces = 1, n_co_tiles = 1;
     // device
     float *w = nullptr, *w2 = nullptr, *bias = nullptr;
+    float* cscale = nullptr;   // fp16-split engine: 2^-p of each output column, [G*Cout] as the bias (fuse: then [Cout] of w2)
     float* w_pair = nullptr;   // the fused RU(32): paired taps [W_j | W_j-1] for the paired kernel (TcKernelCfg::pfn_pair)
     const float *mean = nullptr, *scale = nullptr;
     float head_bias = 0.f;
@@ -479,8 +479,10 @@ int pick_piece_width(const Op& op) {
 // wgmma engines (wg_conv.cuh): weights in K-major, no-swizzle blocks of 16 bytes, the layout WgCfg streams:
 //   [group g][co tile][piece][tap][plane][kb = 16-byte K block][ntw columns][16 B]
 // ntw: columns per tile (NT; 2 NT for the paired taps); one (piece, tap) at ntw = NT is TAP_BYTES.  The planes of a weight w:
-// 3xTF32 hi | lo (4 bytes each), fp16 hi | lo | hi * 2^-11 of w * 2^p (2 bytes each), or one bf16 plane.
-std::vector<float> pack_wg(int prec, const float* weff, int G, int ntiles, int pieces, int taps, int cin_eff, int cout, int p, int ntw) {
+// 3xTF32 hi | lo (4 bytes each), fp16 hi | lo | hi * 2^-11 of w * 2^p (2 bytes each), or one bf16 plane.  p: [G * cout], the power
+// of two of each output column (fp16 only).
+std::vector<float> pack_wg(int prec, const float* weff, int G, int ntiles, int pieces, int taps, int cin_eff, int cout,
+                           const std::vector<int>& p, int ntw) {
     const int eb = prec == PREC_TF32 ? 4 : 2, npl = prec == PREC_F16 ? 3 : prec == PREC_TF32 ? 2 : 1;
     const int epb = 16 / eb, KB = TC_CP / epb;     // elements per block, K blocks per piece
     const size_t plane = (size_t)KB * ntw * epb;    // elements
@@ -501,7 +503,7 @@ std::vector<float> pack_wg(int prec, const float* weff, int G, int ntiles, int p
                                     memcpy(&v[0], &hi, 4);
                                     memcpy(&v[1], &lo, 4);
                                 } else if (prec == PREC_F16) {
-                                    const float ws = std::ldexp(w, p);
+                                    const float ws = nt * ntw + n < cout ? std::ldexp(w, p[(size_t)g * cout + nt * ntw + n]) : 0.f;
                                     v[0] = half_bits(ws);
                                     v[1] = half_bits(ws - half_value(v[0]));
                                     v[2] = half_bits(half_value(v[0]) * (1.0f / 2048.0f));
@@ -534,24 +536,39 @@ int finalize_op_wg(adec_handle* h, Op* op) {
     op->n_pieces = op->Cin_eff / TC_CP;
     op->n_co_tiles = pad_tile ? 1 : op->Cout / NT;
     op->w_tile_floats = (long long)((size_t)op->n_pieces * op->Ktaps * op->tc->tap_bytes / 4);
-    // fp16 planes hold w * 2^p with max |w * 2^p| in [4096, 8192); the kernel scales the sums back by 2^-p.  The other precisions: p = 0
-    auto pow2_scale = [prec](const std::vector<float>& w) {
-        float wmax = 0.f;
-        for (float v : w) wmax = std::max(wmax, std::fabs(v));
-        int p = 0;
-        if (prec == PREC_F16 && wmax > 0.f && std::isfinite(wmax)) {
-            while (std::ldexp(wmax, p) < 4096.f) ++p;
-            while (std::ldexp(wmax, p) >= 8192.f) --p;
+    // fp16 planes hold the weights of output column c times 2^p_c, max |w * 2^p_c| over the column in [4096, 8192), so that a column
+    // far below the op's largest weight keeps its W_lo plane normal; the kernel scales column c's sums back by 2^-p_c (cscale).
+    // p_c stays in [-127, 126]: 2^-p_c is a normal float.  A zero or non-finite column: p_c = 0.  The other precisions: p = 0
+    // (w: [G][taps][cin][cols], column g * cols + co)
+    auto pow2_scales = [prec](const std::vector<float>& w, int G, int cols) {
+        std::vector<float> wmax((size_t)G * cols, 0.f);
+        const size_t per_g = w.size() / G;
+        for (size_t i = 0; i < w.size(); ++i) {
+            float& m = wmax[i / per_g * cols + i % cols];
+            m = std::max(m, std::fabs(w[i]));
         }
+        std::vector<int> p(wmax.size(), 0);
+        for (size_t c = 0; c < p.size(); ++c)
+            if (prec == PREC_F16 && wmax[c] > 0.f && std::isfinite(wmax[c])) {
+                while (p[c] < 126 && std::ldexp(wmax[c], p[c]) < 4096.f) ++p[c];
+                while (p[c] > -127 && std::ldexp(wmax[c], p[c]) >= 8192.f) --p[c];
+            }
         return p;
     };
-    const int p1 = pow2_scale(op->weff);
-    op->w_scale = std::ldexp(1.0f, -p1);
+    std::vector<int> p1 = pow2_scales(op->weff, op->G, op->Cout), p2;
+    if (op->fuse) p2 = pow2_scales(op->weff2, 1, op->Cout);
+    if (prec == PREC_F16) {
+        std::vector<float> cs;
+        for (int p : p1) cs.push_back(std::ldexp(1.0f, -p));
+        for (int p : p2) cs.push_back(std::ldexp(1.0f, -p));
+        if (dev_upload(h, &op->cscale, cs)) return 1;
+    }
     if (dev_upload(h, &op->w, pack_wg(prec, op->weff.data(), op->G, op->n_co_tiles, op->n_pieces, op->Ktaps, op->Cin_eff, op->Cout, p1, NT)))
         return 1;
     if (op->tc->pfn_pair && op->Ktaps % 2 == 1) {
-        // the paired kernel's K + 1 taps [W_j | W_j-1] (W_-1 = W_K = 0), 2 NT columns each, same scale; uniform rows run it, stacked
-        // and varlen rows the unpaired kernel with the same one-tap groups (WgCfg::tpg), so both give the same sums
+        // the paired kernel's K + 1 taps [W_j | W_j-1] (W_-1 = W_K = 0), 2 NT columns each, both halves with column co's scale;
+        // uniform rows run it, stacked and varlen rows the unpaired kernel with the same one-tap groups (WgCfg::tpg), so both give the
+        // same sums
         const int C = op->Cout, Ci = op->Cin_eff, K = op->Ktaps;
         std::vector<float> wp((size_t)(K + 1) * Ci * 2 * C, 0.f);
         for (int j = 0; j <= K; ++j)
@@ -561,13 +578,12 @@ int finalize_op_wg(adec_handle* h, Op* op) {
                     if (j < K) row[co] = op->weff[((size_t)j * Ci + ci) * C + co];
                     if (j > 0) row[C + co] = op->weff[((size_t)(j - 1) * Ci + ci) * C + co];
                 }
-        if (dev_upload(h, &op->w_pair, pack_wg(prec, wp.data(), 1, 1, op->n_pieces, K + 1, Ci, 2 * C, p1, 2 * NT))) return 1;
+        std::vector<int> pp(p1);
+        pp.insert(pp.end(), p1.begin(), p1.end());
+        if (dev_upload(h, &op->w_pair, pack_wg(prec, wp.data(), 1, 1, op->n_pieces, K + 1, Ci, 2 * C, pp, 2 * NT))) return 1;
     }
-    if (op->fuse) {
-        const int p2 = pow2_scale(op->weff2);
-        op->w2_scale = std::ldexp(1.0f, -p2);
-        if (dev_upload(h, &op->w2, pack_wg(prec, op->weff2.data(), 1, 1, op->Cout / TC_CP, 1, op->Cout, op->Cout, p2, NT))) return 1;
-    }
+    if (op->fuse && dev_upload(h, &op->w2, pack_wg(prec, op->weff2.data(), 1, 1, op->Cout / TC_CP, 1, op->Cout, op->Cout, p2, NT)))
+        return 1;
     return 0;
 }
 
@@ -864,7 +880,7 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
             a.y_bs = op.out_nct ? (long long)op.G * op.Cout * Tout : (long long)Tout * op.ldy;
             a.mid_act = op.mid_act;
             a.hist_rep = ((rc.mode == CALL_OFFLINE || rc.mode == CALL_VARLEN) && op.up > 1) ? 1 : 0;
-            a.w_scale = op.w_scale; a.w2_scale = op.w2_scale; a.err = h->d_err;
+            a.cscale = op.cscale; a.err = h->d_err;
             if (h->d_ktrace && h->ktrace_n < 4096) a.dbg = h->d_ktrace + KT_REC * (size_t)(h->ktrace_n++);
             if (op.tc) {
                 // persistent tensor-core kernels: one CTA per SM loops over (time tile, channel tile, stream) tiles
@@ -896,8 +912,10 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
                 }
                 const long long n_tiles = (long long)grid.x * grid.y * grid.z;
                 const int n_ctas = (int)std::min<long long>(n_tiles, h->n_sms);
-                const size_t psmem = op.tc->smem(wrows, op.fuse, pair);
-                a.n_wbuf = op.tc->n_wbuf(wrows, op.fuse, pair);
+                // the fp16-split engine's per-column scales (Op::cscale) live in shared memory during the launch
+                const int sbytes = op.cscale ? (int)(((size_t)(op.G + (op.fuse ? 1 : 0)) * op.Cout * sizeof(float) + 15) / 16 * 16) : 0;
+                const size_t psmem = op.tc->smem(wrows, op.fuse, pair, sbytes);
+                a.n_wbuf = op.tc->n_wbuf(wrows, op.fuse, pair, sbytes);
                 if (a.n_wbuf < 1) return h->fail(fmt("%s: window of %d rows does not fit in shared memory", op.name.c_str(), wrows));
                 e = (vl ? op.tc->pfn_vl : pair ? op.tc->pfn_pair : op.tc->pfn)(a, (int)grid.x, (int)grid.y, (int)n_tiles, n_ctas, (int)psmem, rc.stream);
                 if (h->launch_log)

@@ -213,8 +213,9 @@ struct ConvArgs {
     int mid_act;         // FUSE: activation between the two GEMMs
     int hist_rep;        // non-streaming forward of a transposed conv: history rows = the FIRST input row (ReplicationPad1d,
                          // conv_layer.py:189-192) instead of the stored state
-    // fp16-split tensor-core engine (wg_conv.cuh): weights are stored times a power of two; the epilogue multiplies the sums by these
-    float w_scale, w2_scale;
+    // fp16-split tensor-core engine (wg_conv.cuh): each output column's weights are stored times its own power of two; the sums are
+    // multiplied by cscale[g*Cout_g + co] (FUSE: the intermediate's; the 1x1 conv's are cscale[Cout_g + co]).  nullptr otherwise
+    const float* cscale;
     int n_wbuf;          // window buffers in shared memory (1..4)
     // stacked rows: when a stream contributes fewer rows than a 128-row tile, the tiles run over ONE row space in which stream s owns
     // rows [s * stack_L, (s + 1) * stack_L), stack_L = Tout + (Ktaps - 1) * dil: local rows >= Tout are the receptive-field overlap into

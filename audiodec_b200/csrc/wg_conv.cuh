@@ -8,9 +8,11 @@
 //
 //   PREC_F16 (default, fp32-grade: every layer that must stay within 1e-4 / bit-identical indices)
 //       a     = A_hi + 2^-11 A_lo         A_hi = fp16(a),      A_lo = fp16((a - A_hi) * 2^11)        (producer warps)
-//       w * s = W_hi + W_lo               W_hi = fp16(w * s),  W_lo = fp16(w * s - W_hi),  W_his = 2^-11 W_hi   (host, s = 2^p per op:
-//                                                                                            max|w| s in [2^12, 2^13) keeps all three normal)
-//       a w s ~= A_lo W_his + A_hi W_lo + A_hi W_hi     three fp16 products, fp32 accumulation, result * 2^-p in the epilogue.
+//       w * s = W_hi + W_lo               W_hi = fp16(w * s),  W_lo = fp16(w * s - W_hi),  W_his = 2^-11 W_hi   (host, s = 2^p_c per
+//                                                                    output column c: max|w| s over the column in [2^12, 2^13) keeps
+//                                                                    the column's largest weights' three pieces normal)
+//       a w s ~= A_lo W_his + A_hi W_lo + A_hi W_hi     three fp16 products, fp32 accumulation, result * 2^-p_c in the epilogue
+//                                                       (ConvArgs::cscale).
 //     fp16 and tf32 both carry 11 significand bits, so this is as accurate as 3xTF32, at half the operand bytes per MAC.
 //     Range: |a| < 65504 (checked in the epilogue, ConvArgs::err).
 //   PREC_TF32 (ADEC_CONV_PATH=tf32): a = A_hi + A_lo, w = W_hi + W_lo in tf32; A_lo W_hi + A_hi W_lo + A_hi W_hi.  No range limit.
@@ -44,6 +46,13 @@ constexpr int TC_MIDP = 128;           // rows of the fused intermediate operand
 constexpr float F16_LO_SCALE = 2048.f; // 2^11
 enum { PREC_BF16 = 1, PREC_TF32 = 2, PREC_F16 = 3 };
 
+// two floats from a 32-bit shared-memory address: volatile, so the compiler neither hoists it out of the tile loop nor keeps a
+// generic pointer to the scales live across the kernel
+__device__ __forceinline__ float2 lds_f2(uint32_t saddr) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(saddr));
+    return v;
+}
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ADEC_PHASES builds (kernels.cuh): ADEC_PH(k) adds the SM cycles since the previous mark of this thread to phase k.  The default build
@@ -136,14 +145,16 @@ template <int NT, int PREC> struct WgCfg {
     __host__ __device__ static constexpr int win_pitch(int wrows) { return ((wrows + 1) & ~3) + 2; }   // rows, == 2 mod 4: conflict-free stores
     __host__ __device__ static constexpr int win_bytes(int wrows) { return NPL * KBB * win_pitch(wrows) * 16; }
     // window buffers: as many as fit (1..4): the producers run that many pieces ahead of the MMAs.  wrows: stored window rows
-    static int n_wbuf(int wrows, bool fuse, bool pair) {
-        const long long avail = 227 * 1024 - 512 - (long long)stages(fuse, pair) * stage_alloc(fuse, pair) - (fuse ? (long long)mid_bytes(pair) : 0);
+    // scale_bytes: the per-column weight scales at the end (PREC_F16: ConvArgs::cscale copied in at the start; 0 otherwise)
+    static int n_wbuf(int wrows, bool fuse, bool pair, int scale_bytes) {
+        const long long avail = 227 * 1024 - 512 - (long long)stages(fuse, pair) * stage_alloc(fuse, pair) - (fuse ? (long long)mid_bytes(pair) : 0) -
+                                scale_bytes;
         const long long n = avail / win_bytes(wrows);
         return (int)(n > 4 ? 4 : n);
     }
-    static size_t smem_bytes(int wrows, bool fuse, bool pair) {
-        return 512 + (size_t)stages(fuse, pair) * stage_alloc(fuse, pair) + (size_t)n_wbuf(wrows, fuse, pair) * win_bytes(wrows) +
-               (fuse ? (size_t)mid_bytes(pair) : 0);
+    static size_t smem_bytes(int wrows, bool fuse, bool pair, int scale_bytes) {
+        return 512 + (size_t)stages(fuse, pair) * stage_alloc(fuse, pair) + (size_t)n_wbuf(wrows, fuse, pair, scale_bytes) * win_bytes(wrows) +
+               (fuse ? (size_t)mid_bytes(pair) : 0) + scale_bytes;
     }
 };
 
@@ -309,6 +320,8 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
     const int win_b = Cfg::win_bytes(PAIR ? 2 * prows : wrows);
     unsigned char* wbuf0 = bst + S * STAGE_BYTES;                  // a.n_wbuf window buffers of win_b bytes
     unsigned char* mbuf = wbuf0 + (size_t)a.n_wbuf * win_b;        // FUSE only: [plane][MBLK][MIDP rows][16 B]
+    // PREC_F16: the per-column weight scales, [G * Cout_g] (FUSE: then [Cout_g] of w2), as ConvArgs::cscale, after the intermediate
+    constexpr uint32_t SCALE_OFF = FUSE ? Cfg::mid_bytes(PAIR) : 0;   // bytes past mbuf
     // PAIR: window row m (time) -> its row in the de-interleaved storage
     auto srow = [&](int m) -> int {
         if constexpr (PAIR) {
@@ -331,6 +344,12 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
         for (int s = 0; s < S; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 2); }
         for (int i = 0; i < 4; ++i) { mbar_init(&w_full[i], NPROD); mbar_init(&w_empty[i], 2); }
         mbar_fence_init();
+    }
+    if constexpr (PREC == PREC_F16) {
+        // constants, like the weights: read before griddepcontrol.wait; one shared-memory read per column pair in the tile loop
+        const int n = (n_ytiles / a.n_co_tiles + (FUSE ? 1 : 0)) * a.Cout_g;
+        float* sscale = reinterpret_cast<float*>(mbuf + SCALE_OFF);
+        for (int i = tid; i < n; i += Cfg::THREADS) sscale[i] = __ldg(a.cscale + i);
     }
     __syncthreads();
     // programmatic dependent launch: everything above - and the weight stream, weights being constants - may overlap the previous
@@ -647,6 +666,12 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
             }
         };
         // racc index of (half h, fragment register i) -> column h * PW + 8 * (i >> 2) + col2 + (i & 1), row wrow + 8 * ((i >> 1) & 1)
+        // acc_col(i), i % 4 == 0: the column of racc[i] and racc[i + 2] within the channel tile (racc[i + 1], racc[i + 3]: the next one;
+        // PAIR: the outputs t + dil have the same columns)
+        auto acc_col = [&](int i) {
+            const int fi = PAIR ? i : i % (PW / 2);
+            return ((PAIR ? 0 : i / (PW / 2) * PW) + 8 * (fi >> 2) + col2) % NT;
+        };
         for (TileIter it(blockIdx.x, gridDim.x, n_xtiles, n_ytiles); it.tile < n_tiles; it.next(gridDim.x)) {
             const int xt = it.xt, y = it.y, b = it.b;
             int g = 0, co_tile = y;
@@ -681,7 +706,12 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                 const bool ok0 = !PAIR || wrow < ttile / 2, ok8 = !PAIR || wrow + 8 < ttile / 2;
 #pragma unroll
                 for (int i = 0; i < NACC; i += 4) {
-                    const float4 m4 = apply_act_t<PRE>(make_float4(racc[i] * a.w_scale, racc[i + 1] * a.w_scale, racc[i + 2] * a.w_scale, racc[i + 3] * a.w_scale), a.slope);
+                    float4 s4 = make_float4(racc[i], racc[i + 1], racc[i + 2], racc[i + 3]);
+                    if constexpr (PREC == PREC_F16) {
+                        const float2 sc = lds_f2(mbuf_u + SCALE_OFF + 4u * (uint32_t)acc_col(i));
+                        s4 = make_float4(s4.x * sc.x, s4.y * sc.y, s4.z * sc.x, s4.w * sc.y);
+                    }
+                    const float4 m4 = apply_act_t<PRE>(s4, a.slope);
                     racc[i] = m4.x; racc[i + 1] = m4.y; racc[i + 2] = m4.z; racc[i + 3] = m4.w;
                     if (PAIR) {
                         if (ok0) vmax = fmaxf(vmax, fmaxf(fabsf(m4.x), fabsf(m4.y)));
@@ -740,10 +770,22 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
             // the loads for all the compiler knows, so it keeps every load after the stores before it; the epilogue therefore runs in
             // batches of KB column blocks over all NR rows, each issuing its bias and residual loads before its first store: one round
             // trip per batch instead of one per column pair (DESIGN §4.0).
-            // Each output is round(round(round(racc * oscale) + bias) + residual), three separately rounded operations, never an FMA.
+            // Each output is round(round(round(racc * cscale) + bias) + residual) (PREC_F16; the other precisions have no scale), three
+            // separately rounded operations, never an FMA.  The scale is applied to the accumulators first, while the batches' loads
+            // have no registers yet.
+            if constexpr (PREC == PREC_F16) {
+                const uint32_t cs = wbuf0_u + (uint32_t)a.n_wbuf * (uint32_t)win_b + SCALE_OFF +
+                                    4u * (uint32_t)((FUSE ? a.Cout_g : 0) + g * a.Cout_g + co_tile * NT);
+#pragma unroll
+                for (int i = 0; i < NACC; i += 4) {
+                    const int co = acc_col(i);
+                    const float2 sc = co_tile * NT + co < a.Cout_g ? lds_f2(cs + 4u * (uint32_t)co) : make_float2(0.f, 0.f);
+                    racc[i] = __fmul_rn(racc[i], sc.x); racc[i + 1] = __fmul_rn(racc[i + 1], sc.y);
+                    racc[i + 2] = __fmul_rn(racc[i + 2], sc.x); racc[i + 3] = __fmul_rn(racc[i + 3], sc.y);
+                }
+            }
             constexpr int PB = NT < 128 ? 16 : (PREC == PREC_TF32 && FUSE) || VL ? 4 : 8;   // residual pairs per batch: larger ones spill
             constexpr int NR = PAIR ? 4 : 2, NCB = NACC / (2 * NR), KB = NCB < PB / NR ? NCB : PB / NR;
-            const float oscale = FUSE ? a.w2_scale : a.w_scale;
             const int co0 = co_tile * NT + col2;     // columns from Cout_g on: the zero-padded part of a channel tile (96 outputs of 128)
             int rt[NR], rbo[NR];                     // output row and stream of row rr, rt = -1: not stored
             {
@@ -807,7 +849,7 @@ __global__ void __launch_bounds__(WgCfg<NT, PREC>::THREADS, 1) wg_conv_kernel(co
                     for (int k = 0; k < KB; ++k) {
                         const int co_l = co0 + 8 * (k0 + k), i = 4 * (k0 + k) + 2 * (rr & 1) + (PW / 2) * (rr >> 1);
                         if (co_l >= a.Cout_g) continue;
-                        float v0 = __fmul_rn(racc[i], oscale), v1 = __fmul_rn(racc[i + 1], oscale);
+                        float v0 = racc[i], v1 = racc[i + 1];
                         if (a.bias) { v0 = __fadd_rn(v0, bb[k].x); v1 = __fadd_rn(v1, bb[k].y); }
                         if (a.res) { v0 = __fadd_rn(r2[rr][k].x, v0); v1 = __fadd_rn(r2[rr][k].y, v1); }
                         vmax = fmaxf(vmax, fmaxf(fabsf(v0), fabsf(v1)));
