@@ -40,7 +40,7 @@ class AdecConfig(ctypes.Structure):
     ]
 
 
-MODEL_SYMAD, MODEL_HIFIGAN, MODEL_SYMAD_DECODER = 0, 1, 2
+MODEL_SYMAD, MODEL_HIFIGAN, MODEL_SYMAD_DECODER, MODEL_SYMAD_ENCODER = 0, 1, 2, 3
 GRAPH_TX, GRAPH_RX = 0, 1
 
 
@@ -84,6 +84,12 @@ SYMBOLS = {
     "adec_encode_offline": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "adec_decode_offline": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "adec_decode_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "adec_encode_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "adec_encode_offline_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "adec_encode_offline_varlen_bf16": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),
+    "adec_encode_streams_bf16": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),
+    "adec_quantize_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "adec_quantize_ex_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "adec_decode_offline_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "adec_encode_offline_varlen": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),
     "adec_decode_offline_varlen": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_int), c_int, c_void_p, c_void_p]),

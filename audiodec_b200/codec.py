@@ -22,6 +22,8 @@ Differences from the reference, all extensions:
     layout and dtype contract of the reference's ``decoder.to(torch.bfloat16)``); plain ``.to(torch.bfloat16)`` rounds only the
     conv operands and keeps fp32 activations and fp32 I/O.  ``SymADDecoderStreamGenerator`` is the symAD decoder alone, the
     object the reference's receiver decodes with; a full ``SymADStreamGenerator`` stays fp32-grade.
+  * ``SymADEncoderStreamGenerator`` is the symAD transmitter alone (encoder, projector and RVQ search), the reference's
+    ``tx_encoder``.  Its ``.to(torch.bfloat16)`` runs the encoder's convs on bf16 operands with fp32 activations, state, x and z.
 """
 from __future__ import annotations
 
@@ -105,7 +107,8 @@ class _StreamGeneratorBase:
         self._act_bf16 = False        # decoders only (set_activation_dtype): bf16 activations, state and decode I/O = compute_dtype 2
         self._layout = None           # state_layout, read from the handle once
 
-    # the decoder-only generators (HiFi-GAN vocoder, symAD decoder) have the bf16 modes; a full symAD generator does not
+    # the decoder-only generators (HiFi-GAN vocoder, symAD decoder) and the symAD encoder-only generator have the bf16 modes; a full
+    # symAD generator does not
     _bf16_modes = False
 
     # -- torch.nn.Module look-alikes ------------------------------------------------------------
@@ -195,7 +198,7 @@ class _StreamGeneratorBase:
             want = 1
         else:
             raise NotImplementedError(f"{type(self).__name__} has no {dtype} mode (fp32 everywhere; bf16 for the decoder-only generators: "
-                                      "HiFiGANStreamGenerator, SymADDecoderStreamGenerator)")
+                                      "HiFiGANStreamGenerator, SymADDecoderStreamGenerator, and the encoder-only SymADEncoderStreamGenerator)")
         mode = 2 if self._act_bf16 else want
         if self._h is not None and mode != self._cfg.compute_dtype:
             raise RuntimeError("set the compute dtype before .to(device): the weights are packed when the handle is created")
@@ -461,7 +464,144 @@ def _symad_signature(init):
     return init
 
 
-class SymADStreamGenerator(_StreamGeneratorBase):
+class _SymADTransmitter(_StreamGeneratorBase):
+    """The transmitter side of a symAD generator, shared by the full generator and the encoder-only one: encode (streaming, offline,
+    varlen, stream slots), quantize to indices / packed bytes, and pack.  With bf16 activations (the encoder-only generator's
+    set_activation_dtype(torch.bfloat16)) x and z are bf16 on the device: fp32 inputs are cast there, and z comes back bf16."""
+
+    @property
+    def _act_dtype(self):
+        return torch.bfloat16 if self._act_bf16 else torch.float32
+
+    def _tx_in(self, t):
+        """x or z on the codec's device, contiguous, in the activation dtype, 16-byte aligned (the bf16 kernels read whole vectors)"""
+        t = self._in(t, self._act_dtype)
+        return t.clone() if self._act_bf16 and t.data_ptr() % 16 else t
+
+    def encode(self, x):
+        """(B,1,T) float -> z (B,code_dim,F)   (AudioDec.py:228-234)"""
+        self._ready()
+        if x.dim() != 3:
+            raise RuntimeError("encode expects (batch, channel, length)")
+        if x.size(1) != self.input_channels:
+            x = x.reshape(-1, self.input_channels, x.size(-1))
+        x = self._tx_in(x)
+        b, _, t = x.shape
+        self._batch(b)
+        f = self._lib.adec_frames_for(self._h, t)
+        z = torch.empty(b, self.code_dim, f, device=self._device, dtype=self._act_dtype)
+        _check(self._fn("adec_encode")(self._h, _ptr(x), b, t, _ptr(z), self._stream()), self._h)
+        return z
+
+    def quantize(self, z):
+        """z (B,code_dim,F) -> idx int64 (Nq,F) for B==1 else (Nq,B,F)   (AudioDec.py:237-239)"""
+        self._ready()
+        self._want(z, "quantize", 1, self.code_dim)
+        z = self._tx_in(z)
+        b, _, f = z.shape
+        idx = torch.empty(self.codebook_num, b, f, device=self._device, dtype=torch.int64)
+        _check(self._fn("adec_quantize")(self._h, _ptr(z), b, f, _ptr(idx), self._stream()), self._h)
+        return idx.squeeze(1) if b == 1 else idx
+
+    def quantize_fused(self, z, want_idx=True, want_packed=False, want_zq=True):
+        """quantize -> [pack] -> lookup in ONE launch (adec_quantize_ex): returns (idx or None, packed or None, zq or None) with the
+        shapes of quantize() / pack() / lookup().  Bit-identical to the three separate calls."""
+        self._ready()
+        self._want(z, "quantize_fused", 1, self.code_dim)
+        if want_zq and not hasattr(self, "lookup"):
+            raise RuntimeError(f"audiodec_b200: quantize_fused: {type(self).__name__} has no lookup; pass want_zq=False")
+        z = self._tx_in(z)
+        b, _, f = z.shape
+        idx = torch.empty(self.codebook_num, b, f, device=self._device, dtype=torch.int64) if want_idx else None
+        packed = torch.empty(b, f, self.packed_frame_bytes(), device=self._device, dtype=torch.uint8) if want_packed else None
+        zq = torch.empty(b, f, self.code_dim, device=self._device, dtype=torch.float32) if want_zq else None
+        _check(self._fn("adec_quantize_ex")(self._h, _ptr(z), b, f, _ptr(idx) if want_idx else None, _ptr(packed) if want_packed else None,
+                                          _ptr(zq) if want_zq else None, self._stream()), self._h)
+        if b == 1:
+            idx = idx.squeeze(1) if idx is not None else None
+            packed = packed.squeeze(0) if packed is not None else None
+        return idx, packed, zq
+
+    # ---- non-streaming batch forward (SURVEY.md 8(f) rank 4; codecTest.py:78-95).  These calls discard the streaming state.
+    def encode_offline(self, x):
+        """x (B,1,T) -> z (B,code_dim,F): Encoder.forward + Projector.forward, zero left-pad (conv_layer.py:148-151)."""
+        self._ready()
+        if x.dim() != 3:
+            raise RuntimeError("encode_offline expects (batch, channel, length)")
+        if x.size(1) != self.input_channels:                 # same fold as encode(): every audio channel is its own batch row
+            x = x.reshape(-1, self.input_channels, x.size(-1))
+        x = self._tx_in(x)
+        b, _, t = x.shape
+        f = self._lib.adec_frames_for(self._h, t)
+        z = torch.empty(b, self.code_dim, f, device=self._device, dtype=self._act_dtype)
+        _check(self._fn("adec_encode_offline")(self._h, _ptr(x), b, t, _ptr(z), self._stream()), self._h)
+        return z
+
+    def encode_offline_varlen(self, xs):
+        """Utterances of different lengths in one launch sequence: xs is a list of 1-D (T_b,) or (1, T_b) tensors.  Returns
+        (z (1, code_dim, sum F_b), [F_b]); utterance b's frames are columns [sum_{i<b} F_i, +F_b) and equal encode_offline of that
+        utterance alone.  z is quantize's B = 1 layout (and quantize_offline's), so one call quantizes the whole batch."""
+        self._ready()
+        if len(xs) == 0:
+            raise RuntimeError("audiodec_b200: encode_offline_varlen: no utterances")
+        return self._encode_varlen(self._fn("adec_encode_offline_varlen"), "encode_offline_varlen", "utterances", xs)
+
+    def encode_streams(self, chunks, streams):
+        """Advance streams[b] by chunks[b] (1-D (T_b,) or (1, T_b); lengths may differ) in one launch sequence.  Returns
+        (z (1, code_dim, sum F_b), [F_b]) laid out like encode_offline_varlen; stream b's frames equal a B = 1 streaming encode of its
+        chunk.  Streams not listed keep their state untouched."""
+        self._ready()
+        if len(chunks) != len(streams):
+            raise RuntimeError(f"audiodec_b200: encode_streams: {len(chunks)} chunks for {len(streams)} streams")
+        sarr, _ = _int_array(streams)
+        return self._encode_varlen(self._fn("adec_encode_streams"), "encode_streams", "chunks", chunks, sarr)
+
+    def _encode_varlen(self, fn, what, noun, xs, *slots):
+        """Encode 1-D (T_b,) or (1, T_b) tensors concatenated into one varlen row space through `fn` (its stream array: `slots`) ->
+        (z (1, code_dim, sum F_b), [F_b])."""
+        flat = []
+        for x in xs:
+            x = x[0] if x.dim() == 2 and x.size(0) == 1 else x
+            if x.dim() != 1:
+                raise RuntimeError(f"audiodec_b200: {what}: expected 1-D (T,) or (1, T) {noun}, got {tuple(x.shape)}")
+            flat.append(self._in(x, self._act_dtype))
+        lengths = [x.numel() for x in flat]
+        frames, offsets = varlen_layout(lengths, self.enc_strides)
+        x = torch.cat(flat) if flat else torch.empty(0, device=self._device, dtype=self._act_dtype)
+        z = torch.empty(1, self.code_dim, offsets[-1], device=self._device, dtype=self._act_dtype)
+        arr, b = _int_array(lengths)
+        _check(fn(self._h, _ptr(x), arr, *slots, b, _ptr(z), self._stream()), self._h)
+        return z, frames
+
+    # ---- index bitstream (SURVEY.md 8(f) rank 2; the reference queues the raw int64 tensor, bin/stream.py:224)
+    def packed_frame_bytes(self):
+        self._ready()
+        return self._lib.adec_packed_frame_bytes(self._h)
+
+    def pack(self, idx):
+        """idx (Nq,F) -> uint8 (F,bytes); (Nq,B,F) -> (B,F,bytes): Nq x ceil(log2 N)-bit local indices per frame."""
+        self._ready()
+        idx = self._in(idx, torch.int64)
+        two_d = idx.dim() == 2
+        if two_d:
+            idx = idx.unsqueeze(1)
+        nq, b, f = idx.shape
+        if nq != self.codebook_num:
+            raise RuntimeError(f"audiodec_b200: pack: expected {self.codebook_num} index rows, got {nq}")
+        out = torch.empty(b, f, self.packed_frame_bytes(), device=self._device, dtype=torch.uint8)
+        _check(self._lib.adec_pack_indices(self._h, _ptr(idx), b, f, _ptr(out), self._stream()), self._h)
+        return out.squeeze(0) if two_d else out
+
+    def index_error(self):
+        """True if lookup / pack / unpack met an out-of-range index since the last call (synchronises the stream)."""
+        self._ready()
+        rc = self._lib.adec_index_error(self._h, self._stream())
+        if rc < 0:
+            raise RuntimeError("audiodec_b200: " + _lib.last_error(self._h))
+        return bool(rc)
+
+
+class SymADStreamGenerator(_SymADTransmitter):
     """models/autoencoder/AudioDec.py:166-256."""
 
     @_symad_signature
@@ -478,48 +618,6 @@ class SymADStreamGenerator(_StreamGeneratorBase):
 
     def initial_decoder(self, zq):
         self.decode(zq)                                                              # AudioDec.py:224-225
-
-    def encode(self, x):
-        """(B,1,T) float -> z (B,code_dim,F)   (AudioDec.py:228-234)"""
-        self._ready()
-        if x.dim() != 3:
-            raise RuntimeError("encode expects (batch, channel, length)")
-        if x.size(1) != self.input_channels:
-            x = x.reshape(-1, self.input_channels, x.size(-1))
-        x = self._in(x)
-        b, _, t = x.shape
-        self._batch(b)
-        f = self._lib.adec_frames_for(self._h, t)
-        z = torch.empty(b, self.code_dim, f, device=self._device, dtype=torch.float32)
-        _check(self._lib.adec_encode(self._h, _ptr(x), b, t, _ptr(z), self._stream()), self._h)
-        return z
-
-    def quantize(self, z):
-        """z (B,code_dim,F) -> idx int64 (Nq,F) for B==1 else (Nq,B,F)   (AudioDec.py:237-239)"""
-        self._ready()
-        self._want(z, "quantize", 1, self.code_dim)
-        z = self._in(z)
-        b, _, f = z.shape
-        idx = torch.empty(self.codebook_num, b, f, device=self._device, dtype=torch.int64)
-        _check(self._lib.adec_quantize(self._h, _ptr(z), b, f, _ptr(idx), self._stream()), self._h)
-        return idx.squeeze(1) if b == 1 else idx
-
-    def quantize_fused(self, z, want_idx=True, want_packed=False, want_zq=True):
-        """quantize -> [pack] -> lookup in ONE launch (adec_quantize_ex): returns (idx or None, packed or None, zq or None) with the
-        shapes of quantize() / pack() / lookup().  Bit-identical to the three separate calls."""
-        self._ready()
-        self._want(z, "quantize_fused", 1, self.code_dim)
-        z = self._in(z)
-        b, _, f = z.shape
-        idx = torch.empty(self.codebook_num, b, f, device=self._device, dtype=torch.int64) if want_idx else None
-        packed = torch.empty(b, f, self.packed_frame_bytes(), device=self._device, dtype=torch.uint8) if want_packed else None
-        zq = torch.empty(b, f, self.code_dim, device=self._device, dtype=torch.float32) if want_zq else None
-        _check(self._lib.adec_quantize_ex(self._h, _ptr(z), b, f, _ptr(idx) if want_idx else None, _ptr(packed) if want_packed else None,
-                                          _ptr(zq) if want_zq else None, self._stream()), self._h)
-        if b == 1:
-            idx = idx.squeeze(1) if idx is not None else None
-            packed = packed.squeeze(0) if packed is not None else None
-        return idx, packed, zq
 
     def lookup_packed(self, packed, dtype=torch.float32):
         """uint8 (F,bytes) -> zq (1,F,D); (B,F,bytes) -> (B,F,D): lookup straight from the bitstream (unpack fused into lookup).
@@ -555,57 +653,6 @@ class SymADStreamGenerator(_StreamGeneratorBase):
         zq = torch.empty(b, f, self.code_dim, device=self._device, dtype=dtype)
         _check(fn(self._h, _ptr(idx), b, f, _ptr(zq), self._stream()), self._h)
         return zq
-
-    # ---- non-streaming batch forward (SURVEY.md 8(f) rank 4; codecTest.py:78-95).  These calls discard the streaming state.
-    def encode_offline(self, x):
-        """x (B,1,T) -> z (B,code_dim,F): Encoder.forward + Projector.forward, zero left-pad (conv_layer.py:148-151)."""
-        self._ready()
-        if x.dim() != 3:
-            raise RuntimeError("encode_offline expects (batch, channel, length)")
-        if x.size(1) != self.input_channels:                 # same fold as encode(): every audio channel is its own batch row
-            x = x.reshape(-1, self.input_channels, x.size(-1))
-        x = self._in(x)
-        b, _, t = x.shape
-        f = self._lib.adec_frames_for(self._h, t)
-        z = torch.empty(b, self.code_dim, f, device=self._device, dtype=torch.float32)
-        _check(self._lib.adec_encode_offline(self._h, _ptr(x), b, t, _ptr(z), self._stream()), self._h)
-        return z
-
-    def encode_offline_varlen(self, xs):
-        """Utterances of different lengths in one launch sequence: xs is a list of 1-D (T_b,) or (1, T_b) tensors.  Returns
-        (z (1, code_dim, sum F_b), [F_b]); utterance b's frames are columns [sum_{i<b} F_i, +F_b) and equal encode_offline of that
-        utterance alone.  z is quantize_offline's B = 1 layout, so one quantize_offline call quantizes the whole batch."""
-        self._ready()
-        if len(xs) == 0:
-            raise RuntimeError("audiodec_b200: encode_offline_varlen: no utterances")
-        return self._encode_varlen(self._lib.adec_encode_offline_varlen, "encode_offline_varlen", "utterances", xs)
-
-    def encode_streams(self, chunks, streams):
-        """Advance streams[b] by chunks[b] (1-D (T_b,) or (1, T_b); lengths may differ) in one launch sequence.  Returns
-        (z (1, code_dim, sum F_b), [F_b]) laid out like encode_offline_varlen; stream b's frames equal a B = 1 streaming encode of its
-        chunk.  Streams not listed keep their state untouched."""
-        self._ready()
-        if len(chunks) != len(streams):
-            raise RuntimeError(f"audiodec_b200: encode_streams: {len(chunks)} chunks for {len(streams)} streams")
-        sarr, _ = _int_array(streams)
-        return self._encode_varlen(self._lib.adec_encode_streams, "encode_streams", "chunks", chunks, sarr)
-
-    def _encode_varlen(self, fn, what, noun, xs, *slots):
-        """Encode 1-D (T_b,) or (1, T_b) tensors concatenated into one varlen row space through `fn` (its stream array: `slots`) ->
-        (z (1, code_dim, sum F_b), [F_b])."""
-        flat = []
-        for x in xs:
-            x = x[0] if x.dim() == 2 and x.size(0) == 1 else x
-            if x.dim() != 1:
-                raise RuntimeError(f"audiodec_b200: {what}: expected 1-D (T,) or (1, T) {noun}, got {tuple(x.shape)}")
-            flat.append(self._in(x))
-        lengths = [x.numel() for x in flat]
-        frames, offsets = varlen_layout(lengths, self.enc_strides)
-        x = torch.cat(flat) if flat else torch.empty(0, device=self._device)
-        z = torch.empty(1, self.code_dim, offsets[-1], device=self._device, dtype=torch.float32)
-        arr, b = _int_array(lengths)
-        _check(fn(self._h, _ptr(x), arr, *slots, b, _ptr(z), self._stream()), self._h)
-        return z, frames
 
     def decode_streams(self, zq, frames, streams):
         """Advance streams[b] by frames[b] frames of zq ((1, sum F_b, code_dim) or (sum F_b, code_dim) channels-last, as lookup
@@ -668,25 +715,6 @@ class SymADStreamGenerator(_StreamGeneratorBase):
         that utterance alone."""
         return self._decode_offline_varlen(zq, frames)
 
-    # ---- index bitstream (SURVEY.md 8(f) rank 2; the reference queues the raw int64 tensor, bin/stream.py:224)
-    def packed_frame_bytes(self):
-        self._ready()
-        return self._lib.adec_packed_frame_bytes(self._h)
-
-    def pack(self, idx):
-        """idx (Nq,F) -> uint8 (F,bytes); (Nq,B,F) -> (B,F,bytes): Nq x ceil(log2 N)-bit local indices per frame."""
-        self._ready()
-        idx = self._in(idx, torch.int64)
-        two_d = idx.dim() == 2
-        if two_d:
-            idx = idx.unsqueeze(1)
-        nq, b, f = idx.shape
-        if nq != self.codebook_num:
-            raise RuntimeError(f"audiodec_b200: pack: expected {self.codebook_num} index rows, got {nq}")
-        out = torch.empty(b, f, self.packed_frame_bytes(), device=self._device, dtype=torch.uint8)
-        _check(self._lib.adec_pack_indices(self._h, _ptr(idx), b, f, _ptr(out), self._stream()), self._h)
-        return out.squeeze(0) if two_d else out
-
     def unpack(self, packed):
         """uint8 (F,bytes) -> idx (Nq,F); (B,F,bytes) -> (Nq,B,F) int64 flat indices, ready for lookup()."""
         self._ready()
@@ -701,19 +729,43 @@ class SymADStreamGenerator(_StreamGeneratorBase):
         _check(self._lib.adec_unpack_indices(self._h, _ptr(packed), b, f, _ptr(idx), self._stream()), self._h)
         return idx.squeeze(1) if two_d else idx
 
-    def index_error(self):
-        """True if lookup / pack / unpack met an out-of-range index since the last call (synchronises the stream)."""
-        self._ready()
-        rc = self._lib.adec_index_error(self._h, self._stream())
-        if rc < 0:
-            raise RuntimeError("audiodec_b200: " + _lib.last_error(self._h))
-        return bool(rc)
-
     def decode(self, zq):
         """zq (B,F,D) channels-last -> y (B,1,F*hop)   (AudioDec.py:246-247)"""
         self._ready()
         self._want(zq, "decode", 2, self.code_dim)
         return self._decode(zq)
+
+
+
+class SymADEncoderStreamGenerator(_SymADTransmitter):
+    """The transmitter of a symAD StreamGenerator alone (models/autoencoder/AudioDec.py:216-239): what the reference's transmitter
+    runs as its `tx_encoder` object (initial_encoder / encode / quantize, utils/audiodec.py:100-102).  Same constructor keywords as
+    SymADStreamGenerator, and it loads the same state dict (the decoder keys are ignored).  In fp32 it encodes and quantizes what
+    SymADStreamGenerator gives, bit for bit, in every call mode.  `.to(torch.bfloat16)` runs the encoder's and the projector's convs on
+    bf16 operands (fp32 accumulation; the stem keeps fp32 weights), with fp32 x, activations, state and z, and the RVQ unchanged on
+    that z; `set_activation_dtype(torch.bfloat16)` also keeps x, every activation, the causal state and z in bf16, as the reference's
+    `tx_encoder.to(torch.bfloat16)` stores them (encode takes fp32 or bf16 x and returns bf16 z; the RVQ widens it exactly).  Both
+    change some code indices.  It has no decode or lookup: a receiver needs a full generator's codebooks."""
+    _bf16_modes = True
+
+    @_symad_signature
+    def __init__(self, *args, **params):
+        super().__init__()
+        _symad_init(self, _lib.MODEL_SYMAD_ENCODER, *args, **params)
+
+    def initial_encoder(self, receptive_length, device):
+        """AudioDec.py:216-221 without the lookup: push `receptive_length` zeros through encode and quantize (the transmitter's warm-up,
+        bin/stream.py:49, which discards the result)."""
+        self._ready()
+        self.quantize(self.encode(torch.zeros(1, self.input_channels, receptive_length, device=self._device)))
+
+    def quantize_offline(self, z):
+        """z (B,code_dim,F) -> idx (Nq,B,F): the indices of Quantizer.forward (quantizer.py:31-34) without its zq, which needs the
+        codebooks' lookup (a full generator's quantize_offline)."""
+        self._ready()
+        self._want(z, "quantize_offline", 1, self.code_dim)
+        idx = self.quantize(z)
+        return idx.unsqueeze(1) if idx.dim() == 2 else idx
 
 
 class SymADDecoderStreamGenerator(_StreamGeneratorBase):
@@ -886,19 +938,20 @@ class _StepGraph:
 
 
 class TransmitterGraph(_StepGraph):
-    """tx_encoder.encode(x) -> tx_encoder.quantize(z) for n_streams streams of `chunk` samples as one CUDA graph launch; with wire,
-    quantize_fused(z, want_idx=False, want_packed=True, want_zq=False) instead.  `input` is x (n_streams, 1, chunk) float32; `output`
+    """tx_encoder.encode(x) -> tx_encoder.quantize(z) (tx_encoder: a full or encoder-only symAD generator) for n_streams streams of `chunk` samples as one CUDA graph launch; with wire,
+    quantize_fused(z, want_idx=False, want_packed=True, want_zq=False) instead.  `input` is x (n_streams, 1, chunk), float32 (bf16 for a
+    transmitter with bf16 activations, which also takes float32 x and casts it); `output`
     is what the eager calls return: indices (Nq, F) for one stream, (Nq, n_streams, F) otherwise, or with wire the packed bytes
     (F, bytes) / (n_streams, F, bytes).  The output is overwritten by the next call."""
 
     def __init__(self, tx_encoder, n_streams, chunk, wire=False):
-        if not isinstance(tx_encoder, SymADStreamGenerator):
-            raise TypeError(f"audiodec_b200: TransmitterGraph needs a SymADStreamGenerator (encoder, projector and RVQ), got "
-                            f"{type(tx_encoder).__name__}")
+        if not isinstance(tx_encoder, _SymADTransmitter):
+            raise TypeError(f"audiodec_b200: TransmitterGraph needs a SymADStreamGenerator or SymADEncoderStreamGenerator (encoder, "
+                            f"projector and RVQ), got {type(tx_encoder).__name__}")
         tx_encoder._ready()
         dev, b = tx_encoder._device, int(n_streams)
         f = tx_encoder._lib.adec_frames_for(tx_encoder._h, int(chunk))
-        self.input = torch.zeros(b, tx_encoder.input_channels, int(chunk), device=dev, dtype=torch.float32)
+        self.input = torch.zeros(b, tx_encoder.input_channels, int(chunk), device=dev, dtype=tx_encoder._act_dtype)
         if wire:
             raw = torch.empty(b, f, tx_encoder.packed_frame_bytes(), device=dev, dtype=torch.uint8)
             self.output = raw.squeeze(0) if b == 1 else raw
@@ -935,7 +988,7 @@ class ReceiverGraph(_StepGraph):
 
 def is_library_codec(tx_encoder, rx_encoder, decoder):
     """True when the three codec objects are this library's generators on a CUDA device, so a stream step can run as graphs."""
-    return (isinstance(tx_encoder, SymADStreamGenerator) and isinstance(rx_encoder, SymADStreamGenerator)
+    return (isinstance(tx_encoder, _SymADTransmitter) and isinstance(rx_encoder, SymADStreamGenerator)
             and isinstance(decoder, _StreamGeneratorBase) and all(g._h is not None for g in (tx_encoder, rx_encoder, decoder)))
 
 

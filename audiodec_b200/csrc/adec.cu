@@ -530,7 +530,8 @@ int finalize_op_wg(adec_handle* h, Op* op) {
     const bool pad_tile = !op->fuse && NT == 32 && op->Cout > 64 && op->Cout < 128;
     if (pad_tile) NT = 128;
     const int prec = h->engine == 1 ? PREC_TF32 : h->bf16 ? PREC_BF16 : PREC_F16;
-    if (h->act_bf16 && op->RG > 1) return h->fail(op->name + ": bf16 activations are built for stride-1 and transposed convs only");
+    // bf16 storage reads a window row as whole 16-byte vectors of one s * Cin row: no 4-channel strided convs
+    if (h->act_bf16 && op->RG > 1 && op->Cin < 8) return h->fail(op->name + ": bf16 activations need strided convs with Cin >= 8");
     op->tc = find_tc_kernel(NT, op->fuse, op->pre_act, prec, h->act_bf16);
     if (!op->tc || (op->fuse && (NT != op->Cout || op->mid_act != op->pre_act))) return h->fail(op->name + ": no tensor-core kernel");
     op->n_pieces = op->Cin_eff / TC_CP;
@@ -850,7 +851,9 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
             a.w = op.w; a.bias = op.bias; a.y = yout; a.y_bs = (long long)T * op.ldy;
             a.vl_off = vl_in; a.vl_B = rc.B; a.vl_slot = vl_slot;
             dim3 grid((T + 1023) / 1024, nb);
-            if (vl) stem_kernel<32, 7, true><<<grid, 256, 0, rc.stream>>>(a);
+            if (vl && h->act_bf16) stem_kernel<32, 7, true, true><<<grid, 256, 0, rc.stream>>>(a);
+            else if (vl) stem_kernel<32, 7, true><<<grid, 256, 0, rc.stream>>>(a);
+            else if (h->act_bf16) stem_kernel<32, 7, false, true><<<grid, 256, 0, rc.stream>>>(a);
             else stem_kernel<32, 7><<<grid, 256, 0, rc.stream>>>(a);
             e = cudaGetLastError();
         } else if (op.kind == OP_HEAD) {
@@ -931,7 +934,7 @@ int run_ops(adec_handle* h, std::vector<Op>& ops, const RunCtx& rc, int T_in, in
         }
         if (h->launch_log && op.kind != OP_CONV)
             h->launch_log->insert(h->launch_log->end(), {op.kind == OP_STEM ? ADEC_TEST_LAUNCH_STEM : ADEC_TEST_LAUNCH_HEAD, 0, 0, op.pre_act,
-                                                         0, vl, 0, 0, op.kind == OP_HEAD && h->act_bf16});
+                                                         0, vl, 0, 0, h->act_bf16});
         if (e != cudaSuccess) return h->fail(fmt("launch of %s failed: %s", op.name.c_str(), cudaGetErrorString(e)));
         ++h->launches;
         if (h->profiling) {
@@ -1097,10 +1100,10 @@ int build_symad_decoder_only(adec_handle* h) {
     return 0;
 }
 
-int build_symad(adec_handle* h) {
+// ---- encoder (models/autoencoder/modules/encoder.py:84-142) and projector: what a full symAD handle and an encoder-only one
+// (ADEC_MODEL_SYMAD_ENCODER) both encode with
+int build_symad_encoder(adec_handle* h) {
     const adec_config& c = h->cfg;
-    if (check_symad_cfg(h)) return 1;
-    // ---- encoder (models/autoencoder/modules/encoder.py:84-142)
     Wire w; w.cur = BUF_EXT_IN; w.cur_ld = 1;
     {
         Op op;
@@ -1136,8 +1139,12 @@ int build_symad(adec_handle* h) {
         if (op.Cout != c.code_dim) return h->fail("projector: code_dim must be a multiple of 32");
         h->enc_ops.push_back(std::move(op));
     }
-    if (build_symad_decoder(h)) return 1;
-    // ---- residual VQ (layers/vq_module.py)
+    return 0;
+}
+
+// ---- residual VQ (layers/vq_module.py): the codebooks of a full symAD handle and of an encoder-only one
+int build_symad_rvq(adec_handle* h) {
+    const adec_config& c = h->cfg;
     const int nq = c.codebook_num, D = c.code_dim, N = c.codebook_size;
     if (N != 1024) return h->fail("RVQ: only codebook_size=1024 is built");
     std::vector<float> embed((size_t)nq * D * N), e2((size_t)nq * N), cb((size_t)nq * N * D);
@@ -1164,6 +1171,18 @@ int build_symad(adec_handle* h) {
         find(h, fmt("quantizer.codebook.layers.%d.embed_avg", i));
     }
     if (dev_upload(h, &h->d_embed, embed) || dev_upload(h, &h->d_e2, e2) || dev_upload(h, &h->d_codebook, cb)) return 1;
+    return 0;
+}
+
+int build_symad(adec_handle* h) {
+    return check_symad_cfg(h) || build_symad_encoder(h) || build_symad_decoder(h) || build_symad_rvq(h);
+}
+
+// The encoder-only handle loads a full generator state dict: the decoder keys are accepted and ignored.
+int build_symad_encoder_only(adec_handle* h) {
+    if (check_symad_cfg(h) || build_symad_encoder(h) || build_symad_rvq(h)) return 1;
+    for (const auto& kv : h->tensors)
+        if (kv.first.compare(0, 8, "decoder.") == 0) h->consumed.insert(kv.first);
     return 0;
 }
 
@@ -1321,19 +1340,32 @@ int build_hifigan(adec_handle* h) {
 
 int hop_of(const adec_handle* h) {
     int hop = 1;
-    if (h->cfg.model_type == ADEC_MODEL_SYMAD) for (int i = 0; i < h->cfg.n_enc; ++i) hop *= h->cfg.enc_strides[i];
-    else if (h->cfg.model_type == ADEC_MODEL_SYMAD_DECODER) for (int i = 0; i < h->cfg.n_dec; ++i) hop *= h->cfg.dec_strides[i];
+    const int mt = h->cfg.model_type;
+    if (mt == ADEC_MODEL_SYMAD || mt == ADEC_MODEL_SYMAD_ENCODER) for (int i = 0; i < h->cfg.n_enc; ++i) hop *= h->cfg.enc_strides[i];
+    else if (mt == ADEC_MODEL_SYMAD_DECODER) for (int i = 0; i < h->cfg.n_dec; ++i) hop *= h->cfg.dec_strides[i];
     else for (int i = 0; i < h->cfg.n_up; ++i) hop *= h->cfg.upsample_scales[i];
     return hop;
 }
 
-// The entry points that need the encoder, projector or RVQ: a full symAD handle only
-int need_full_symad(adec_handle* h, const std::string& what) {
-    if (h->cfg.model_type == ADEC_MODEL_SYMAD) return 0;
+int fail_encoder_only(adec_handle* h, const std::string& what) {
+    return h->fail(what + ": a symAD encoder-only handle (ADEC_MODEL_SYMAD_ENCODER) has no decoder, lookup or unpack; use a full symAD "
+                          "handle (ADEC_MODEL_SYMAD) or a decoder handle");
+}
+
+// The entry points that need the encoder, projector or the RVQ's nearest-codeword search (encode, quantize, pack): a full symAD handle
+// or an encoder-only one
+int need_symad_tx(adec_handle* h, const std::string& what) {
+    if (h->cfg.model_type == ADEC_MODEL_SYMAD || h->cfg.model_type == ADEC_MODEL_SYMAD_ENCODER) return 0;
     if (h->cfg.model_type == ADEC_MODEL_SYMAD_DECODER)
         return h->fail(what + ": a symAD decoder-only handle (ADEC_MODEL_SYMAD_DECODER) has no encoder, projector or RVQ; use a full symAD "
                               "handle (ADEC_MODEL_SYMAD)");
     return h->fail(what + ": not a symAD handle");
+}
+
+// The entry points of a full symAD handle only: lookup, unpack, the RVQ's forward sum and its moments
+int need_full_symad(adec_handle* h, const std::string& what) {
+    if (h->cfg.model_type == ADEC_MODEL_SYMAD_ENCODER) return fail_encoder_only(h, what);
+    return need_symad_tx(h, what);
 }
 
 // The state map from the ops' keys, and the 32 x 32 (channel, row) tiles the export / import kernels run over
@@ -1406,16 +1438,19 @@ int adec_create(const adec_config* cfg, int device, adec_handle** out) {
         delete h;
         return 1;
     }
-    if (h->bf16 && ((cfg->model_type != ADEC_MODEL_HIFIGAN && cfg->model_type != ADEC_MODEL_SYMAD_DECODER) || h->engine != 2)) {
+    const bool enc_only = cfg->model_type == ADEC_MODEL_SYMAD_ENCODER;
+    if (h->bf16 && ((cfg->model_type != ADEC_MODEL_HIFIGAN && cfg->model_type != ADEC_MODEL_SYMAD_DECODER && !enc_only) || h->engine != 2)) {
         g_create_error = "compute_dtype = bf16 is built for the decoder handles - the HiFi-GAN vocoder and the symAD decoder-only handle "
-                         "(ADEC_MODEL_SYMAD_DECODER) - on the f16 tensor-core engine only (the encoder, projector and RVQ of a full symAD "
-                         "handle must stay fp32-grade for bit-identical indices)";
+                         "(ADEC_MODEL_SYMAD_DECODER) - and for the symAD encoder-only handle (ADEC_MODEL_SYMAD_ENCODER), on the f16 "
+                         "tensor-core engine only (the encoder, projector and RVQ of a full symAD handle must stay fp32-grade for "
+                         "bit-identical indices)";
         delete h;
         return 1;
     }
-    const int zq_dim = cfg->model_type == ADEC_MODEL_SYMAD_DECODER ? cfg->code_dim : cfg->in_channels;
+    const bool symad_part = cfg->model_type == ADEC_MODEL_SYMAD_DECODER || enc_only;
+    const int zq_dim = symad_part ? cfg->code_dim : cfg->in_channels;
     if (h->act_bf16 && zq_dim % 8) {      // a bf16 zq row must be whole 16-byte vectors
-        g_create_error = cfg->model_type == ADEC_MODEL_SYMAD_DECODER ? "compute_dtype = 2 needs code_dim to be a multiple of 8"
+        g_create_error = symad_part ? "compute_dtype = 2 needs code_dim to be a multiple of 8"
                                                                      : "compute_dtype = 2 needs in_channels to be a multiple of 8";
         delete h;
         return 1;
@@ -1465,6 +1500,7 @@ int adec_finalize(adec_handle* h) {
     int rc = h->cfg.model_type == ADEC_MODEL_SYMAD ? build_symad(h)
            : h->cfg.model_type == ADEC_MODEL_HIFIGAN ? build_hifigan(h)
            : h->cfg.model_type == ADEC_MODEL_SYMAD_DECODER ? build_symad_decoder_only(h)
+           : h->cfg.model_type == ADEC_MODEL_SYMAD_ENCODER ? build_symad_encoder_only(h)
            : h->fail("unknown model_type");
     if (rc) return rc;
     for (const auto& kv : h->tensors)   // load_state_dict(strict=True): unexpected keys are an error
@@ -1552,7 +1588,9 @@ int adec_reset(adec_handle* h, void* stream) {
 }
 
 int adec_frames_for(const adec_handle* h, int T) {
-    if (!h || (h->cfg.model_type != ADEC_MODEL_SYMAD && h->cfg.model_type != ADEC_MODEL_SYMAD_DECODER)) return -1;
+    if (!h || (h->cfg.model_type != ADEC_MODEL_SYMAD && h->cfg.model_type != ADEC_MODEL_SYMAD_DECODER &&
+               h->cfg.model_type != ADEC_MODEL_SYMAD_ENCODER))
+        return -1;
     int t = T;
     for (int i = 0; i < h->cfg.n_enc; ++i) t = (t - 1) / h->cfg.enc_strides[i] + 1;
     return t;
@@ -1598,14 +1636,17 @@ static int run_call(adec_handle* h, const Call& c, const void* in, int B, int T,
     static const char* const kModeName[] = {"", "_offline", "_offline_varlen", "_streams"};
     const std::string base = std::string(c.decode ? "decode" : "encode") + kModeName[c.mode];
     const std::string name = base + (c.bf16_io ? "_bf16" : "");
-    if (!c.decode && need_full_symad(h, name)) return 1;
+    if (!c.decode && need_symad_tx(h, name)) return 1;
+    if (c.decode && h->cfg.model_type == ADEC_MODEL_SYMAD_ENCODER) return fail_encoder_only(h, name);
+    const char* io = c.decode ? "zq / y" : "x / z";
     if (h->act_bf16 && !c.bf16_io)
-        return h->fail(fmt("%s: this handle has bf16 activations (compute_dtype 2); call adec_%s_bf16 with bf16 zq / y", name.c_str(),
-                           base.c_str()));
+        return h->fail(fmt("%s: this handle has bf16 activations (compute_dtype 2); call adec_%s_bf16 with bf16 %s", name.c_str(),
+                           base.c_str(), io));
     if (!h->act_bf16 && c.bf16_io)
-        return h->fail(fmt("%s: this handle has fp32 activations (compute_dtype %d); call adec_%s with fp32 zq / y", name.c_str(),
-                           h->cfg.compute_dtype, base.c_str()));
-    if (c.bf16_io && (((uintptr_t)in | (uintptr_t)out) & 15)) return h->fail(name + ": zq and y must be 16-byte aligned");
+        return h->fail(fmt("%s: this handle has fp32 activations (compute_dtype %d); call adec_%s with fp32 %s", name.c_str(),
+                           h->cfg.compute_dtype, base.c_str(), io));
+    if (c.bf16_io && (((uintptr_t)in | (uintptr_t)out) & 15))
+        return h->fail(name + (c.decode ? ": zq and y must be 16-byte aligned" : ": x and z must be 16-byte aligned"));
     RunCtx rc{B, (const float*)in, (float*)out, (cudaStream_t)stream, c.mode, c.lengths, c.slots, name.c_str()};
     if (rc.varlen()) {
         if (varlen_args(h, rc.what, c.lengths, B)) return 1;
@@ -1665,6 +1706,22 @@ int adec_encode_offline_varlen(adec_handle* h, const float* x, const int* length
 // The varlen row space with each utterance's history read from, and its new state written to, its stream's slot (ConvArgs::vl_slot).
 int adec_encode_streams(adec_handle* h, const float* x, const int* lengths, const int* streams, int B, float* z, void* stream) {
     return run_call(h, {false, CALL_SLOTS, false, lengths, streams}, x, B, 0, z, stream);
+}
+
+int adec_encode_bf16(adec_handle* h, const uint16_t* x, int B, int T, uint16_t* z, void* stream) {
+    return run_call(h, {false, CALL_STREAM, true}, x, B, T, z, stream);
+}
+
+int adec_encode_offline_bf16(adec_handle* h, const uint16_t* x, int B, int T, uint16_t* z, void* stream) {
+    return run_call(h, {false, CALL_OFFLINE, true}, x, B, T, z, stream);
+}
+
+int adec_encode_offline_varlen_bf16(adec_handle* h, const uint16_t* x, const int* lengths, int B, uint16_t* z, void* stream) {
+    return run_call(h, {false, CALL_VARLEN, true, lengths}, x, B, 0, z, stream);
+}
+
+int adec_encode_streams_bf16(adec_handle* h, const uint16_t* x, const int* lengths, const int* streams, int B, uint16_t* z, void* stream) {
+    return run_call(h, {false, CALL_SLOTS, true, lengths, streams}, x, B, 0, z, stream);
 }
 
 int adec_decode(adec_handle* h, const float* zq, int B, int F, float* y, void* stream) {
@@ -1804,15 +1861,15 @@ int adec_set_stream_state(adec_handle* h, const int* streams, int n, const void*
 static int index_bits(int n) { int b = 1; while ((1 << b) < n) ++b; return b; }
 
 int adec_packed_frame_bytes(const adec_handle* h) {
-    if (!h || h->cfg.model_type != ADEC_MODEL_SYMAD) return -1;
+    if (!h || (h->cfg.model_type != ADEC_MODEL_SYMAD && h->cfg.model_type != ADEC_MODEL_SYMAD_ENCODER)) return -1;
     return (h->cfg.codebook_num * index_bits(h->cfg.codebook_size) + 7) / 8;
 }
 
 // residual VQ launch: pick frames-per-pass FP and passes per block so that the grid is ONE wave with the smallest idle tail
-extern "C++" template <int FP, bool FWD>
+extern "C++" template <int FP, bool FWD, bool ZB>
 cudaError_t launch_rvq(const adec_handle* h, RvqArgs a, cudaStream_t s, int* cost) {
     static int per_sm[64] = {0};
-    auto kern = rvq_kernel<64, 4, FP, FWD>;
+    auto kern = rvq_kernel<64, 4, FP, FWD, ZB>;
     const int dev = h->device;
     const auto smem_of = [&](int n_pass) { const int FR = n_pass * FP; return (size_t)FR * (3 * 64 + 1 + 2 * (RVQ_THREADS / 32) + a.nq) * 4; };
     if (dev < 64 && !per_sm[dev]) {
@@ -1831,39 +1888,58 @@ cudaError_t launch_rvq(const adec_handle* h, RvqArgs a, cudaStream_t s, int* cos
     return cudaGetLastError();
 }
 
-extern "C++" template <bool FWD>
+extern "C++" template <bool FWD, bool ZB = false>
 cudaError_t launch_rvq_best(const adec_handle* h, const RvqArgs& a, cudaStream_t s) {
     int c16 = 0, c12 = 0, c8 = 0;
-    launch_rvq<16, FWD>(h, a, nullptr, &c16); launch_rvq<12, FWD>(h, a, nullptr, &c12); launch_rvq<8, FWD>(h, a, nullptr, &c8);
-    return (c12 <= c16 && c12 <= c8) ? launch_rvq<12, FWD>(h, a, s, nullptr)
-         : (c16 <= c8)               ? launch_rvq<16, FWD>(h, a, s, nullptr)
-                                     : launch_rvq<8, FWD>(h, a, s, nullptr);
+    launch_rvq<16, FWD, ZB>(h, a, nullptr, &c16); launch_rvq<12, FWD, ZB>(h, a, nullptr, &c12); launch_rvq<8, FWD, ZB>(h, a, nullptr, &c8);
+    return (c12 <= c16 && c12 <= c8) ? launch_rvq<12, FWD, ZB>(h, a, s, nullptr)
+         : (c16 <= c8)               ? launch_rvq<16, FWD, ZB>(h, a, s, nullptr)
+                                     : launch_rvq<8, FWD, ZB>(h, a, s, nullptr);
 }
 
-// fwd: zq receives ResidualVQ.forward's sum instead of lookup's (rvq_kernel's FWD)
-static int quantize_common(adec_handle* h, const float* z, int B, int F, int64_t* idx, uint8_t* packed, float* zq, bool fwd,
+// fwd: zq receives ResidualVQ.forward's sum instead of lookup's (rvq_kernel's FWD).  zb: z is bf16 (rvq_kernel's ZB), which a handle
+// with bf16 activations takes and every other handle refuses
+static int quantize_common(adec_handle* h, const void* z, int B, int F, int64_t* idx, uint8_t* packed, float* zq, bool fwd, bool zb,
                            void* stream) {
     if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    if (need_full_symad(h, "quantize")) return 1;
+    if (need_symad_tx(h, "quantize")) return 1;
+    if (h->act_bf16 && !zb)
+        return h->fail("quantize: this handle has bf16 activations (compute_dtype 2); call adec_quantize_bf16 / adec_quantize_ex_bf16 with bf16 z");
+    if (!h->act_bf16 && zb)
+        return h->fail(fmt("quantize_bf16: this handle has fp32 activations (compute_dtype %d); call adec_quantize / adec_quantize_ex with "
+                           "fp32 z", h->cfg.compute_dtype));
+    if (zb && (uintptr_t)z % 16) return h->fail("quantize_bf16: z must be 16-byte aligned");
+    // an encoder-only handle quantizes to indices and packed bytes; zq (the lookup) and the forward sum are the full handle's
+    if (zq && h->cfg.model_type == ADEC_MODEL_SYMAD_ENCODER) return fail_encoder_only(h, fwd ? "quantize_forward" : "quantize_ex (zq)");
     if (B < 1 || F < 1) return h->fail("quantize: empty input");
     if (!idx && !packed && !zq) return h->fail("quantize: no output requested");
     DeviceGuard dg(h->device);
     RvqArgs a{};
-    a.z = z; a.B = B; a.F = F; a.nq = h->cfg.codebook_num; a.embed = h->d_embed; a.e2 = h->d_e2; a.idx = (long long*)idx;
+    a.z = (const float*)z; a.B = B; a.F = F; a.nq = h->cfg.codebook_num; a.embed = h->d_embed; a.e2 = h->d_e2; a.idx = (long long*)idx;
     a.packed = packed; a.zq = zq; a.bits = index_bits(h->cfg.codebook_size); a.bpf = adec_packed_frame_bytes(h);
-    const cudaError_t e = fwd ? launch_rvq_best<true>(h, a, (cudaStream_t)stream) : launch_rvq_best<false>(h, a, (cudaStream_t)stream);
+    const cudaError_t e = fwd ? launch_rvq_best<true>(h, a, (cudaStream_t)stream)
+                        : zb  ? launch_rvq_best<false, true>(h, a, (cudaStream_t)stream)
+                              : launch_rvq_best<false>(h, a, (cudaStream_t)stream);
     if (e != cudaSuccess) return h->fail(fmt("launch of rvq_kernel failed: %s", cudaGetErrorString(e)));
     ++h->launches;
     return 0;
 }
 
 int adec_quantize_ex(adec_handle* h, const float* z, int B, int F, int64_t* idx, uint8_t* packed, float* zq, void* stream) {
-    return quantize_common(h, z, B, F, idx, packed, zq, false, stream);
+    return quantize_common(h, z, B, F, idx, packed, zq, false, false, stream);
+}
+
+int adec_quantize_ex_bf16(adec_handle* h, const uint16_t* z, int B, int F, int64_t* idx, uint8_t* packed, float* zq, void* stream) {
+    return quantize_common(h, z, B, F, idx, packed, zq, false, true, stream);
+}
+
+int adec_quantize_bf16(adec_handle* h, const uint16_t* z, int B, int F, int64_t* idx, void* stream) {
+    return quantize_common(h, z, B, F, idx, nullptr, nullptr, false, true, stream);
 }
 
 int adec_quantize_forward(adec_handle* h, const float* z, int B, int F, int64_t* idx, float* zq_fwd, void* stream) {
     if (h && !zq_fwd) return h->fail("quantize_forward: zq_fwd is NULL");
-    return quantize_common(h, z, B, F, idx, nullptr, zq_fwd, true, stream);
+    return quantize_common(h, z, B, F, idx, nullptr, zq_fwd, true, false, stream);
 }
 
 int adec_zq_moments(adec_handle* h, const float* zq, const int* frames, int B, double* sum, double* m2, void* stream) {
@@ -1975,7 +2051,7 @@ int adec_codec_host(adec_handle* enc, adec_handle* dec, const float* x_host, int
 
 static int pack_common(adec_handle* h, const char* what, int64_t* idx, int B, int F, uint8_t* packed, void* stream, bool pack) {
     if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    if (need_full_symad(h, what)) return 1;
+    if (pack ? need_symad_tx(h, what) : need_full_symad(h, what)) return 1;
     if (B < 1 || F < 1) return h->fail(std::string(what) + ": empty input");
     if (h->cfg.codebook_size < 2 || h->cfg.codebook_size > 65536) return h->fail(std::string(what) + ": codebook_size must be in [2, 65536]");
     DeviceGuard dg(h->device);
@@ -2143,7 +2219,7 @@ struct adec_graph {
     bool wire = false;
     const void* in = nullptr;
     void* out = nullptr;
-    void* mid = nullptr;          // TX: z (B, code_dim, F) fp32; RX: zq (B, F, code_dim), bf16 when the decoder has bf16 activations
+    void* mid = nullptr;          // TX: z (B, code_dim, F); RX: zq (B, F, code_dim); bf16 when the stateful handle has bf16 activations
     cudaStream_t cs = nullptr;    // private capture stream
     // by the parity (op.cur) of the stateful op list: both captured together, each instantiated the first time it is launched
     cudaGraph_t graph[2] = {nullptr, nullptr};
@@ -2171,9 +2247,9 @@ static int list_parity(const std::vector<Op>& ops) {
 static int graph_body(adec_graph* g, cudaStream_t s) {
     adec_handle *a = g->a, *b = g->b;
     if (g->kind == ADEC_GRAPH_TX) {
-        if (run_call(a, {false, CALL_STREAM, false}, g->in, g->B, g->T, g->mid, s)) return 1;
-        return quantize_common(a, (const float*)g->mid, g->B, g->F, g->wire ? nullptr : (int64_t*)g->out,
-                               g->wire ? (uint8_t*)g->out : nullptr, nullptr, false, s);
+        if (run_call(a, {false, CALL_STREAM, a->act_bf16}, g->in, g->B, g->T, g->mid, s)) return 1;
+        return quantize_common(a, g->mid, g->B, g->F, g->wire ? nullptr : (int64_t*)g->out, g->wire ? (uint8_t*)g->out : nullptr, nullptr,
+                               false, a->act_bf16, s);
     }
     if (lookup_common(a, g->wire ? nullptr : (const int64_t*)g->in, g->wire ? (const uint8_t*)g->in : nullptr, g->B, g->F, g->mid,
                       b->act_bf16, s))
@@ -2319,7 +2395,9 @@ int adec_graph_create(int kind, adec_handle* a, adec_handle* b, int B, int T_or_
     const bool tx = kind == ADEC_GRAPH_TX;
     if (tx && b) return a->fail("graph_create: a transmitter graph takes no decoder handle");
     if (!tx && (!b || !b->finalized)) return a->fail("graph_create: a receiver graph needs a finalized decoder handle");
-    if (need_full_symad(a, tx ? "graph_create (transmitter: encode, quantize)" : "graph_create (receiver: lookup)")) return 1;
+    if (tx ? need_symad_tx(a, "graph_create (transmitter: encode, quantize)") : need_full_symad(a, "graph_create (receiver: lookup)"))
+        return 1;
+    if (!tx && b->cfg.model_type == ADEC_MODEL_SYMAD_ENCODER) return fail_encoder_only(a, "graph_create (receiver: decoder)");
     if (b && b->device != a->device)
         return a->fail(fmt("graph_create: the rx handle is on device %d, the decoder on device %d", a->device, b->device));
     if (!in || !out) return a->fail("graph_create: in and out must be device buffers");
@@ -2338,7 +2416,7 @@ int adec_graph_create(int kind, adec_handle* a, adec_handle* b, int B, int T_or_
     g->kind = kind; g->a = a; g->b = b; g->device = a->device; g->B = B; g->wire = wire != 0; g->in = in; g->out = out;
     g->T = tx ? T_or_F : 0;
     g->F = tx ? adec_frames_for(a, T_or_F) : T_or_F;
-    const size_t mid_bytes = (size_t)B * g->F * a->cfg.code_dim * (!tx && b->act_bf16 ? 2 : 4);
+    const size_t mid_bytes = (size_t)B * g->F * a->cfg.code_dim * ((tx ? a : b)->act_bf16 ? 2 : 4);
     cudaError_t e = cudaStreamCreateWithFlags(&g->cs, cudaStreamNonBlocking);
     if (e == cudaSuccess) e = cudaMalloc(&g->mid, mid_bytes);
     if (e != cudaSuccess) {
@@ -2713,8 +2791,7 @@ int adec_test_conv_op(int device, const adec_test_op* d, int mode, int n_calls, 
         rc = make_convtr_op(h, &ops[0], "test_convtr", tensor({d->Cin, d->Cout, 2 * d->stride}, d->w), d->bias ? &Bt : nullptr, d->stride,
                             d->pre_act, d->slope);
         break;
-    case ADEC_TEST_STEM:     // through the state dict, as build_symad builds encoder.conv
-        if (h->bf16) { rc = h->fail("test_conv_op: the stem is fp32-grade only (compute_dtype 0)"); break; }
+    case ADEC_TEST_STEM:     // through the state dict, as build_symad builds encoder.conv: fp32 weights in every compute_dtype
         h->tensors["test.conv.weight"] = tensor({32, 1, 7}, d->w);
         if (d->bias) h->tensors["test.conv.bias"] = tensor({32}, d->bias);
         rc = build_stem(h, &ops[0], "test", 32);

@@ -503,20 +503,29 @@ struct StemArgs {
 };
 
 // VL: one row space of concatenated utterances, each with a zero left pad and no state written; with vl_slot, each with its slot's
-// history, and the slot's new state written by the block that holds the utterance's last row
-template <int COUT, int K, bool VL = false>
+// history, and the slot's new state written by the block that holds the utterance's last row.
+// BST: bf16 x, state and output (the encoder-only handle's compute_dtype 2); weights, bias and the FMA chain stay fp32, each output
+// is rounded once to nearest even, and the state holds the input samples as they are.
+template <int COUT, int K, bool VL = false, bool BST = false>
 __global__ void __launch_bounds__(256) stem_kernel(const StemArgs a) {
+    using XT = typename std::conditional<BST, __nv_bfloat16, float>::type;
     constexpr int TT = 1024, P = K - 1, Q = COUT / 4;
     __shared__ float xw[TT + P];
     __shared__ __align__(16) float sw[K * COUT];
     __shared__ __align__(16) float sb[COUT];
     const int b = blockIdx.y, j0 = blockIdx.x * TT, tid = threadIdx.x;
-    const float* xg = a.x + (long long)b * a.x_bs;
+    const XT* xg = reinterpret_cast<const XT*>(a.x) + (long long)b * a.x_bs;
+    const XT* st_in = reinterpret_cast<const XT*>(a.st_in);
+    XT* st_out = reinterpret_cast<XT*>(a.st_out);
+    auto widen = [](XT v) -> float {
+        if constexpr (BST) return __bfloat162float(v);
+        else return v;
+    };
     for (int i = tid; i < TT + P; i += 256) {
         const long long r = (long long)j0 + i;       // x~ row
         float v = 0.f;
-        if (r < P) { if (!VL) v = a.st_in[b * P + r]; }
-        else if (r - P < a.T) v = __ldg(xg + r - P);
+        if (r < P) { if (!VL) v = widen(st_in[b * P + r]); }
+        else if (r - P < a.T) v = widen(__ldg(xg + r - P));
         xw[i] = v;
     }
     for (int i = tid; i < K * COUT; i += 256) sw[i] = a.w[i];
@@ -542,20 +551,21 @@ __global__ void __launch_bounds__(256) stem_kernel(const StemArgs a) {
         };
         if (VL && a.vl_slot && j0 + t - u_start < P) {
             // the first P rows of a stream-slot utterance: taps before it read the slot's history
-            const float* hs = slot_rows(a.vl_slot, u, a.st_in, a.st_out, P, true);
-            for (int k = 0; k < K; ++k) tap(k, j0 + t + k - P < u_start ? __ldg(hs + (j0 + t + k - u_start)) : xw[t + k]);
+            const XT* hs = slot_rows(a.vl_slot, u, st_in, st_out, P, true);
+            for (int k = 0; k < K; ++k) tap(k, j0 + t + k - P < u_start ? widen(__ldg(hs + (j0 + t + k - u_start))) : xw[t + k]);
         } else {
 #pragma unroll
             for (int k = 0; k < K; ++k) tap(k, (!VL || j0 + t + k - P >= u_start) ? xw[t + k] : 0.f);   // taps before the utterance: its zero pad
         }
         const float4 b4 = *reinterpret_cast<const float4*>(sb + q * 4);
         acc.x += b4.x; acc.y += b4.y; acc.z += b4.z; acc.w += b4.w;
-        *reinterpret_cast<float4*>(yg + (long long)(j0 + t) * COUT + q * 4) = acc;
+        if constexpr (BST) st4(reinterpret_cast<__nv_bfloat16*>(a.y) + (long long)b * a.y_bs + (long long)(j0 + t) * COUT + q * 4, acc);
+        else *reinterpret_cast<float4*>(yg + (long long)(j0 + t) * COUT + q * 4) = acc;
     }
     if (!VL && blockIdx.x == gridDim.x - 1) {
         for (int r = tid; r < P; r += 256) {
             const long long i = (long long)a.T + r;
-            a.st_out[b * P + r] = (i < P) ? a.st_in[b * P + i] : xg[i - P];
+            st_out[b * P + r] = (i < P) ? st_in[b * P + i] : xg[i - P];
         }
     }
     if (VL && a.vl_slot) {
@@ -567,8 +577,8 @@ __global__ void __launch_bounds__(256) stem_kernel(const StemArgs a) {
             const int s0 = __ldg(a.vl_off + u), s1 = __ldg(a.vl_off + u + 1);
             if (s1 - 1 < j0 || s1 - 1 >= j0 + TT) continue;
             const int i = s1 - s0 + r;
-            const float v = i < P ? __ldg(slot_rows(a.vl_slot, u, a.st_in, a.st_out, P, true) + i) : __ldg(xg + s0 + i - P);
-            slot_rows(a.vl_slot, u, a.st_in, a.st_out, P, false)[r] = v;
+            const XT v = i < P ? __ldg(slot_rows(a.vl_slot, u, st_in, st_out, P, true) + i) : __ldg(xg + s0 + i - P);
+            slot_rows(a.vl_slot, u, st_in, st_out, P, false)[r] = v;
         }
     }
 }
@@ -711,7 +721,9 @@ constexpr int RVQ_THREADS = 256;
 // tail (adec_quantize), which alone took the 64 x 160-frame case from 0.58 ms (320 blocks of 32 frames = 1.08 waves) to one wave.
 // FWD: zq accumulates ResidualVQ.forward's quantized_out, the sum of r + (e - r) from 0. (vq_module.py:136-143), instead of
 // lookup's sum of the codewords; shared memory, grid and every other output are the same.
-template <int D, int NPT, int FP, bool FWD>   // codebook size N = RVQ_THREADS * NPT
+// ZB: z is bf16 (raw words, the encoder-only handle's compute_dtype 2), widened exactly to fp32 on load; the arithmetic after the
+// load is the fp32 instantiation's, so the outputs are the spec applied to float(z).
+template <int D, int NPT, int FP, bool FWD, bool ZB = false>   // codebook size N = RVQ_THREADS * NPT
 __global__ void __launch_bounds__(RVQ_THREADS) rvq_kernel(const RvqArgs a) {
     constexpr int N = RVQ_THREADS * NPT, NW = RVQ_THREADS / 32;
     static_assert(D % 32 == 0 && FP % 4 == 0, "D must be a multiple of 32, FP of 4");
@@ -734,7 +746,8 @@ __global__ void __launch_bounds__(RVQ_THREADS) rvq_kernel(const RvqArgs a) {
         float v = 0.f;
         if (fr < nfr) {
             const long long bb = fr / a.F, ff = fr - bb * a.F;
-            v = a.z[(bb * D + k) * a.F + ff];        // quantizer.py:43 z.transpose(2,1)
+            if constexpr (ZB) v = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(a.z)[(bb * D + k) * a.F + ff]);
+            else v = a.z[(bb * D + k) * a.F + ff];  // quantizer.py:43 z.transpose(2,1)
         }
         r[f * D + k] = v;
         r2[f * D + k] = 2.0f * v;

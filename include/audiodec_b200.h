@@ -40,12 +40,24 @@ typedef struct adec_handle adec_handle;
 enum adec_model_type {
     ADEC_MODEL_SYMAD = 0,      /* models/autoencoder/AudioDec.py:166 StreamGenerator (codec='audiodec') */
     ADEC_MODEL_HIFIGAN = 1,    /* models/vocoder/HiFiGAN.py:222 StreamGenerator, MultiGroupConv1d fusion (AD v1) */
-    ADEC_MODEL_SYMAD_DECODER = 2   /* the decoder of a symAD StreamGenerator alone: what the receiver's `decoder` object runs
+    ADEC_MODEL_SYMAD_DECODER = 2,  /* the decoder of a symAD StreamGenerator alone: what the receiver's `decoder` object runs
                                       (initial_decoder / decode, utils/audiodec.py:104-106).  Same config as ADEC_MODEL_SYMAD; loads a
                                       full generator state dict (decoder.* strict, encoder.* / projector.* / quantizer.* ignored).  The
                                       decode entry points, the state calls, adec_hop_length / adec_frames_for and the diagnostics work on
                                       it; encode, quantize*, lookup*, pack / unpack and adec_zq_moments fail.  compute_dtype 1 and 2 on
                                       the f16 engine, as for HiFi-GAN. */
+    ADEC_MODEL_SYMAD_ENCODER = 3   /* the transmitter of a symAD StreamGenerator alone: encoder, projector and RVQ search, what the
+                                      transmitter's `tx_encoder` object runs (initial_encoder / encode / quantize, utils/audiodec.py:
+                                      100-102).  Same config as ADEC_MODEL_SYMAD; loads a full generator state dict (encoder.* /
+                                      projector.* / quantizer.* strict, decoder.* ignored).  adec_encode*, adec_quantize,
+                                      adec_quantize_ex (idx / packed; zq must be NULL), adec_pack_indices, the state calls,
+                                      adec_frames_for / adec_hop_length / adec_packed_frame_bytes, ADEC_GRAPH_TX and the diagnostics work
+                                      on it; decode*, lookup*, unpack, adec_quantize_forward, adec_zq_moments and serving as `enc` of
+                                      adec_codec_host fail.  compute_dtype 0 encodes and quantizes bit for bit as a full symAD handle;
+                                      compute_dtype 1 (f16 engine) runs the encoder's convs on bf16 operands with fp32 activations,
+                                      state, x and z, and the RVQ on that fp32 z unchanged; compute_dtype 2 also keeps x, every
+                                      activation, the causal state and z in bf16 (adec_encode*_bf16, adec_quantize*_bf16).  The stem
+                                      keeps fp32 weights in both. */
 };
 
 /* POD mirror of config.yml `generator_params` (exp/.../config.yml:102-134 resp. :102-130). */
@@ -72,10 +84,14 @@ typedef struct adec_config {
     /* appended in round 2 */
     int compute_dtype;                                     /* 0 = fp32-grade (default); 1 = bf16 conv operands with fp32 accumulation, HiFi-GAN vocoder
                                                               and symAD decoder-only handles: what `decoder.to(torch.bfloat16)` asks of the
-                                                              reference (BASELINE configs[2]);
+                                                              reference (BASELINE configs[2]); symAD encoder-only handles: the
+                                                              encoder's and projector's convs on bf16 operands (the stem keeps fp32
+                                                              weights; fp32 x, activations, state and z);
                                                               2 = as 1, and every activation, the causal state and the decode input / output are
                                                               bf16 in memory (the reference's bf16 data layout and dtype contract): decode with
-                                                              adec_decode_bf16 / adec_decode_offline_bf16.  1 and 2 need the f16 engine. */
+                                                              adec_decode_bf16 / adec_decode_offline_bf16 (decoder handles), resp. encode and
+                                                              quantize with adec_encode*_bf16 / adec_quantize*_bf16 (encoder-only handle).  1 and
+                                                              2 need the f16 engine. */
 } adec_config;
 
 /* -- lifetime ---------------------------------------------------------------- */
@@ -133,6 +149,18 @@ int adec_decode(adec_handle *h, const float *zq, int B, int F, float *y, void *s
  * bf16 (raw 16-bit words), both
  * 16-byte aligned.  adec_decode on such a handle fails, and so does adec_decode_bf16 on any other handle. */
 int adec_decode_bf16(adec_handle *h, const uint16_t *zq, int B, int F, uint16_t *y, void *stream);
+
+/* The encode family and quantize for a symAD encoder-only handle with compute_dtype 2: x (B,1,T) and z (B,code_dim,F) are bf16 (raw
+ * 16-bit words), 16-byte aligned; the stem reads bf16 x, every activation and the causal state are bf16, the projector stores bf16 z.
+ * adec_quantize_bf16 / adec_quantize_ex_bf16 widen bf16 z exactly and then run the fp32 RVQ unchanged, so the indices and packed bytes
+ * are the spec applied to float(z) (zq must be NULL on an encoder-only handle).  The fp32 entry points fail on such a handle, and these
+ * fail on every other handle.  Varlen / slot layouts as adec_encode_offline_varlen / adec_encode_streams. */
+int adec_encode_bf16(adec_handle *h, const uint16_t *x, int B, int T, uint16_t *z, void *stream);
+int adec_encode_offline_bf16(adec_handle *h, const uint16_t *x, int B, int T, uint16_t *z, void *stream);
+int adec_encode_offline_varlen_bf16(adec_handle *h, const uint16_t *x, const int *lengths, int B, uint16_t *z, void *stream);
+int adec_encode_streams_bf16(adec_handle *h, const uint16_t *x, const int *lengths, const int *streams, int B, uint16_t *z, void *stream);
+int adec_quantize_bf16(adec_handle *h, const uint16_t *z, int B, int F, int64_t *idx, void *stream);
+int adec_quantize_ex_bf16(adec_handle *h, const uint16_t *z, int B, int F, int64_t *idx, uint8_t *packed, float *zq, void *stream);
 
 /* -- the non-streaming batch forward (SURVEY.md 8(f) rank 4; codecTest.py:78-95, codecStatistic.py:92-98) ---------- */
 /* Encoder.forward + Projector.forward (models/autoencoder/modules/encoder.py:131, projector.py:49-50): every causal
@@ -212,7 +240,7 @@ int adec_codec_host(adec_handle *enc, adec_handle *dec, const float *x_host, int
  * (bin/stream.py:224).  Packed frame = Nq local indices (idx - i*codebook_size) of ceil(log2 codebook_size) bits each,
  * stage 0 first, little-endian bit order, zero-padded to whole bytes: 8 x 10 bit = 10 bytes / frame = 12.8 kbit/s at
  * hop 300 / 48 kHz.  idx (Nq,B,F) int64 flat <-> packed (B,F,adec_packed_frame_bytes) uint8, device pointers. */
-int adec_packed_frame_bytes(const adec_handle *h);       /* -1 if h is not a full symAD handle (ADEC_MODEL_SYMAD) */
+int adec_packed_frame_bytes(const adec_handle *h);       /* -1 if h is not a full or encoder-only symAD handle */
 int adec_pack_indices(adec_handle *h, const int64_t *idx, int B, int F, uint8_t *packed, void *stream);
 int adec_unpack_indices(adec_handle *h, const uint8_t *packed, int B, int F, int64_t *idx, void *stream);
 /* lookup straight from the packed bitstream (unpack fused into lookup): packed (B,F,bytes) -> zq (B,F,code_dim) */
@@ -234,8 +262,8 @@ int adec_lookup_packed_bf16(adec_handle *h, const uint8_t *packed, int B, int F,
 int64_t adec_launch_count(const adec_handle *h);
 
 /* -- graphed stream steps: one CUDA graph launch for the launches of a transmitter or receiver step ------------------------------
- * ADEC_GRAPH_TX (a = full symAD tx handle, b = NULL, T_or_F = samples per chunk):
- *   in x (B, 1, T) fp32 -> adec_encode -> adec_quantize_ex -> out idx (Nq, B, F) int64, or with `wire` packed (B, F, bytes) uint8.
+ * ADEC_GRAPH_TX (a = full or encoder-only symAD tx handle, b = NULL, T_or_F = samples per chunk):
+ *   in x (B, 1, T) fp32 (bf16 when a has bf16 activations) -> adec_encode -> adec_quantize_ex -> out idx (Nq, B, F) int64, or with `wire` packed (B, F, bytes) uint8.
  * ADEC_GRAPH_RX (a = full symAD rx handle, b = any decoder handle, may equal a; T_or_F = frames per chunk):
  *   in idx (Nq, B, F) int64, or with `wire` packed (B, F, bytes) -> adec_lookup[_packed] -> adec_decode -> out y (B, F * hop), fp32, or
  *   bf16 when b has bf16 activations (compute_dtype 2; the lookup then writes bf16 zq itself, adec_lookup_bf16).
@@ -328,7 +356,7 @@ typedef struct adec_test_op {
     int post_tanh;     /* head: tanh after the conv                                                                             */
     const float *w, *w2, *bias, *mean, *scale;   /* bias, mean, scale may be NULL                                             */
     int compute_dtype; /* 0: the fp32-grade engine ADEC_CONV_PATH names; 1 / 2: the op as a symAD decoder-only handle with that
-                        * compute_dtype builds it (f16 engine; no stem, no strided conv): x, res, state and y are fp32 for 0 and 1 and
+                        * compute_dtype builds it (f16 engine; the stem keeps fp32 weights): x, res, state and y are fp32 for 0 and 1 and
                         * bf16 words for 2                                                                                          */
 } adec_test_op;
 /* launch records: 9 ints {launch kind, NT (FFMA: output tile), fuse, pre_act, prec (wg_conv.cuh PREC_*), varlen, paired, stacked,
