@@ -17,6 +17,10 @@ runs is fed silence (counted as an ``underrun``); a stream whose backlog exceeds
 dropped (counted in ``frame_drops``), which is the reference's flush-when-late policy (bin/stream.py:262-270) applied
 per stream.  The codec objects are duck-typed exactly like the reference's (``encode / quantize / lookup / decode``), so
 the class also runs on stand-ins in the CPU tests.
+
+SessionCodecServer advances only the open sessions that have audio, through stream slots.  TransmitterSessionServer and
+ReceiverSessionServer split it at the wire: the first turns sessions' PCM into packets of packed code frames (audiodec_b200.wire), the
+second turns packets back into PCM, so the two halves can run in different processes on different machines.
 """
 from __future__ import annotations
 
@@ -30,6 +34,7 @@ import numpy as np
 import torch
 
 from .codec import ReceiverGraph, TransmitterGraph, is_library_codec
+from .wire import HEADER_BYTES, Packet, decode_packet, encode_packet
 
 
 class StreamStats:
@@ -45,6 +50,21 @@ class StreamStats:
         lat = np.asarray(self.latencies, dtype=np.float64)
         return {"n_frames": self.n_frames, "frame_drops": self.frame_drops, "underruns": self.underruns,
                 "latency_ms": (float(lat.mean() * 1e3), float(lat.std() * 1e3)) if lat.size else (float("nan"), float("nan"))}
+
+
+def _frame_in(frame, frame_size: int) -> np.ndarray:
+    f = np.asarray(frame, dtype=np.float32).reshape(-1)
+    if f.shape[0] != frame_size:
+        raise ValueError(f"frame has {f.shape[0]} samples, server frame_size is {frame_size}")
+    return f
+
+
+def _queue_frame(q: Deque, item, max_backlog: int, stats: StreamStats) -> None:
+    """Append (frame, capture stamp) to a stream's input queue; a stream running late loses its OLDEST frames (bin/stream.py:262-270)."""
+    q.append(item)
+    while len(q) > max_backlog:
+        q.popleft()
+        stats.frame_drops += 1
 
 
 class MultiStreamCodecServer:
@@ -84,15 +104,9 @@ class MultiStreamCodecServer:
     # ------------------------------------------------------------------ producer / consumer side (audio callbacks)
     def submit(self, stream: int, frame, t_capture: Optional[float] = None) -> None:
         """Queue one (frame_size,) float32 frame of stream `stream`.  Late streams lose their OLDEST queued frames."""
-        f = np.asarray(frame, dtype=np.float32).reshape(-1)
-        if f.shape[0] != self.frame_size:
-            raise ValueError(f"frame has {f.shape[0]} samples, server frame_size is {self.frame_size}")
+        f = _frame_in(frame, self.frame_size)
         with self._lock:
-            q = self._in[stream]
-            q.append((f, self._clock() if t_capture is None else t_capture))
-            while len(q) > self.max_backlog:
-                q.popleft()
-                self.stats[stream].frame_drops += 1
+            _queue_frame(self._in[stream], (f, self._clock() if t_capture is None else t_capture), self.max_backlog, self.stats[stream])
 
     def poll(self, stream: int) -> Optional[np.ndarray]:
         """Next decoded (frame_size,) frame of `stream`, or None if the pipeline has nothing for it yet (the reference
@@ -259,22 +273,146 @@ class MultiStreamCodecServer:
 
 
 class SessionState:
-    """What a detached session needs to continue on another SessionCodecServer (of the same config and dtypes, on any device):
-    per stateful generator of the server its state_layout and its (1, S) device state, the queued input frames with their capture
-    stamps, and the decoded frames it has not polled yet."""
+    """What a detached session needs to continue on another server of the same kind (same config and dtypes, on any device): per
+    stateful generator of the server its state_layout and its (1, S) device state, the queued input (frames with their capture stamps
+    on SessionCodecServer and TransmitterSessionServer, held packets on ReceiverSessionServer), and the decoded frames it has not polled
+    yet.  On the split servers also the session's wire id and the next sequence number it sends or expects."""
 
-    def __init__(self, layouts, states, inputs, outputs):
+    def __init__(self, layouts, states, inputs, outputs, session_id=None, seq=0):
         self.layouts: List[list] = layouts
         self.states: List[torch.Tensor] = states
-        self.inputs: List[Tuple[np.ndarray, float]] = inputs
+        self.inputs: list = inputs
         self.outputs: List[np.ndarray] = outputs
+        self.session_id: Optional[int] = session_id
+        self.seq: int = seq
 
     def to(self, device) -> "SessionState":
         """A copy with the states on `device` (the frames are host arrays and are shared)."""
-        return SessionState(self.layouts, [t.to(device) for t in self.states], list(self.inputs), list(self.outputs))
+        return SessionState(self.layouts, [t.to(device) for t in self.states], list(self.inputs), list(self.outputs), self.session_id,
+                            self.seq)
 
 
-class SessionCodecServer(MultiStreamCodecServer):
+class _SessionSlots:
+    """The slot bookkeeping of the session servers.  Every stateful generator holds `capacity` stream slots plus one template slot (the
+    last) with the warm state that ``load_transmitter`` / ``load_receiver`` left in it; the template is never advanced.  A session is
+    opened in a free slot from the template or attached from a detached SessionState, and is known to the caller by an id: the slot
+    itself (``_open_slot()``) or an id the caller chose (``_open_slot(sid)``).  Subclasses keep their per-slot queues and counters and
+    say how to clear, export and import them (``_reset_slot`` / ``_take_slot`` / ``_restore_slot``, called with ``_lock`` held).
+
+    Locks: ``_lock`` guards the queues and the slot lists (submit / poll may come from audio callbacks while step() runs in a worker),
+    ``_codec_lock`` the generators (driven by step(), open() and attach() from different threads), ``_step_lock`` a whole step, output
+    hand-off included, so that detach() waits for it."""
+
+    _noun = "stream"
+
+    def __init__(self, capacity: int, stateful):
+        if capacity < 1:
+            raise ValueError("capacity must be >= 1")
+        self.capacity = capacity
+        self.template = capacity                      # slot index of the warm template
+        stateful = tuple(stateful)
+        self._stateful = [g for i, g in enumerate(stateful) if g not in stateful[:i]]
+        for g in self._stateful:
+            if g.n_streams != 1:                      # growing from more than one stream adds zero-history slots: a cold template
+                raise ValueError(f"{type(g).__name__} holds {g.n_streams} streams; {type(self).__name__} needs generators with the one "
+                                 "warmed stream that load_transmitter / load_receiver leave")
+        for g in self._stateful:
+            g.set_streams(capacity + 1)               # replicates the one warmed stream into every slot
+        self._free = list(range(capacity))
+        self._open: set = set()
+        self._ids: Dict[int, int] = {}                # session id -> slot
+        self._session = [0] * capacity                # per slot: bumped by every open, so a step hands out only its own session's frames
+        self._lock = threading.Lock()
+        self._codec_lock = threading.Lock()
+        self._step_lock = threading.Lock()
+
+    def _reset_slot(self, s: int) -> None:
+        raise NotImplementedError
+
+    def _take_slot(self, s: int):
+        """-> (inputs, outputs, seq) of slot s, leaving its queues empty"""
+        raise NotImplementedError
+
+    def _restore_slot(self, s: int, state: SessionState) -> None:
+        raise NotImplementedError
+
+    def _slot(self, sid) -> int:
+        s = self._ids.get(sid)
+        if s is None or s not in self._open:
+            raise KeyError(f"{self._noun} {sid} is not open")
+        return s
+
+    def _claim(self, sid):
+        """A free slot for session `sid` (None: the slot is the id) -> (sid, slot); the slot is reserved, not yet open.  _lock held."""
+        if sid is not None and sid in self._ids:
+            raise ValueError(f"{self._noun} {sid} is already open")
+        if not self._free:
+            raise RuntimeError(f"server is full: all {self.capacity} streams are open")
+        s = min(self._free)
+        self._free.remove(s)
+        self._session[s] += 1
+        sid = s if sid is None else sid
+        self._ids[sid] = s
+        return sid, s
+
+    def _open_slot(self, sid=None):
+        """Start a session in a free slot, warm as the template; returns its id."""
+        with self._lock:
+            sid, s = self._claim(sid)
+            self._reset_slot(s)
+        with self._codec_lock:
+            for g in self._stateful:
+                g.copy_stream_state(self.template, [s])
+        with self._lock:
+            self._open.add(s)
+        return sid
+
+    def _close_slot(self, sid) -> None:
+        with self._lock:
+            s = self._slot(sid)
+            self._open.remove(s)
+            del self._ids[sid]
+            self._reset_slot(s)
+            self._free.append(s)
+
+    def _detach_slot(self, sid) -> SessionState:
+        with self._step_lock:
+            with self._lock:
+                s = self._slot(sid)
+                self._open.remove(s)
+                del self._ids[sid]
+                inputs, outputs, seq = self._take_slot(s)
+            with self._codec_lock:       # the slot stays taken until its state is out
+                states = [g.stream_state([s]) for g in self._stateful]
+            layouts = [list(g.state_layout) for g in self._stateful]
+            with self._lock:
+                self._free.append(s)
+        return SessionState(layouts, states, inputs, outputs, seq=seq)
+
+    def _attach_slot(self, state: SessionState, sid=None):
+        if len(state.states) != len(self._stateful) or len(state.layouts) != len(self._stateful):
+            raise ValueError(f"the session holds the state of {len(state.states)} generators; this server has {len(self._stateful)}")
+        for g, layout in zip(self._stateful, state.layouts):
+            if [tuple(e) for e in layout] != [tuple(e) for e in g.state_layout]:
+                raise ValueError(f"the session's state layout does not match this server's {type(g).__name__}")
+        with self._lock:
+            sid, s = self._claim(sid)
+        try:
+            with self._codec_lock:
+                for g, layout, t in zip(self._stateful, state.layouts, state.states):
+                    g.load_stream_state([s], t, layout)
+        except Exception:
+            with self._lock:
+                del self._ids[sid]
+                self._free.append(s)
+            raise
+        with self._lock:
+            self._restore_slot(s, state)
+            self._open.add(s)
+        return sid
+
+
+class SessionCodecServer(_SessionSlots, MultiStreamCodecServer):
     """Duplex streams that open and close while others run, each advanced only when it has audio.
 
     The codec handles hold ``capacity`` stream slots plus one template slot (the last) with the warm state that
@@ -290,101 +428,45 @@ class SessionCodecServer(MultiStreamCodecServer):
 
     def __init__(self, tx_encoder, rx_encoder, decoder, capacity: int, frame_size: int = 1500, sample_rate: int = 48000,
                  max_latency: float = 0.1, device=None, wire: bool = False, clock=time.time):
-        super().__init__(tx_encoder, rx_encoder, decoder, capacity, frame_size=frame_size, sample_rate=sample_rate,
-                         max_latency=max_latency, device=device, wire=wire, clock=clock)
-        self.capacity = capacity
-        self.template = capacity                      # slot index of the warm template
-        self._stateful = [g for i, g in enumerate((tx_encoder, decoder)) if g not in (tx_encoder, decoder)[:i]]
-        for g in self._stateful:
-            if g.n_streams != 1:                      # growing from more than one stream adds zero-history slots: a cold template
-                raise ValueError(f"{type(g).__name__} holds {g.n_streams} streams; SessionCodecServer needs generators with the one "
-                                 "warmed stream that load_transmitter / load_receiver leave")
-        for g in self._stateful:
-            g.set_streams(capacity + 1)               # replicates the one warmed stream into every slot
-        self._free = list(range(capacity))
-        self._open: set = set()
-        self._session = [0] * capacity                # per slot: bumped by every open(), so a step hands out only its own session's frames
-        self._codec_lock = threading.Lock()           # the codec handles are driven by step() and open() from different threads
-        self._step_lock = threading.Lock()            # held for a whole step, output hand-off included: detach() waits for it
+        MultiStreamCodecServer.__init__(self, tx_encoder, rx_encoder, decoder, capacity, frame_size=frame_size, sample_rate=sample_rate,
+                                        max_latency=max_latency, device=device, wire=wire, clock=clock)
+        _SessionSlots.__init__(self, capacity, (tx_encoder, decoder))
+
+    def _reset_slot(self, s):
+        self._in[s].clear()
+        self._out[s].clear()
+
+    def _take_slot(self, s):
+        inputs, outputs = list(self._in[s]), list(self._out[s])
+        self._reset_slot(s)
+        return inputs, outputs, 0
+
+    def _restore_slot(self, s, state):
+        self._reset_slot(s)
+        self._in[s].extend(state.inputs)
+        self._out[s].extend(state.outputs)
+        self.stats[s] = StreamStats()
 
     # ------------------------------------------------------------------ sessions
     def open(self) -> int:
         """Start a stream in a free slot, warm as the template; returns its id.  Raises RuntimeError when every slot is taken."""
-        with self._lock:
-            if not self._free:
-                raise RuntimeError(f"server is full: all {self.capacity} streams are open")
-            s = min(self._free)
-            self._free.remove(s)
-            self._session[s] += 1
-            self._in[s].clear()
-            self._out[s].clear()
-        with self._codec_lock:
-            for g in self._stateful:
-                g.copy_stream_state(self.template, [s])
-        with self._lock:
-            self._open.add(s)
-        return s
+        return self._open_slot()
 
     def close(self, stream: int) -> None:
         """End stream `stream`: its slot becomes free and its queued input and output are dropped."""
-        with self._lock:
-            if stream not in self._open:
-                raise KeyError(f"stream {stream} is not open")
-            self._open.remove(stream)
-            self._in[stream].clear()
-            self._out[stream].clear()
-            self._free.append(stream)
+        self._close_slot(stream)
 
     def detach(self, stream: int) -> SessionState:
         """Close stream `stream` and return what it needs to continue elsewhere (attach(), on this or another server): its causal state
         in every stateful generator, its queued input frames and its undelivered output frames.  Waits for a step in progress to finish
         and hand off its frames, so no frame in flight is lost.  Raises KeyError if the stream is not open."""
-        with self._step_lock:
-            with self._lock:
-                if stream not in self._open:
-                    raise KeyError(f"stream {stream} is not open")
-                self._open.remove(stream)
-                inputs, outputs = list(self._in[stream]), list(self._out[stream])
-                self._in[stream].clear()
-                self._out[stream].clear()
-            with self._codec_lock:       # the slot stays taken until its state is out
-                states = [g.stream_state([stream]) for g in self._stateful]
-            layouts = [list(g.state_layout) for g in self._stateful]
-            with self._lock:
-                self._free.append(stream)
-        return SessionState(layouts, states, inputs, outputs)
+        return self._detach_slot(stream)
 
     def attach(self, state: SessionState) -> int:
         """Open a stream in a free slot from a detached session instead of the template: it continues exactly where it left off, with
         its queued and undelivered frames, and fresh per-stream counters.  The state must be on this server's device (SessionState.to).
         Raises ValueError if the session comes from codecs of another layout, RuntimeError when every slot is taken."""
-        if len(state.states) != len(self._stateful) or len(state.layouts) != len(self._stateful):
-            raise ValueError(f"the session holds the state of {len(state.states)} generators; this server has {len(self._stateful)}")
-        for g, layout in zip(self._stateful, state.layouts):
-            if [tuple(e) for e in layout] != [tuple(e) for e in g.state_layout]:
-                raise ValueError(f"the session's state layout does not match this server's {type(g).__name__}")
-        with self._lock:
-            if not self._free:
-                raise RuntimeError(f"server is full: all {self.capacity} streams are open")
-            s = min(self._free)
-            self._free.remove(s)
-            self._session[s] += 1
-        try:
-            with self._codec_lock:
-                for g, layout, t in zip(self._stateful, state.layouts, state.states):
-                    g.load_stream_state([s], t, layout)
-        except Exception:
-            with self._lock:
-                self._free.append(s)
-            raise
-        with self._lock:
-            self._in[s].clear()
-            self._in[s].extend(state.inputs)
-            self._out[s].clear()
-            self._out[s].extend(state.outputs)
-            self.stats[s] = StreamStats()
-            self._open.add(s)
-        return s
+        return self._attach_slot(state)
 
     @property
     def open_streams(self) -> List[int]:
@@ -447,3 +529,390 @@ class SessionCodecServer(MultiStreamCodecServer):
         frames = out["frames"]
         out["wire_kbps_per_stream"] = (8e-3 * self.wire_bytes) / (frames * self.frame_size / self.sample_rate) if self.wire and frames else None
         return out
+
+
+def _pinned(n: int, dtype, device) -> torch.Tensor:
+    """A 1-D host buffer of n elements, page-locked when the codec runs on a GPU (a pageable copy is staged by the driver)."""
+    return torch.empty(n, dtype=dtype, pin_memory=device.type == "cuda")
+
+
+def _ms(times: List[float]):
+    st = np.asarray(times, dtype=np.float64)
+    return (float(st.mean() * 1e3), float(st.std() * 1e3)) if st.size else (float("nan"), float("nan"))
+
+
+class TransmitterSessionServer(_SessionSlots):
+    """The sending half of SessionCodecServer: sessions of PCM frames in, one wire packet (audiodec_b200.wire) per session per step out.
+
+    tx_encoder: a SymADStreamGenerator or SymADEncoderStreamGenerator in any dtype mode, holding the one warmed stream
+    ``load_transmitter`` leaves.  Sessions are known by a u32 id the caller chooses and shares with the receiver: ``open(session_id)``
+    starts one warm from the template slot, ``close`` ends it, ``detach`` / ``attach`` move its causal state, its queued frames and its
+    next sequence number to another transmitter server.  ``submit`` queues a (frame_size,) frame with the lock-step server's drop
+    policy.  ``step()`` runs ONE ``encode_streams`` over the open sessions that have a frame queued, ONE fused quantize that writes the
+    packed bytes, and ONE device-to-host copy of only those bytes; ``poll_packets()`` returns the packets made so far as
+    (session_id, bytes), in step order and, within a step, in session id order.  Packets already made stay with the server that made
+    them when their session is detached.  Moving the bytes to the receiver is the caller's business."""
+
+    _noun = "session"
+
+    def __init__(self, tx_encoder, capacity: int, frame_size: int = 1500, sample_rate: int = 48000, max_latency: float = 0.1,
+                 device=None):
+        if frame_size < 1:
+            raise ValueError("frame_size must be >= 1")
+        self.tx_encoder = tx_encoder
+        self.frame_size, self.sample_rate, self.max_latency = frame_size, sample_rate, max_latency
+        self.device = torch.device(device) if device is not None else torch.device("cpu")
+        self.max_backlog = max(1, int(max_latency * sample_rate / frame_size))     # frames a session may have queued
+        super().__init__(capacity, (tx_encoder,))
+        self._in: List[Deque[Tuple[np.ndarray, float]]] = [collections.deque() for _ in range(capacity)]
+        self._seq = [0] * capacity
+        self.stats = [StreamStats() for _ in range(capacity)]
+        self._packets: Deque[Tuple[int, bytes]] = collections.deque()
+        self.step_times: List[float] = []
+        self.wire_bytes = 0
+        self._x_host = _pinned(capacity * frame_size, torch.float32, self.device).view(capacity, frame_size)
+        self._x_np = self._x_host.numpy()
+        self._p_host = None                            # the packed bytes of a step, sized on the first step
+
+    def _reset_slot(self, s):
+        self._in[s].clear()
+        self._seq[s] = 0
+        self.stats[s] = StreamStats()
+
+    def _take_slot(self, s):
+        inputs, seq = list(self._in[s]), self._seq[s]
+        self._reset_slot(s)
+        return inputs, [], seq
+
+    def _restore_slot(self, s, state):
+        self._reset_slot(s)
+        self._in[s].extend(state.inputs)
+        self._seq[s] = state.seq
+
+    # ------------------------------------------------------------------ sessions
+    def open(self, session_id: int) -> int:
+        """Start session `session_id` (a u32) warm as the template.  ValueError if it is open already, RuntimeError when every slot
+        is taken."""
+        if not 0 <= session_id < 1 << 32:
+            raise ValueError(f"session id {session_id} does not fit in a u32")
+        return self._open_slot(session_id)
+
+    def close(self, session_id: int) -> None:
+        """End the session: its slot becomes free and its queued frames are dropped."""
+        self._close_slot(session_id)
+
+    def detach(self, session_id: int) -> SessionState:
+        """Close the session and return its causal state, queued frames and next sequence number (waits for a step in progress)."""
+        state = self._detach_slot(session_id)
+        state.session_id = session_id
+        return state
+
+    def attach(self, state: SessionState) -> int:
+        """Continue a session detached from a transmitter server of the same config and dtype, under its own id, from its next
+        sequence number.  The state must be on this server's device (SessionState.to)."""
+        if state.session_id is None:
+            raise ValueError("the session has no wire session id: it was not detached from a transmitter server")
+        return self._attach_slot(state, state.session_id)
+
+    @property
+    def open_sessions(self) -> List[int]:
+        with self._lock:
+            return sorted(self._ids)
+
+    def submit(self, session_id: int, frame, t_capture: Optional[float] = None) -> None:
+        """Queue one (frame_size,) float32 frame of the session.  A late session loses its OLDEST queued frames."""
+        f = _frame_in(frame, self.frame_size)
+        with self._lock:
+            s = self._slot(session_id)
+            _queue_frame(self._in[s], (f, time.time() if t_capture is None else t_capture), self.max_backlog, self.stats[s])
+
+    def pending(self, session_id: int) -> int:
+        with self._lock:
+            return len(self._in[self._slot(session_id)])
+
+    def poll_packets(self) -> List[Tuple[int, bytes]]:
+        """Every packet made since the last call, as (session_id, bytes), in the order the steps made them."""
+        with self._lock:
+            out = list(self._packets)
+            self._packets.clear()
+        return out
+
+    # ------------------------------------------------------------------ one step
+    def step(self) -> int:
+        """Encode one queued frame of every open session that has one, into one packet each.  Returns the number of packets made."""
+        with self._step_lock:
+            return self._step()
+
+    def _step(self) -> int:
+        t0 = time.time()
+        slots, sids, stamps, sessions = [], [], [], []
+        with self._lock:
+            for sid, s in sorted(self._ids.items()):
+                if s not in self._open:
+                    continue
+                q = self._in[s]
+                if q:
+                    f, t = q.popleft()
+                    self._x_np[len(slots)] = f
+                    slots.append(s)
+                    sids.append(sid)
+                    stamps.append(t)
+                    sessions.append(self._session[s])
+                else:
+                    self.stats[s].underruns += 1
+        n = len(slots)
+        if n == 0:
+            self.step_times.append(time.time() - t0)
+            return 0
+        tx = self.tx_encoder
+        with torch.no_grad(), self._codec_lock:
+            x = self._x_host[:n].to(self.device, non_blocking=True)
+            z, frames = tx.encode_streams(list(x), slots)
+            _, packed, _ = tx.quantize_fused(z, want_idx=False, want_packed=True, want_zq=False)    # (sum F, frame_bytes)
+            nb = packed.shape[-1]
+            if self._p_host is None or self._p_host.numel() < packed.numel():
+                self._p_host = _pinned(max(packed.numel(), self.capacity * frames[0] * nb), torch.uint8, self.device)
+            p_host = self._p_host[:packed.numel()]
+            p_host.copy_(packed.reshape(-1), non_blocking=True)
+            if packed.device.type == "cuda":
+                torch.cuda.current_stream(packed.device).synchronize()
+        now = time.time()
+        buf = p_host.numpy()
+        made = 0
+        with self._lock:
+            o = 0
+            for k, s in enumerate(slots):
+                payload = buf[o * nb:(o + frames[k]) * nb]
+                o += frames[k]
+                if s not in self._open or self._session[s] != sessions[k]:
+                    continue                        # closed while the step ran: no packet, and no sequence number spent
+                pkt = encode_packet(sids[k], self._seq[s], tx.codebook_num, nb, payload)
+                self._seq[s] += 1
+                self._packets.append((sids[k], pkt))
+                self.wire_bytes += len(pkt)
+                st = self.stats[s]
+                st.n_frames += 1
+                st.latencies.append(now - stamps[k])
+                made += 1
+        self.step_times.append(now - t0)
+        return made
+
+    def statistics(self) -> Dict:
+        """steps, ms per step (mean, std), the open sessions and, per open session, the input counters of StreamStats (n_frames: frames
+        encoded here) and the next sequence number."""
+        with self._lock:
+            per = {sid: dict(self.stats[s].as_dict(), next_seq=self._seq[s]) for sid, s in sorted(self._ids.items())}
+        return {"capacity": self.capacity, "open_sessions": len(per), "steps": len(self.step_times), "step_ms": _ms(self.step_times),
+                "wire_bytes": self.wire_bytes, "per_session": per}
+
+
+class ReceiveStats:
+    """Per-session counters of a ReceiverSessionServer."""
+
+    def __init__(self):
+        self.packets = 0           # packets decoded
+        self.frames = 0            # code frames decoded
+        self.bytes = 0             # wire bytes of the decoded packets, headers included
+        self.samples = 0           # PCM samples decoded
+        self.duplicates = 0        # packets dropped because the session had already decoded, held or given up their sequence number
+        self.reorders = 0          # packets that arrived after a packet with a higher sequence number and were put back in order
+        self.losses = 0            # sequence numbers given up as lost
+
+    def as_dict(self, sample_rate):
+        return {"packets": self.packets, "frames": self.frames, "duplicates": self.duplicates, "reorders": self.reorders,
+                "losses": self.losses,
+                "wire_kbps": 8e-3 * self.bytes / (self.samples / sample_rate) if self.samples else None}
+
+
+class ReceiverSessionServer(_SessionSlots):
+    """The receiving half of SessionCodecServer: wire packets (audiodec_b200.wire) in, decoded PCM frames per session out.
+
+    rx_encoder: a SymADStreamGenerator, for its codebooks (as in ``load_receiver``).  decoder: any of the library's decoders in any dtype
+    mode, holding the one warmed stream ``load_receiver`` leaves; bf16 output (bf16 activations) is widened to float32 frames.
+    frames_per_packet: the most code frames a packet may carry (the transmitter's frame_size over the codec hop), which sizes the
+    staging buffers.  ``open(session_id)`` binds a remote session to a warm slot; ``close``, ``detach`` and ``attach`` move the
+    decoder state, the held packets and the undelivered PCM frames.
+
+    ``submit_packet(bytes)`` parses and checks a packet (ValueError when it is malformed or made for another codec).  The defined
+    receive behaviour, per session: sequence numbers start at 0 and do not wrap.  A packet whose session is not open is counted
+    (``unknown_session_packets``) and dropped.  A packet whose sequence number the session has already decoded, holds or given up as
+    lost is counted in ``duplicates`` and dropped.  Packets are decoded in sequence order; one that arrives early is held.  When
+    ``reorder_window`` packets are held behind a missing one and another arrives (or a step finds more than that many), the missing
+    sequence numbers are counted as ``losses`` and decoding continues with the next packet held.  Nothing is concealed: the decoder
+    advances only by the frames it received, so a loss shortens the session's output by the lost packets' frames.
+
+    ``step()`` takes the next in-order packet of every open session that has one, copies their payloads to the device in ONE copy,
+    runs ONE ``lookup_packed`` over the concatenated frames and ONE ``decode_streams`` with each session's frame count, and copies the
+    PCM back in ONE copy.  ``poll(session_id)`` returns the session's next decoded frame (frames x hop float32 samples) or None."""
+
+    _noun = "session"
+    reorder_window = 4                 # packets held behind a missing one before it is given up
+
+    def __init__(self, rx_encoder, decoder, capacity: int, frames_per_packet: int, sample_rate: int = 48000, device=None):
+        if frames_per_packet < 1:
+            raise ValueError("frames_per_packet must be >= 1")
+        self.rx_encoder, self.decoder = rx_encoder, decoder
+        self.frames_per_packet, self.sample_rate = frames_per_packet, sample_rate
+        self.device = torch.device(device) if device is not None else torch.device("cpu")
+        self.codebook_num, self.frame_bytes = rx_encoder.codebook_num, rx_encoder.packed_frame_bytes()
+        super().__init__(capacity, (decoder,))
+        self._held: List[Dict[int, Packet]] = [{} for _ in range(capacity)]
+        self._next = [0] * capacity
+        self._out: List[Deque[np.ndarray]] = [collections.deque() for _ in range(capacity)]
+        self.stats = [ReceiveStats() for _ in range(capacity)]
+        self.unknown_session_packets = 0
+        self.step_times: List[float] = []
+        # a decoder with bf16 activations takes bf16 zq: the lookup rounds its fp32 sum once, as the decoder's own cast would
+        self._zq_kw = {"dtype": torch.bfloat16} if getattr(decoder, "_act_bf16", False) else {}
+        self._p_host = _pinned(capacity * frames_per_packet * self.frame_bytes, torch.uint8, self.device)
+        self._p_np = self._p_host.numpy()
+        self._y_host = None                            # the PCM of a step, sized on the first step
+
+    def _reset_slot(self, s):
+        self._held[s].clear()
+        self._next[s] = 0
+        self._out[s].clear()
+        self.stats[s] = ReceiveStats()
+
+    def _take_slot(self, s):
+        inputs, outputs, seq = [self._held[s][q] for q in sorted(self._held[s])], list(self._out[s]), self._next[s]
+        self._reset_slot(s)
+        return inputs, outputs, seq
+
+    def _restore_slot(self, s, state):
+        self._reset_slot(s)
+        self._held[s].update((p.seq, p) for p in state.inputs)
+        self._next[s] = state.seq
+        self._out[s].extend(state.outputs)
+
+    # ------------------------------------------------------------------ sessions
+    def open(self, session_id: int) -> int:
+        """Bind remote session `session_id` to a warm slot; its first packet is sequence number 0.  ValueError if it is open
+        already, RuntimeError when every slot is taken."""
+        return self._open_slot(session_id)
+
+    def close(self, session_id: int) -> None:
+        """End the session: its slot becomes free, its held packets and undelivered frames are dropped."""
+        self._close_slot(session_id)
+
+    def detach(self, session_id: int) -> SessionState:
+        """Close the session and return its decoder state, held packets, undelivered frames and the next sequence number it expects
+        (waits for a step in progress)."""
+        state = self._detach_slot(session_id)
+        state.session_id = session_id
+        return state
+
+    def attach(self, state: SessionState) -> int:
+        """Continue a session detached from a receiver server of the same config and dtype, under its own id, with fresh counters.
+        The state must be on this server's device (SessionState.to)."""
+        if state.session_id is None:
+            raise ValueError("the session has no wire session id: it was not detached from a receiver server")
+        return self._attach_slot(state, state.session_id)
+
+    @property
+    def open_sessions(self) -> List[int]:
+        with self._lock:
+            return sorted(self._ids)
+
+    def _give_up_gap(self, s) -> None:
+        """More than reorder_window packets held behind a missing one: count the missing ones lost and move on to the first held."""
+        held = self._held[s]
+        if len(held) > self.reorder_window and self._next[s] not in held:
+            first = min(held)
+            self.stats[s].losses += first - self._next[s]
+            self._next[s] = first
+
+    def submit_packet(self, buf) -> bool:
+        """Take one packet.  Returns True if it was queued for decoding, False if it was counted and dropped (session not open,
+        duplicate).  Raises ValueError for a malformed packet, one made for another codec, or one of more than frames_per_packet
+        frames."""
+        p = decode_packet(buf, self.codebook_num, self.frame_bytes)
+        if p.frames > self.frames_per_packet:
+            raise ValueError(f"frames: packet has {p.frames}, this receiver takes at most {self.frames_per_packet}")
+        with self._lock:
+            s = self._ids.get(p.session_id)
+            if s is None or s not in self._open:
+                self.unknown_session_packets += 1
+                return False
+            held, st = self._held[s], self.stats[s]
+            if p.seq < self._next[s] or p.seq in held:
+                st.duplicates += 1
+                return False
+            if any(q > p.seq for q in held):
+                st.reorders += 1
+            held[p.seq] = p
+            self._give_up_gap(s)
+            return True
+
+    def poll(self, session_id: int) -> Optional[np.ndarray]:
+        """The session's next decoded frame (float32, frames x hop samples), or None."""
+        with self._lock:
+            q = self._out[self._slot(session_id)]
+            return q.popleft() if q else None
+
+    # ------------------------------------------------------------------ one step
+    def step(self) -> int:
+        """Decode the next in-order packet of every open session that has one.  Returns the number of packets decoded."""
+        with self._step_lock:
+            return self._step()
+
+    def _step(self) -> int:
+        t0 = time.time()
+        taken: List[Tuple[int, int, Packet]] = []          # (slot, open counter, packet)
+        with self._lock:
+            for sid, s in sorted(self._ids.items()):
+                if s not in self._open:
+                    continue
+                self._give_up_gap(s)
+                p = self._held[s].pop(self._next[s], None)
+                if p is not None:
+                    self._next[s] += 1
+                    taken.append((s, self._session[s], p))
+        if not taken:
+            self.step_times.append(time.time() - t0)
+            return 0
+        nb = self.frame_bytes
+        frames = [p.frames for _, _, p in taken]
+        total = sum(frames)
+        o = 0
+        for _, _, p in taken:
+            self._p_np[o:o + len(p.payload)] = np.frombuffer(p.payload, dtype=np.uint8)
+            o += len(p.payload)
+        with torch.no_grad(), self._codec_lock:
+            packed = self._p_host[:total * nb].to(self.device, non_blocking=True).view(1, total, nb)
+            zq = self.rx_encoder.lookup_packed(packed, **self._zq_kw)
+            ys = self.decoder.decode_streams(zq, frames, [s for s, _, _ in taken])
+            y = torch.cat([v.reshape(-1) for v in ys])
+            hop = y.numel() // total
+            if self._y_host is None or self._y_host.dtype != y.dtype or self._y_host.numel() < y.numel():
+                self._y_host = _pinned(max(y.numel(), self.capacity * self.frames_per_packet * hop), y.dtype, self.device)
+            y_host = self._y_host[:y.numel()]
+            y_host.copy_(y, non_blocking=True)
+            if y.device.type == "cuda":
+                torch.cuda.current_stream(y.device).synchronize()
+        # one copy out of the staging buffer (widened from bf16 with bf16 activations); the queues hold views of it
+        y_np = (y_host.float() if y_host.dtype == torch.bfloat16 else y_host.clone()).numpy()
+        with self._lock:
+            o = 0
+            for (s, session, p), f in zip(taken, frames):
+                chunk = y_np[o * hop:(o + f) * hop]
+                o += f
+                if s not in self._open or self._session[s] != session:
+                    continue                        # closed while the step ran: the frame is dropped
+                self._out[s].append(chunk)
+                st = self.stats[s]
+                st.packets += 1
+                st.frames += f
+                st.bytes += HEADER_BYTES + len(p.payload)
+                st.samples += chunk.size
+        self.step_times.append(time.time() - t0)
+        return len(taken)
+
+    def statistics(self) -> Dict:
+        """steps, ms per step (mean, std), the open sessions, packets for sessions that were not open, and per open session: packets,
+        frames, duplicates, reorders, losses and the wire kbps received (packet bytes, headers included, over the seconds of audio
+        decoded)."""
+        with self._lock:
+            per = {sid: self.stats[s].as_dict(self.sample_rate) for sid, s in sorted(self._ids.items())}
+        return {"capacity": self.capacity, "open_sessions": len(per), "steps": len(self.step_times), "step_ms": _ms(self.step_times),
+                "unknown_session_packets": self.unknown_session_packets, "per_session": per}
