@@ -54,6 +54,12 @@ class AdecTestOp(ctypes.Structure):
     ]
 
 
+class AdecConcealRow(ctypes.Structure):
+    """struct adec_conceal_row (include/audiodec_b200.h): one output row of adec_lookup_packed_conceal."""
+    _fields_ = [("src", ctypes.c_int32), ("next", ctypes.c_int32), ("slot", ctypes.c_int32), ("j", ctypes.c_int32),
+                ("den", ctypes.c_int32)]
+
+
 TEST_CONV, TEST_RU, TEST_CONVTR, TEST_STEM, TEST_HEAD = 0, 1, 2, 3, 4
 TEST_REC = 9
 
@@ -76,6 +82,10 @@ SYMBOLS = {
     "adec_lookup_packed": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "adec_lookup_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "adec_lookup_packed_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "adec_lookup_packed_conceal": (c_int, [c_void_p, c_void_p, c_int, ctypes.POINTER(AdecConcealRow), c_int, c_void_p, c_int, c_void_p,
+                                           c_void_p]),
+    "adec_lookup_packed_conceal_bf16": (c_int, [c_void_p, c_void_p, c_int, ctypes.POINTER(AdecConcealRow), c_int, c_void_p, c_int,
+                                                c_void_p, c_void_p]),
     "adec_graph_create": (c_int, [c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, ctypes.POINTER(c_void_p)]),
     "adec_graph_launch": (c_int, [c_void_p, c_void_p]),
     "adec_graph_info": (c_int, [c_void_p, ctypes.POINTER(c_int), ctypes.POINTER(c_int), ctypes.POINTER(c_int)]),

@@ -30,6 +30,7 @@ from __future__ import annotations
 import ctypes
 import inspect
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -632,6 +633,34 @@ class SymADStreamGenerator(_SymADTransmitter):
         fn = self._lookup_fn("adec_lookup_packed", dtype)
         zq = torch.empty(b, f, self.code_dim, device=self._device, dtype=dtype)
         _check(fn(self._h, _ptr(packed), b, f, _ptr(zq), self._stream()), self._h)
+        return zq
+
+    def lookup_packed_conceal(self, packed, rows, anchors, dtype=torch.float32):
+        """The packed lookup with loss concealment, in ONE launch (adec_lookup_packed_conceal): uint8 packed frames (F, bytes) or
+        (1, F, bytes), and one descriptor per output row -> zq (1, R, D).  rows: R rows of (src, next, slot, j, den) ints (an (R, 5)
+        array or a sequence of 5-tuples), checked before anything runs.  A real row (src >= 0) is lookup_packed's row of frame src and,
+        with slot >= 0, stores its fp32 sum in anchors[slot].  A concealed row (src = -1) is fl(fl(fl(j / den) * fl(s_b - a)) + a) with
+        s_b the sum of frame next and a = anchors[slot], or s_b with slot = -1.  anchors: a contiguous float32 (n_anchors, code_dim)
+        device tensor, updated in place.  dtype=torch.bfloat16: bf16 zq, the fp32 result rounded once."""
+        self._ready()
+        packed = self._in(packed, torch.uint8)
+        if packed.dim() == 3 and packed.size(0) == 1:
+            packed = packed[0]
+        if packed.dim() != 2 or packed.size(1) != self.packed_frame_bytes():
+            raise RuntimeError(f"audiodec_b200: lookup_packed_conceal: expected (F, {self.packed_frame_bytes()}) packed frames, got "
+                               f"{tuple(packed.shape)}")
+        if not isinstance(anchors, torch.Tensor) or anchors.device != self._device or anchors.dtype != torch.float32 or \
+                anchors.dim() != 2 or anchors.size(1) != self.code_dim or not anchors.is_contiguous():
+            raise RuntimeError(f"audiodec_b200: lookup_packed_conceal: anchors must be a contiguous float32 (n, {self.code_dim}) tensor "
+                               f"on {self._device}")
+        desc = np.ascontiguousarray(rows, dtype=np.int32)
+        if desc.ndim != 2 or desc.shape[1] != 5:
+            raise ValueError(f"audiodec_b200: lookup_packed_conceal: rows must be (R, 5) (src, next, slot, j, den), got {desc.shape}")
+        r = desc.shape[0]
+        fn = self._lookup_fn("adec_lookup_packed_conceal", dtype)
+        zq = torch.empty(1, r, self.code_dim, device=self._device, dtype=dtype)
+        _check(fn(self._h, _ptr(packed), packed.size(0), desc.ctypes.data_as(ctypes.POINTER(_lib.AdecConcealRow)), r, _ptr(anchors),
+                  anchors.size(0), _ptr(zq), self._stream()), self._h)
         return zq
 
     def _lookup_fn(self, name, dtype):

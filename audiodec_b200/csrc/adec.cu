@@ -279,6 +279,7 @@ struct adec_handle {
     DevBuf hx, hz, hzq, hy;
     DevBuf vl_tab;                // varlen row tables of the last call (ints)
     DevBuf mom_tab;               // row offsets of the last adec_zq_moments call (ints)
+    DevBuf conceal_tab;           // row descriptors of the last adec_lookup_packed_conceal call (adec_conceal_row)
     SlotBits enc_slots, dec_slots;
     DevBuf slot_tab;              // stream pairs of the last state copy (ints)
     // the state map: every reference pad_buffer the handle runs, in plan order (encoder ops, then decoder ops), one stream's exported
@@ -1474,7 +1475,7 @@ void adec_destroy(adec_handle* h) {
         for (Op& op : *ops)
             for (int i = 0; i < 2; ++i) if (op.st[i]) cudaFree(op.st[i]);
     for (auto& b : h->ws) if (b.p) cudaFree(b.p);
-    for (DevBuf* b : {&h->hx, &h->hz, &h->hzq, &h->hy, &h->vl_tab, &h->mom_tab, &h->slot_tab, &h->st_tab}) if (b->p) cudaFree(b->p);
+    for (DevBuf* b : {&h->hx, &h->hz, &h->hzq, &h->hy, &h->vl_tab, &h->mom_tab, &h->conceal_tab, &h->slot_tab, &h->st_tab}) if (b->p) cudaFree(b->p);
     if (h->hidx) cudaFree(h->hidx);
     if (h->d_err) cudaFree(h->d_err);
     if (h->d_ktrace) cudaFree(h->d_ktrace);
@@ -2007,6 +2008,74 @@ int adec_lookup_packed(adec_handle* h, const uint8_t* packed, int B, int F, floa
 
 int adec_lookup_packed_bf16(adec_handle* h, const uint8_t* packed, int B, int F, uint16_t* zq, void* stream) {
     return lookup_common(h, nullptr, packed, B, F, zq, true, stream);
+}
+
+static_assert(sizeof(adec_conceal_row) == sizeof(ConcealRow), "adec_conceal_row and ConcealRow must share a layout");
+
+// Every descriptor is checked here, before anything is enqueued, so that a bad one fails with the field's name instead of a fault
+static int conceal_common(adec_handle* h, const uint8_t* packed, int F, const adec_conceal_row* rows, int R, float* anchors,
+                          int n_anchors, void* zq, bool bf16, void* stream) {
+    if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
+    const std::string what = bf16 ? "lookup_packed_conceal_bf16" : "lookup_packed_conceal";
+    if (need_full_symad(h, what)) return 1;
+    if (F < 1 || R < 1) return h->fail(what + ": empty input (F and R must be >= 1)");
+    if (n_anchors < 0) return h->fail(what + ": n_anchors < 0");
+    if (!packed || !rows || !zq) return h->fail(what + ": packed, rows and zq must be given");
+    if (n_anchors > 0 && (!anchors || (uintptr_t)anchors % 16)) return h->fail(what + ": anchors must be a 16-byte aligned device buffer");
+    if (bf16 && (h->cfg.code_dim % 8 || (uintptr_t)zq % 16))
+        return h->fail(what + ": needs code_dim % 8 == 0 and a 16-byte aligned zq");
+    std::vector<int> reader(n_anchors, -1), writer(n_anchors, -1);     // per anchor slot: a row that reads it, a row that writes it
+    for (int r = 0; r < R; ++r) {
+        const adec_conceal_row& d = rows[r];
+        const bool real = d.src >= 0;
+        if (real && d.src >= F) return h->fail(fmt("%s: rows[%d].src = %d is out of range [0, %d)", what.c_str(), r, d.src, F));
+        if (real && d.next != -1) return h->fail(fmt("%s: rows[%d].next = %d: a real row (src >= 0) has next = -1", what.c_str(), r, d.next));
+        if (!real && d.src != -1) return h->fail(fmt("%s: rows[%d].src = %d is out of range: a frame in [0, %d) or -1", what.c_str(), r, d.src, F));
+        if (!real && (d.next < 0 || d.next >= F))
+            return h->fail(fmt("%s: rows[%d].next = %d is out of range [0, %d)", what.c_str(), r, d.next, F));
+        if (!real && d.den < 2) return h->fail(fmt("%s: rows[%d].den = %d: a concealed row needs den >= 2", what.c_str(), r, d.den));
+        if (!real && (d.j < 1 || d.j >= d.den))
+            return h->fail(fmt("%s: rows[%d].j = %d is outside [1, den = %d)", what.c_str(), r, d.j, d.den));
+        if (d.slot < -1 || d.slot >= n_anchors)
+            return h->fail(fmt("%s: rows[%d].slot = %d is out of range: an anchor in [0, %d) or -1", what.c_str(), r, d.slot, n_anchors));
+        if (d.slot < 0) continue;
+        std::vector<int>& mine = real ? writer : reader;
+        const std::vector<int>& other = real ? reader : writer;
+        if (other[d.slot] >= 0)
+            return h->fail(fmt("%s: rows[%d].slot = %d: anchor %d is read by row %d and written by row %d of the same call", what.c_str(), r,
+                               d.slot, d.slot, real ? other[d.slot] : r, real ? r : other[d.slot]));
+        if (real && mine[d.slot] >= 0)
+            return h->fail(fmt("%s: rows[%d].slot = %d: anchor %d is written by rows %d and %d of the same call", what.c_str(), r, d.slot,
+                               d.slot, mine[d.slot], r));
+        mine[d.slot] = r;
+    }
+    DeviceGuard dg(h->device);
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (ensure(h, h->conceal_tab, (size_t)R * sizeof(adec_conceal_row) / sizeof(float))) return 1;
+    CK(h, cudaMemcpyAsync(h->conceal_tab.p, rows, (size_t)R * sizeof(adec_conceal_row), cudaMemcpyHostToDevice, s));
+    ConcealArgs c{};
+    LookupArgs& a = c.l;
+    a.packed = packed; a.nfr = R; a.nq = h->cfg.codebook_num; a.D = h->cfg.code_dim;
+    a.N = h->cfg.codebook_size; a.bits = index_bits(a.N); a.bpf = adec_packed_frame_bytes(h);
+    a.codebook = h->d_codebook; a.n_rows = (long long)h->cfg.codebook_num * h->cfg.codebook_size; a.zq = (float*)zq; a.err = h->d_err;
+    c.rows = reinterpret_cast<const ConcealRow*>(h->conceal_tab.p);
+    c.anchors = anchors;
+    const long long nth = a.nfr * (a.D / 4);
+    if (bf16) lookup_conceal_kernel<true><<<(unsigned)((nth + 255) / 256), 256, 0, s>>>(c);
+    else lookup_conceal_kernel<false><<<(unsigned)((nth + 255) / 256), 256, 0, s>>>(c);
+    CK(h, cudaGetLastError());
+    ++h->launches;
+    return 0;
+}
+
+int adec_lookup_packed_conceal(adec_handle* h, const uint8_t* packed, int F, const adec_conceal_row* rows, int R, float* anchors,
+                               int n_anchors, float* zq, void* stream) {
+    return conceal_common(h, packed, F, rows, R, anchors, n_anchors, zq, false, stream);
+}
+
+int adec_lookup_packed_conceal_bf16(adec_handle* h, const uint8_t* packed, int F, const adec_conceal_row* rows, int R, float* anchors,
+                                    int n_anchors, uint16_t* zq, void* stream) {
+    return conceal_common(h, packed, F, rows, R, anchors, n_anchors, zq, true, stream);
 }
 
 int adec_codec_host(adec_handle* enc, adec_handle* dec, const float* x_host, int B, int T, int64_t* idx_host,

@@ -19,6 +19,8 @@
 //   rvq_kernel        - 8-stage residual VQ: fp32 distances in the reference's rounding order,
 //                       first-index arg-min by warp shuffles, int64 flat indices.
 //   lookup_kernel     - codebook gather-sum (fp32 zq, or bf16 zq rounded once).
+//   lookup_conceal_kernel - the packed lookup per row descriptor: real frames, plus concealed frames interpolated between a
+//                       session's last real frame (an fp32 anchor row) and the frame after a loss.
 //   zq_moments_kernel - per-utterance fp64 sums and centred second moments of zq (corpus statistics).
 #pragma once
 #include <cuda_bf16.h>
@@ -934,6 +936,65 @@ __global__ void __launch_bounds__(256) lookup_kernel(const LookupArgs a) {
         *reinterpret_cast<uint2*>(reinterpret_cast<uint16_t*>(a.zq) + fr * a.D + k4) = make_uint2(bf2_bits(s.x, s.y), bf2_bits(s.z, s.w));
     else
         *reinterpret_cast<float4*>(a.zq + fr * a.D + k4) = s;
+}
+
+// Loss concealment on the packed lookup: output row r follows descriptor rows[r] (adec_conceal_row, checked on the host).
+//   real row (src >= 0):      zq[r] = the sum of packed frame src, as lookup_kernel computes it; with slot >= 0 the fp32 sum also goes
+//                             to anchors[slot] (the session's last real frame of the launch).
+//   concealed row (src < 0):  s_b = the sum of packed frame next, a = anchors[slot]; with w = fl(j / den),
+//                             zq[r] = fl(fl(w * fl(s_b - a)) + a), each operation rounded separately; slot < 0 (no anchor): zq[r] = s_b.
+// BF16 rounds the fp32 result once, as lookup_kernel<true> does.  The host refuses a slot that one row reads and another writes, so
+// no row of a launch sees another's anchor store.
+struct ConcealRow {
+    int src, next, slot, j, den;   // adec_conceal_row
+};
+
+struct ConcealArgs {
+    LookupArgs l;                  // packed frames, codebook, err; l.nfr = output rows, l.zq = (rows, D)
+    const ConcealRow* rows;        // (l.nfr)
+    float* anchors;                // (n_anchors, D) fp32, 16-byte aligned
+};
+
+template <bool BF16>
+__global__ void __launch_bounds__(256) lookup_conceal_kernel(const ConcealArgs c) {
+    const LookupArgs& a = c.l;
+    const int vpf = a.D / 4;
+    const long long gid = (long long)blockIdx.x * 256 + threadIdx.x;
+    if (gid >= a.nfr * vpf) return;
+    const long long r = gid / vpf;
+    const int k4 = (int)(gid - r * vpf) * 4;
+    const ConcealRow d = c.rows[r];
+    const bool real = d.src >= 0;
+    const unsigned char* in = a.packed + (long long)(real ? d.src : d.next) * a.bpf;
+    const unsigned long long mask = (1ull << a.bits) - 1ull;
+    unsigned long long accb = 0;
+    int nb = 0, ib = 0;
+    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int i = 0; i < a.nq; ++i) {
+        while (nb < a.bits) { accb |= (unsigned long long)in[ib++] << nb; nb += 8; }
+        const long long v = (long long)(accb & mask);
+        accb >>= a.bits; nb -= a.bits;
+        const long long row = v < a.N ? v + (long long)i * a.N : -1;
+        if (row < 0 || row >= a.n_rows) { atomicOr(a.err, 1); continue; }
+        const float4 q = __ldg(reinterpret_cast<const float4*>(a.codebook + row * a.D + k4));
+        if (i == 0) s = q;
+        else { s.x = __fadd_rn(s.x, q.x); s.y = __fadd_rn(s.y, q.y); s.z = __fadd_rn(s.z, q.z); s.w = __fadd_rn(s.w, q.w); }
+    }
+    float4* anchor = d.slot >= 0 ? reinterpret_cast<float4*>(c.anchors + (long long)d.slot * a.D + k4) : nullptr;
+    if (real) {
+        if (anchor) *anchor = s;
+    } else if (anchor) {
+        const float4 av = *anchor;
+        const float w = __fdiv_rn((float)d.j, (float)d.den);
+        s.x = __fadd_rn(__fmul_rn(w, __fsub_rn(s.x, av.x)), av.x);
+        s.y = __fadd_rn(__fmul_rn(w, __fsub_rn(s.y, av.y)), av.y);
+        s.z = __fadd_rn(__fmul_rn(w, __fsub_rn(s.z, av.z)), av.z);
+        s.w = __fadd_rn(__fmul_rn(w, __fsub_rn(s.w, av.w)), av.w);
+    }
+    if constexpr (BF16)
+        *reinterpret_cast<uint2*>(reinterpret_cast<uint16_t*>(a.zq) + r * a.D + k4) = make_uint2(bf2_bits(s.x, s.y), bf2_bits(s.z, s.w));
+    else
+        *reinterpret_cast<float4*>(a.zq + r * a.D + k4) = s;
 }
 
 // Per-utterance moments of the quantizer output (codecStatistic.py:104-105 calls StandardScaler.partial_fit once per file), fp64

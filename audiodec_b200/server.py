@@ -276,20 +276,25 @@ class SessionState:
     """What a detached session needs to continue on another server of the same kind (same config and dtypes, on any device): per
     stateful generator of the server its state_layout and its (1, S) device state, the queued input (frames with their capture stamps
     on SessionCodecServer and TransmitterSessionServer, held packets on ReceiverSessionServer), and the decoded frames it has not polled
-    yet.  On the split servers also the session's wire id and the next sequence number it sends or expects."""
+    yet.  On the split servers also the session's wire id and the next sequence number it sends or expects.  On a ReceiverSessionServer
+    that conceals losses also the fp32 anchor row (the lookup sum of the session's last real frame, a (code_dim,) device tensor, None
+    before its first real frame) and the concealment still pending, (packets left, frames per packet, frames concealed so far, frames in
+    the gap), or None."""
 
-    def __init__(self, layouts, states, inputs, outputs, session_id=None, seq=0):
+    def __init__(self, layouts, states, inputs, outputs, session_id=None, seq=0, anchor=None, conceal=None):
         self.layouts: List[list] = layouts
         self.states: List[torch.Tensor] = states
         self.inputs: list = inputs
         self.outputs: List[np.ndarray] = outputs
         self.session_id: Optional[int] = session_id
         self.seq: int = seq
+        self.anchor: Optional[torch.Tensor] = anchor
+        self.conceal: Optional[Tuple[int, int, int, int]] = conceal
 
     def to(self, device) -> "SessionState":
-        """A copy with the states on `device` (the frames are host arrays and are shared)."""
+        """A copy with the states and the anchor on `device` (the frames are host arrays and are shared)."""
         return SessionState(self.layouts, [t.to(device) for t in self.states], list(self.inputs), list(self.outputs), self.session_id,
-                            self.seq)
+                            self.seq, None if self.anchor is None else self.anchor.to(device), self.conceal)
 
 
 class _SessionSlots:
@@ -336,6 +341,10 @@ class _SessionSlots:
     def _restore_slot(self, s: int, state: SessionState) -> None:
         raise NotImplementedError
 
+    def _export_slot(self, s: int) -> dict:
+        """-> the SessionState keywords of what slot s carries besides its queues and causal state (called before _take_slot)"""
+        return {}
+
     def _slot(self, sid) -> int:
         s = self._ids.get(sid)
         if s is None or s not in self._open:
@@ -381,13 +390,14 @@ class _SessionSlots:
                 s = self._slot(sid)
                 self._open.remove(s)
                 del self._ids[sid]
+                extra = self._export_slot(s)
                 inputs, outputs, seq = self._take_slot(s)
             with self._codec_lock:       # the slot stays taken until its state is out
                 states = [g.stream_state([s]) for g in self._stateful]
             layouts = [list(g.state_layout) for g in self._stateful]
             with self._lock:
                 self._free.append(s)
-        return SessionState(layouts, states, inputs, outputs, seq=seq)
+        return SessionState(layouts, states, inputs, outputs, seq=seq, **extra)
 
     def _attach_slot(self, state: SessionState, sid=None):
         if len(state.states) != len(self._stateful) or len(state.layouts) != len(self._stateful):
@@ -717,10 +727,13 @@ class ReceiveStats:
         self.duplicates = 0        # packets dropped because the session had already decoded, held or given up their sequence number
         self.reorders = 0          # packets that arrived after a packet with a higher sequence number and were put back in order
         self.losses = 0            # sequence numbers given up as lost
+        self.concealed = 0         # lost sequence numbers decoded as concealed packets (conceal_packets > 0)
+        self.concealed_frames = 0  # code frames of those packets
 
     def as_dict(self, sample_rate):
+        """packets, frames and wire_kbps count the real packets only"""
         return {"packets": self.packets, "frames": self.frames, "duplicates": self.duplicates, "reorders": self.reorders,
-                "losses": self.losses,
+                "losses": self.losses, "concealed": self.concealed, "concealed_frames": self.concealed_frames,
                 "wire_kbps": 8e-3 * self.bytes / (self.samples / sample_rate) if self.samples else None}
 
 
@@ -738,21 +751,39 @@ class ReceiverSessionServer(_SessionSlots):
     (``unknown_session_packets``) and dropped.  A packet whose sequence number the session has already decoded, holds or given up as
     lost is counted in ``duplicates`` and dropped.  Packets are decoded in sequence order; one that arrives early is held.  When
     ``reorder_window`` packets are held behind a missing one and another arrives (or a step finds more than that many), the missing
-    sequence numbers are counted as ``losses`` and decoding continues with the next packet held.  Nothing is concealed: the decoder
-    advances only by the frames it received, so a loss shortens the session's output by the lost packets' frames.
+    sequence numbers are counted as ``losses`` and decoding continues with the next packet held.  With ``conceal_packets = 0`` (the
+    default) nothing is concealed: the decoder advances only by the frames it received, so a loss shortens the session's output by the
+    lost packets' frames.
+
+    ``conceal_packets = K > 0`` conceals losses.  When a session gives up a gap of G sequence numbers in front of held packet b, the
+    last min(G, K) of them are decoded as concealed packets of b.frames frames each (any earlier ones stay lost), one per step and in
+    sequence order, before b; their PCM is queued for ``poll`` like a real packet's, so the output stays in step with the sender and
+    the decoder's causal state runs through the gap.  Concealed frame j of the M = min(G, K) * b.frames frames in the gap is the fp32
+    interpolation a + fl(j / (M + 1)) * (s_b - a), each operation rounded on its own, between a, the lookup sum of the session's last
+    real frame, and s_b, the sum of b's first frame (s_b alone if the session has decoded no real frame yet); a decoder with bf16
+    activations gets it rounded once to bf16.  ``losses`` still counts all G; ``concealed`` and ``concealed_frames`` count what was
+    concealed, and the other counters count real packets only.  A loss needs a following packet to be concealed, so one at the end of
+    a talk spurt waits as before.  A late packet for a concealed sequence number is a duplicate.
 
     ``step()`` takes the next in-order packet of every open session that has one, copies their payloads to the device in ONE copy,
     runs ONE ``lookup_packed`` over the concatenated frames and ONE ``decode_streams`` with each session's frame count, and copies the
-    PCM back in ONE copy.  ``poll(session_id)`` returns the session's next decoded frame (frames x hop float32 samples) or None."""
+    PCM back in ONE copy.  With concealment the lookup is ONE ``lookup_packed_conceal`` instead, which also keeps every session's
+    anchor row (a (capacity, code_dim) fp32 device tensor); a session that conceals this step stages b's first frame in place of a
+    payload.  ``poll(session_id)`` returns the session's next decoded frame (frames x hop float32 samples) or None.  ``detach`` /
+    ``attach`` also carry the anchor row and any concealment still pending; a receiver without concealment drops them."""
 
     _noun = "session"
     reorder_window = 4                 # packets held behind a missing one before it is given up
 
-    def __init__(self, rx_encoder, decoder, capacity: int, frames_per_packet: int, sample_rate: int = 48000, device=None):
+    def __init__(self, rx_encoder, decoder, capacity: int, frames_per_packet: int, sample_rate: int = 48000, device=None,
+                 conceal_packets: int = 0):
         if frames_per_packet < 1:
             raise ValueError("frames_per_packet must be >= 1")
+        if conceal_packets < 0:
+            raise ValueError("conceal_packets must be >= 0")
         self.rx_encoder, self.decoder = rx_encoder, decoder
         self.frames_per_packet, self.sample_rate = frames_per_packet, sample_rate
+        self.conceal_packets = conceal_packets
         self.device = torch.device(device) if device is not None else torch.device("cpu")
         self.codebook_num, self.frame_bytes = rx_encoder.codebook_num, rx_encoder.packed_frame_bytes()
         super().__init__(capacity, (decoder,))
@@ -767,12 +798,25 @@ class ReceiverSessionServer(_SessionSlots):
         self._p_host = _pinned(capacity * frames_per_packet * self.frame_bytes, torch.uint8, self.device)
         self._p_np = self._p_host.numpy()
         self._y_host = None                            # the PCM of a step, sized on the first step
+        # concealment: per slot the fp32 lookup sum of the last real frame decoded, whether there is one, and the pending plan
+        # [packets left, frames per packet, frames concealed so far, frames in the gap]
+        self._anchors = torch.zeros(capacity, rx_encoder.code_dim, dtype=torch.float32, device=self.device) if conceal_packets else None
+        self._has_anchor = [False] * capacity
+        self._plan: List[Optional[list]] = [None] * capacity
 
     def _reset_slot(self, s):
         self._held[s].clear()
         self._next[s] = 0
         self._out[s].clear()
         self.stats[s] = ReceiveStats()
+        self._has_anchor[s] = False
+        self._plan[s] = None
+
+    def _export_slot(self, s):
+        if not self.conceal_packets:
+            return {}
+        plan = self._plan[s]
+        return {"anchor": self._anchors[s].clone() if self._has_anchor[s] else None, "conceal": None if plan is None else tuple(plan)}
 
     def _take_slot(self, s):
         inputs, outputs, seq = [self._held[s][q] for q in sorted(self._held[s])], list(self._out[s]), self._next[s]
@@ -784,6 +828,12 @@ class ReceiverSessionServer(_SessionSlots):
         self._held[s].update((p.seq, p) for p in state.inputs)
         self._next[s] = state.seq
         self._out[s].extend(state.outputs)
+        if self.conceal_packets:
+            if state.anchor is not None:
+                self._anchors[s].copy_(state.anchor)
+                self._has_anchor[s] = True
+            if state.conceal is not None:
+                self._plan[s] = list(state.conceal)
 
     # ------------------------------------------------------------------ sessions
     def open(self, session_id: int) -> int:
@@ -815,12 +865,17 @@ class ReceiverSessionServer(_SessionSlots):
             return sorted(self._ids)
 
     def _give_up_gap(self, s) -> None:
-        """More than reorder_window packets held behind a missing one: count the missing ones lost and move on to the first held."""
+        """More than reorder_window packets held behind a missing one: count the missing ones lost and move on to the first held.  With
+        concealment, plan the last conceal_packets of them as concealed packets of the first held packet's frame count."""
         held = self._held[s]
         if len(held) > self.reorder_window and self._next[s] not in held:
             first = min(held)
-            self.stats[s].losses += first - self._next[s]
+            gap = first - self._next[s]
+            self.stats[s].losses += gap
             self._next[s] = first
+            if self.conceal_packets:
+                n, f = min(gap, self.conceal_packets), held[first].frames
+                self._plan[s] = [n, f, 0, n * f]
 
     def submit_packet(self, buf) -> bool:
         """Take one packet.  Returns True if it was queued for decoding, False if it was counted and dropped (session not open,
@@ -852,36 +907,57 @@ class ReceiverSessionServer(_SessionSlots):
 
     # ------------------------------------------------------------------ one step
     def step(self) -> int:
-        """Decode the next in-order packet of every open session that has one.  Returns the number of packets decoded."""
+        """Decode the next in-order packet of every open session that has one, or its next concealed packet.  Returns the number of
+        packets decoded, concealed ones included."""
         with self._step_lock:
             return self._step()
 
     def _step(self) -> int:
         t0 = time.time()
-        taken: List[Tuple[int, int, Packet]] = []          # (slot, open counter, packet)
+        # (slot, open counter, packet, concealment): a real packet with None, or a concealed one with (first j, M + 1, anchor slot or
+        # -1) and the packet after the gap, still held, as its packet
+        taken: List[Tuple[int, int, Packet, Optional[Tuple[int, int, int]]]] = []
         with self._lock:
             for sid, s in sorted(self._ids.items()):
                 if s not in self._open:
                     continue
                 self._give_up_gap(s)
+                plan = self._plan[s]
+                if plan is not None:
+                    taken.append((s, self._session[s], self._held[s][self._next[s]],
+                                  (plan[2] + 1, plan[3] + 1, s if self._has_anchor[s] else -1)))
+                    plan[0] -= 1
+                    plan[2] += plan[1]
+                    if plan[0] == 0:
+                        self._plan[s] = None
+                    continue
                 p = self._held[s].pop(self._next[s], None)
                 if p is not None:
                     self._next[s] += 1
-                    taken.append((s, self._session[s], p))
+                    taken.append((s, self._session[s], p, None))
+                    self._has_anchor[s] = True
         if not taken:
             self.step_times.append(time.time() - t0)
             return 0
         nb = self.frame_bytes
-        frames = [p.frames for _, _, p in taken]
+        frames = [p.frames for _, _, p, _ in taken]
         total = sum(frames)
         o = 0
-        for _, _, p in taken:
-            self._p_np[o:o + len(p.payload)] = np.frombuffer(p.payload, dtype=np.uint8)
-            o += len(p.payload)
+        staged = []                                    # per taken packet: its first frame in the staged bytes
+        for _, _, p, c in taken:
+            n = nb if c is not None else len(p.payload)   # a concealed packet stages only the first frame after the gap
+            self._p_np[o:o + n] = np.frombuffer(p.payload, dtype=np.uint8, count=n)
+            staged.append(o // nb)
+            o += n
         with torch.no_grad(), self._codec_lock:
-            packed = self._p_host[:total * nb].to(self.device, non_blocking=True).view(1, total, nb)
-            zq = self.rx_encoder.lookup_packed(packed, **self._zq_kw)
-            ys = self.decoder.decode_streams(zq, frames, [s for s, _, _ in taken])
+            if self.conceal_packets:
+                packed = self._p_host[:o].to(self.device, non_blocking=True).view(o // nb, nb)
+                zq = self.rx_encoder.lookup_packed_conceal(packed, self._conceal_rows(taken, frames, staged), self._anchors,
+                                                           **self._zq_kw)
+            else:
+                packed = self._p_host[:total * nb].to(self.device, non_blocking=True).view(1, total, nb)
+                zq = self.rx_encoder.lookup_packed(packed, **self._zq_kw)
+            ys = self.decoder.decode_streams(zq, frames, [s for s, _, _, _ in taken])
             y = torch.cat([v.reshape(-1) for v in ys])
             hop = y.numel() // total
             if self._y_host is None or self._y_host.dtype != y.dtype or self._y_host.numel() < y.numel():
@@ -894,13 +970,17 @@ class ReceiverSessionServer(_SessionSlots):
         y_np = (y_host.float() if y_host.dtype == torch.bfloat16 else y_host.clone()).numpy()
         with self._lock:
             o = 0
-            for (s, session, p), f in zip(taken, frames):
+            for (s, session, p, c), f in zip(taken, frames):
                 chunk = y_np[o * hop:(o + f) * hop]
                 o += f
                 if s not in self._open or self._session[s] != session:
                     continue                        # closed while the step ran: the frame is dropped
                 self._out[s].append(chunk)
                 st = self.stats[s]
+                if c is not None:
+                    st.concealed += 1
+                    st.concealed_frames += f
+                    continue
                 st.packets += 1
                 st.frames += f
                 st.bytes += HEADER_BYTES + len(p.payload)
@@ -908,10 +988,36 @@ class ReceiverSessionServer(_SessionSlots):
         self.step_times.append(time.time() - t0)
         return len(taken)
 
+    @staticmethod
+    def _conceal_rows(taken, frames, staged) -> np.ndarray:
+        """The (R, 5) adec_conceal_row descriptors (src, next, slot, j, den) of a step, one per zq row.  A real packet's rows read its
+        staged frames, and its last row stores the session's anchor.  A concealed packet's rows read the one staged frame after the gap
+        and the session's anchor (or none), with j counted on from where the gap's previous packets stopped."""
+        f = np.asarray(frames, dtype=np.int64)
+        if not any(t[3] for t in taken):                 # no concealment this step: row r reads staged frame r
+            rows = np.zeros((int(f.sum()), 5), dtype=np.int32)
+            rows[:, 0] = np.arange(rows.shape[0])
+            rows[:, 1:3] = -1
+            rows[np.cumsum(f) - 1, 2] = [t[0] for t in taken]
+            return rows
+        real = np.array([c is None for *_, c in taken])
+        first_j = np.array([0 if c is None else c[0] for *_, c in taken], dtype=np.int64)
+        den = np.array([0 if c is None else c[1] for *_, c in taken], dtype=np.int64)
+        slot = np.array([s if c is None else c[2] for s, *_, c in taken], dtype=np.int64)
+        k = np.arange(int(f.sum())) - np.repeat(np.cumsum(f) - f, f)          # row within its packet
+        real_r, base = np.repeat(real, f), np.repeat(np.asarray(staged, dtype=np.int64), f)
+        rows = np.empty((k.size, 5), dtype=np.int32)
+        rows[:, 0] = np.where(real_r, base + k, -1)
+        rows[:, 1] = np.where(real_r, -1, base)
+        rows[:, 2] = np.where(real_r & (k != np.repeat(f - 1, f)), -1, np.repeat(slot, f))
+        rows[:, 3] = np.where(real_r, 0, np.repeat(first_j, f) + k)
+        rows[:, 4] = np.repeat(den, f)
+        return rows
+
     def statistics(self) -> Dict:
         """steps, ms per step (mean, std), the open sessions, packets for sessions that were not open, and per open session: packets,
-        frames, duplicates, reorders, losses and the wire kbps received (packet bytes, headers included, over the seconds of audio
-        decoded)."""
+        frames, duplicates, reorders, losses, concealed packets and frames, and the wire kbps received (real packet bytes, headers
+        included, over the seconds of real audio decoded)."""
         with self._lock:
             per = {sid: self.stats[s].as_dict(self.sample_rate) for sid, s in sorted(self._ids.items())}
         return {"capacity": self.capacity, "open_sessions": len(per), "steps": len(self.step_times), "step_ms": _ms(self.step_times),

@@ -258,6 +258,30 @@ int adec_range_error(adec_handle *h, void *stream);
 int adec_lookup_bf16(adec_handle *h, const int64_t *idx, int B, int F, uint16_t *zq, void *stream);
 int adec_lookup_packed_bf16(adec_handle *h, const uint8_t *packed, int B, int F, uint16_t *zq, void *stream);
 
+/* -- loss concealment on the packed lookup ------------------------------------------------------------------------------------------
+ * One output row of adec_lookup_packed_conceal.  A real row (src >= 0) is the lookup of packed frame src, bit for bit
+ * adec_lookup_packed's; with slot >= 0 its fp32 sum is also stored in anchors[slot] (a session's last real frame of the call).  A
+ * concealed row (src = -1) stands for a lost frame: with s_b the fp32 sum of packed frame `next` (the first frame after the loss) and
+ * a = anchors[slot] (the session's last real frame before it), zq = fl(fl(fl(j / den) * fl(s_b - a)) + a) in fp32, every operation
+ * rounded to nearest on its own (no contraction); slot = -1 means no anchor and zq = s_b.  j counts the lost frames from 1 and den is
+ * their number plus one. */
+typedef struct adec_conceal_row {
+    int32_t src;   /* real row: packed frame in [0, F); -1 for a concealed row */
+    int32_t next;  /* concealed row: packed frame in [0, F) after the loss; -1 for a real row */
+    int32_t slot;  /* anchor row in [0, n_anchors), or -1: written by a real row, read by a concealed one */
+    int32_t j;     /* concealed row: 1 <= j < den (ignored for a real row) */
+    int32_t den;   /* concealed row: >= 2 (ignored for a real row) */
+} adec_conceal_row;
+/* packed (F, bytes) and anchors (n_anchors, code_dim) fp32, 16-byte aligned, are device buffers; rows (R) is a HOST array, checked
+ * before anything runs (an error names the field: src / next / slot out of range, den < 2, j outside [1, den), an anchor that one row
+ * reads and another writes, or that two rows write) and uploaded in stream order; zq (R, code_dim).  One launch.  Full symAD handle
+ * only; an out-of-range code index sets the flag adec_index_error reads.  _bf16: zq is bf16, the fp32 result rounded once to nearest
+ * even (as adec_lookup_packed_bf16); the anchors stay fp32. */
+int adec_lookup_packed_conceal(adec_handle *h, const uint8_t *packed, int F, const adec_conceal_row *rows, int R, float *anchors,
+                               int n_anchors, float *zq, void *stream);
+int adec_lookup_packed_conceal_bf16(adec_handle *h, const uint8_t *packed, int F, const adec_conceal_row *rows, int R, float *anchors,
+                                    int n_anchors, uint16_t *zq, void *stream);
+
 /* number of kernel launches issued by this handle since creation (bench.py's gpu_launches) */
 int64_t adec_launch_count(const adec_handle *h);
 
