@@ -60,6 +60,12 @@ class AdecConcealRow(ctypes.Structure):
                 ("den", ctypes.c_int32)]
 
 
+class AdecPlayoutRow(ctypes.Structure):
+    """struct adec_playout_row (include/audiodec_b200.h): one output row of adec_lookup_packed_playout."""
+    _fields_ = [("src", ctypes.c_int32), ("next", ctypes.c_int32), ("target", ctypes.c_int32), ("slot", ctypes.c_int32),
+                ("j", ctypes.c_int32), ("den", ctypes.c_int32)]
+
+
 TEST_CONV, TEST_RU, TEST_CONVTR, TEST_STEM, TEST_HEAD = 0, 1, 2, 3, 4
 TEST_REC = 9
 
@@ -85,6 +91,10 @@ SYMBOLS = {
     "adec_lookup_packed_conceal": (c_int, [c_void_p, c_void_p, c_int, ctypes.POINTER(AdecConcealRow), c_int, c_void_p, c_int, c_void_p,
                                            c_void_p]),
     "adec_lookup_packed_conceal_bf16": (c_int, [c_void_p, c_void_p, c_int, ctypes.POINTER(AdecConcealRow), c_int, c_void_p, c_int,
+                                                c_void_p, c_void_p]),
+    "adec_lookup_packed_playout": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p,
+                                           c_void_p]),
+    "adec_lookup_packed_playout_bf16": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int,
                                                 c_void_p, c_void_p]),
     "adec_graph_create": (c_int, [c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, ctypes.POINTER(c_void_p)]),
     "adec_graph_launch": (c_int, [c_void_p, c_void_p]),

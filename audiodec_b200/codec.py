@@ -663,6 +663,58 @@ class SymADStreamGenerator(_SymADTransmitter):
                   anchors.size(0), _ptr(zq), self._stream()), self._h)
         return zq
 
+    def lookup_packed_playout(self, packed, rows, anchors, targets, dtype=torch.float32):
+        """The packed lookup of a receiver's playout clock, in ONE launch (adec_lookup_packed_playout): uint8 packed frames (F, bytes)
+        or (1, F, bytes), F = 0 allowed, and one descriptor per output row -> zq (1, R, D).  rows: R rows of (src, next, target, slot,
+        j, den) ints: an (R, 6) int32 array (it may be a page-locked buffer, which must then stay unchanged until the stream has run the
+        call), or a sequence of 6-tuples; checked before anything runs.  A real row (src >= 0) and an interpolated row (src = -1,
+        next >= 0) are lookup_packed_conceal's rows.  A fade row (src = next = -1) is t = targets[target] when j >= den or slot = -1,
+        and otherwise fl(fl(fl(j / den) * fl(t - a)) + a) with a = anchors[slot].  anchors: a contiguous float32 (n_anchors, code_dim)
+        device tensor, updated in place; targets: a contiguous float32 (n_targets, code_dim) device tensor.  dtype=torch.bfloat16: bf16
+        zq, the fp32 result rounded once."""
+        self._ready()
+        what = "lookup_packed_playout"
+        packed = self._in(packed, torch.uint8)
+        if packed.dim() == 3 and packed.size(0) == 1:
+            packed = packed[0]
+        if packed.dim() != 2 or packed.size(1) != self.packed_frame_bytes():
+            raise RuntimeError(f"audiodec_b200: {what}: expected (F, {self.packed_frame_bytes()}) packed frames, got {tuple(packed.shape)}")
+        for name, t in (("anchors", anchors), ("targets", targets)):
+            if not isinstance(t, torch.Tensor) or t.device != self._device or t.dtype != torch.float32 or t.dim() != 2 or \
+                    t.size(1) != self.code_dim or not t.is_contiguous():
+                raise RuntimeError(f"audiodec_b200: {what}: {name} must be a contiguous float32 (n, {self.code_dim}) tensor on "
+                                   f"{self._device}")
+        if isinstance(rows, torch.Tensor):
+            rows = rows.numpy()
+        desc = np.ascontiguousarray(rows, dtype=np.int32)
+        if desc.ndim != 2 or desc.shape[1] != 6:
+            raise ValueError(f"audiodec_b200: {what}: rows must be (R, 6) (src, next, target, slot, j, den), got {desc.shape}")
+        r = desc.shape[0]
+        fn = self._lookup_fn("adec_lookup_packed_playout", dtype)
+        zq = torch.empty(1, r, self.code_dim, device=self._device, dtype=dtype)
+        _check(fn(self._h, _ptr(packed) if packed.size(0) else None, packed.size(0), ctypes.c_void_p(desc.ctypes.data), r, _ptr(anchors),
+                  anchors.size(0), _ptr(targets), targets.size(0), _ptr(zq), self._stream()), self._h)
+        return zq
+
+    def silence_frame(self, receptive_length=8192):
+        """The codec's silence frame, a (code_dim,) float32 device tensor: the lookup sum of the RVQ code of the last frame of
+        encode_offline on `receptive_length` zeros (rounded up to a hop multiple), i.e. quantize_offline(encode_offline(zeros))[0][0, :, -1].
+        A playout receiver fades toward it when a session's packets stop.  The encoder runs on a scratch encoder-only handle with this
+        generator's config and weights (bit for bit this handle's encode in fp32), so no stream of this generator is touched."""
+        self._ready()
+        enc = SymADEncoderStreamGenerator.__new__(SymADEncoderStreamGenerator)
+        _StreamGeneratorBase.__init__(enc)
+        ctypes.memmove(ctypes.addressof(enc._cfg), ctypes.addressof(self._cfg), ctypes.sizeof(self._cfg))
+        enc._cfg.model_type = _lib.MODEL_SYMAD_ENCODER
+        enc.input_channels, enc.code_dim, enc.codebook_num, enc.enc_strides = \
+            self.input_channels, self.code_dim, self.codebook_num, self.enc_strides
+        enc._sd = self._sd
+        enc.to(self._device)
+        hop = self._lib.adec_hop_length(self._h)
+        t = -(-receptive_length // hop) * hop
+        idx = enc.quantize_offline(enc.encode_offline(torch.zeros(1, self.input_channels, t, device=self._device)))   # (Nq, 1, F)
+        return self.lookup(idx[:, 0, -1:].contiguous())[0, 0]
+
     def _lookup_fn(self, name, dtype):
         if dtype not in (torch.float32, torch.bfloat16):
             raise NotImplementedError(f"audiodec_b200: {name[5:]}: zq is float32 or bfloat16, not {dtype}")

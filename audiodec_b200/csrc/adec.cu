@@ -280,6 +280,7 @@ struct adec_handle {
     DevBuf vl_tab;                // varlen row tables of the last call (ints)
     DevBuf mom_tab;               // row offsets of the last adec_zq_moments call (ints)
     DevBuf conceal_tab;           // row descriptors of the last adec_lookup_packed_conceal call (adec_conceal_row)
+    DevBuf playout_tab;           // row descriptors of the last adec_lookup_packed_playout call (adec_playout_row)
     SlotBits enc_slots, dec_slots;
     DevBuf slot_tab;              // stream pairs of the last state copy (ints)
     // the state map: every reference pad_buffer the handle runs, in plan order (encoder ops, then decoder ops), one stream's exported
@@ -1475,7 +1476,8 @@ void adec_destroy(adec_handle* h) {
         for (Op& op : *ops)
             for (int i = 0; i < 2; ++i) if (op.st[i]) cudaFree(op.st[i]);
     for (auto& b : h->ws) if (b.p) cudaFree(b.p);
-    for (DevBuf* b : {&h->hx, &h->hz, &h->hzq, &h->hy, &h->vl_tab, &h->mom_tab, &h->conceal_tab, &h->slot_tab, &h->st_tab}) if (b->p) cudaFree(b->p);
+    for (DevBuf* b : {&h->hx, &h->hz, &h->hzq, &h->hy, &h->vl_tab, &h->mom_tab, &h->conceal_tab, &h->playout_tab,
+                      &h->slot_tab, &h->st_tab}) if (b->p) cudaFree(b->p);
     if (h->hidx) cudaFree(h->hidx);
     if (h->d_err) cudaFree(h->d_err);
     if (h->d_ktrace) cudaFree(h->d_ktrace);
@@ -2076,6 +2078,84 @@ int adec_lookup_packed_conceal(adec_handle* h, const uint8_t* packed, int F, con
 int adec_lookup_packed_conceal_bf16(adec_handle* h, const uint8_t* packed, int F, const adec_conceal_row* rows, int R, float* anchors,
                                     int n_anchors, uint16_t* zq, void* stream) {
     return conceal_common(h, packed, F, rows, R, anchors, n_anchors, zq, true, stream);
+}
+
+static_assert(sizeof(adec_playout_row) == sizeof(PlayoutRow), "adec_playout_row and PlayoutRow must share a layout");
+
+// conceal_common with the fade row kind; every descriptor is checked before anything is enqueued
+static int playout_common(adec_handle* h, const uint8_t* packed, int F, const adec_playout_row* rows, int R, float* anchors,
+                          int n_anchors, const float* targets, int n_targets, void* zq, bool bf16, void* stream) {
+    if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
+    const std::string what = bf16 ? "lookup_packed_playout_bf16" : "lookup_packed_playout";
+    if (need_full_symad(h, what)) return 1;
+    if (F < 0 || R < 1) return h->fail(what + ": empty input (F must be >= 0 and R >= 1)");
+    if (n_anchors < 0 || n_targets < 0) return h->fail(what + ": n_anchors and n_targets must be >= 0");
+    if ((F > 0 && !packed) || !rows || !zq) return h->fail(what + ": packed (when F > 0), rows and zq must be given");
+    if (n_anchors > 0 && (!anchors || (uintptr_t)anchors % 16)) return h->fail(what + ": anchors must be a 16-byte aligned device buffer");
+    if (n_targets > 0 && (!targets || (uintptr_t)targets % 16)) return h->fail(what + ": targets must be a 16-byte aligned device buffer");
+    if (bf16 && (h->cfg.code_dim % 8 || (uintptr_t)zq % 16))
+        return h->fail(what + ": needs code_dim % 8 == 0 and a 16-byte aligned zq");
+    std::vector<int> reader(n_anchors, -1), writer(n_anchors, -1);     // per anchor slot: a row that reads it, a row that writes it
+    for (int r = 0; r < R; ++r) {
+        const adec_playout_row& d = rows[r];
+        const bool real = d.src >= 0, fade = d.src == -1 && d.next == -1;
+        if (real && d.src >= F) return h->fail(fmt("%s: rows[%d].src = %d is out of range [0, %d)", what.c_str(), r, d.src, F));
+        if (real && d.next != -1) return h->fail(fmt("%s: rows[%d].next = %d: a real row (src >= 0) has next = -1", what.c_str(), r, d.next));
+        if (!real && d.src != -1) return h->fail(fmt("%s: rows[%d].src = %d is out of range: a frame in [0, %d) or -1", what.c_str(), r, d.src, F));
+        if (!real && !fade && (d.next < 0 || d.next >= F))
+            return h->fail(fmt("%s: rows[%d].next = %d is out of range: a frame in [0, %d) or -1", what.c_str(), r, d.next, F));
+        if (!fade && d.target != -1)
+            return h->fail(fmt("%s: rows[%d].target = %d: only a fade row (src = next = -1) has a target", what.c_str(), r, d.target));
+        if (fade && (d.target < 0 || d.target >= n_targets))
+            return h->fail(fmt("%s: rows[%d].target = %d is out of range [0, %d)", what.c_str(), r, d.target, n_targets));
+        if (!real && !fade && d.den < 2)
+            return h->fail(fmt("%s: rows[%d].den = %d: an interpolated row needs den >= 2", what.c_str(), r, d.den));
+        if (!real && !fade && (d.j < 1 || d.j >= d.den))
+            return h->fail(fmt("%s: rows[%d].j = %d is outside [1, den = %d)", what.c_str(), r, d.j, d.den));
+        if (fade && d.den < 1) return h->fail(fmt("%s: rows[%d].den = %d: a fade row needs den >= 1", what.c_str(), r, d.den));
+        if (fade && d.j < 1) return h->fail(fmt("%s: rows[%d].j = %d: a fade row needs j >= 1", what.c_str(), r, d.j));
+        if (d.slot < -1 || d.slot >= n_anchors)
+            return h->fail(fmt("%s: rows[%d].slot = %d is out of range: an anchor in [0, %d) or -1", what.c_str(), r, d.slot, n_anchors));
+        if (d.slot < 0) continue;
+        std::vector<int>& mine = real ? writer : reader;
+        const std::vector<int>& other = real ? reader : writer;
+        if (other[d.slot] >= 0)
+            return h->fail(fmt("%s: rows[%d].slot = %d: anchor %d is read by row %d and written by row %d of the same call", what.c_str(), r,
+                               d.slot, d.slot, real ? other[d.slot] : r, real ? r : other[d.slot]));
+        if (real && mine[d.slot] >= 0)
+            return h->fail(fmt("%s: rows[%d].slot = %d: anchor %d is written by rows %d and %d of the same call", what.c_str(), r, d.slot,
+                               d.slot, mine[d.slot], r));
+        mine[d.slot] = r;
+    }
+    DeviceGuard dg(h->device);
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (ensure(h, h->playout_tab, (size_t)R * sizeof(adec_playout_row) / sizeof(float))) return 1;
+    // from a page-locked `rows` this copy is asynchronous: the header asks the caller to keep the buffer until the stream gets here
+    CK(h, cudaMemcpyAsync(h->playout_tab.p, rows, (size_t)R * sizeof(adec_playout_row), cudaMemcpyHostToDevice, s));
+    PlayoutArgs c{};
+    LookupArgs& a = c.l;
+    a.packed = packed; a.nfr = R; a.nq = h->cfg.codebook_num; a.D = h->cfg.code_dim;
+    a.N = h->cfg.codebook_size; a.bits = index_bits(a.N); a.bpf = adec_packed_frame_bytes(h);
+    a.codebook = h->d_codebook; a.n_rows = (long long)h->cfg.codebook_num * h->cfg.codebook_size; a.zq = (float*)zq; a.err = h->d_err;
+    c.rows = reinterpret_cast<const PlayoutRow*>(h->playout_tab.p);
+    c.anchors = anchors;
+    c.targets = targets;
+    const long long nth = a.nfr * (a.D / 4);
+    if (bf16) lookup_conceal_kernel<true, true><<<(unsigned)((nth + 255) / 256), 256, 0, s>>>(c);
+    else lookup_conceal_kernel<false, true><<<(unsigned)((nth + 255) / 256), 256, 0, s>>>(c);
+    CK(h, cudaGetLastError());
+    ++h->launches;
+    return 0;
+}
+
+int adec_lookup_packed_playout(adec_handle* h, const uint8_t* packed, int F, const adec_playout_row* rows, int R, float* anchors,
+                               int n_anchors, const float* targets, int n_targets, float* zq, void* stream) {
+    return playout_common(h, packed, F, rows, R, anchors, n_anchors, targets, n_targets, zq, false, stream);
+}
+
+int adec_lookup_packed_playout_bf16(adec_handle* h, const uint8_t* packed, int F, const adec_playout_row* rows, int R, float* anchors,
+                                    int n_anchors, const float* targets, int n_targets, uint16_t* zq, void* stream) {
+    return playout_common(h, packed, F, rows, R, anchors, n_anchors, targets, n_targets, zq, true, stream);
 }
 
 int adec_codec_host(adec_handle* enc, adec_handle* dec, const float* x_host, int B, int T, int64_t* idx_host,

@@ -20,7 +20,8 @@
 //                       first-index arg-min by warp shuffles, int64 flat indices.
 //   lookup_kernel     - codebook gather-sum (fp32 zq, or bf16 zq rounded once).
 //   lookup_conceal_kernel - the packed lookup per row descriptor: real frames, plus concealed frames interpolated between a
-//                       session's last real frame (an fp32 anchor row) and the frame after a loss.
+//                       session's last real frame (an fp32 anchor row) and the frame after a loss; with PLAYOUT also fade
+//                       frames interpolated from the anchor toward a device target row (a receiver's playout clock).
 //   zq_moments_kernel - per-utterance fp64 sums and centred second moments of zq (corpus statistics).
 #pragma once
 #include <cuda_bf16.h>
@@ -955,15 +956,53 @@ struct ConcealArgs {
     float* anchors;                // (n_anchors, D) fp32, 16-byte aligned
 };
 
-template <bool BF16>
-__global__ void __launch_bounds__(256) lookup_conceal_kernel(const ConcealArgs c) {
+// PLAYOUT adds a third row kind, the fade row (src < 0 and next < 0): t = targets[target], a = anchors[slot]; zq[r] = t when
+// j >= den or slot < 0, otherwise fl(fl(fl(j / den) * fl(t - a)) + a).  A fade row reads no packed frame.  Real and interpolated rows
+// are the rows above, bit for bit.
+struct PlayoutRow {
+    int src, next, target, slot, j, den;   // adec_playout_row
+};
+
+struct PlayoutArgs {
+    LookupArgs l;                  // as ConcealArgs; l.packed may be null when every row fades
+    const PlayoutRow* rows;        // (l.nfr)
+    float* anchors;                // (n_anchors, D) fp32, 16-byte aligned
+    const float* targets;          // (n_targets, D) fp32, 16-byte aligned
+};
+
+template <bool PLAYOUT> struct ConcealKind { using Args = ConcealArgs; };
+template <> struct ConcealKind<true> { using Args = PlayoutArgs; };
+
+template <bool BF16, bool PLAYOUT = false>
+__global__ void __launch_bounds__(256) lookup_conceal_kernel(const typename ConcealKind<PLAYOUT>::Args c) {
     const LookupArgs& a = c.l;
     const int vpf = a.D / 4;
     const long long gid = (long long)blockIdx.x * 256 + threadIdx.x;
     if (gid >= a.nfr * vpf) return;
     const long long r = gid / vpf;
     const int k4 = (int)(gid - r * vpf) * 4;
-    const ConcealRow d = c.rows[r];
+    if constexpr (PLAYOUT) {
+        const PlayoutRow* row = c.rows + r;
+        if (row->src < 0 && row->next < 0) {           // fade row
+            float4 s = __ldg(reinterpret_cast<const float4*>(c.targets + (long long)row->target * a.D + k4));
+            const int slot = row->slot, j = row->j, den = row->den;
+            if (slot >= 0 && j < den) {
+                const float4 av = *reinterpret_cast<const float4*>(c.anchors + (long long)slot * a.D + k4);
+                const float w = __fdiv_rn((float)j, (float)den);
+                s.x = __fadd_rn(__fmul_rn(w, __fsub_rn(s.x, av.x)), av.x);
+                s.y = __fadd_rn(__fmul_rn(w, __fsub_rn(s.y, av.y)), av.y);
+                s.z = __fadd_rn(__fmul_rn(w, __fsub_rn(s.z, av.z)), av.z);
+                s.w = __fadd_rn(__fmul_rn(w, __fsub_rn(s.w, av.w)), av.w);
+            }
+            if constexpr (BF16)
+                *reinterpret_cast<uint2*>(reinterpret_cast<uint16_t*>(a.zq) + r * a.D + k4) =
+                    make_uint2(bf2_bits(s.x, s.y), bf2_bits(s.z, s.w));
+            else
+                *reinterpret_cast<float4*>(a.zq + r * a.D + k4) = s;
+            return;
+        }
+    }
+    const auto d = c.rows[r];
     const bool real = d.src >= 0;
     const unsigned char* in = a.packed + (long long)(real ? d.src : d.next) * a.bpf;
     const unsigned long long mask = (1ull << a.bits) - 1ull;

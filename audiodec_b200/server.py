@@ -279,9 +279,12 @@ class SessionState:
     yet.  On the split servers also the session's wire id and the next sequence number it sends or expects.  On a ReceiverSessionServer
     that conceals losses also the fp32 anchor row (the lookup sum of the session's last real frame, a (code_dim,) device tensor, None
     before its first real frame) and the concealment still pending, (packets left, frames per packet, frames concealed so far, frames in
-    the gap), or None."""
+    the gap), or None.  On a ReceiverSessionServer with a playout clock also `playout`, a dict of the playout position: whether the
+    session is playing, the steps each held packet has waited (in the order of `inputs`), the frames concealed or faded since the last
+    real frame, the consecutive fade packets, the last real packet's frame count and the sequence numbers given up by the clock; None
+    elsewhere."""
 
-    def __init__(self, layouts, states, inputs, outputs, session_id=None, seq=0, anchor=None, conceal=None):
+    def __init__(self, layouts, states, inputs, outputs, session_id=None, seq=0, anchor=None, conceal=None, playout=None):
         self.layouts: List[list] = layouts
         self.states: List[torch.Tensor] = states
         self.inputs: list = inputs
@@ -290,11 +293,12 @@ class SessionState:
         self.seq: int = seq
         self.anchor: Optional[torch.Tensor] = anchor
         self.conceal: Optional[Tuple[int, int, int, int]] = conceal
+        self.playout: Optional[dict] = playout
 
     def to(self, device) -> "SessionState":
         """A copy with the states and the anchor on `device` (the frames are host arrays and are shared)."""
         return SessionState(self.layouts, [t.to(device) for t in self.states], list(self.inputs), list(self.outputs), self.session_id,
-                            self.seq, None if self.anchor is None else self.anchor.to(device), self.conceal)
+                            self.seq, None if self.anchor is None else self.anchor.to(device), self.conceal, self.playout)
 
 
 class _SessionSlots:
@@ -729,12 +733,20 @@ class ReceiveStats:
         self.losses = 0            # sequence numbers given up as lost
         self.concealed = 0         # lost sequence numbers decoded as concealed packets (conceal_packets > 0)
         self.concealed_frames = 0  # code frames of those packets
+        self.late = 0              # packets dropped because the playout clock had given their sequence number up (playout_delay)
+        self.underruns = 0         # playout steps with nothing held: a fade packet was played
+        self.faded_frames = 0      # code frames of those fade packets
+        self.pauses = 0            # times the session stopped playing after max_fade_packets fade packets in a row
 
-    def as_dict(self, sample_rate):
-        """packets, frames and wire_kbps count the real packets only"""
-        return {"packets": self.packets, "frames": self.frames, "duplicates": self.duplicates, "reorders": self.reorders,
-                "losses": self.losses, "concealed": self.concealed, "concealed_frames": self.concealed_frames,
-                "wire_kbps": 8e-3 * self.bytes / (self.samples / sample_rate) if self.samples else None}
+    def as_dict(self, sample_rate, buffered=None):
+        """packets, frames and wire_kbps count the real packets only; buffered (the packets held ahead of the playout point) adds the
+        playout counters"""
+        out = {"packets": self.packets, "frames": self.frames, "duplicates": self.duplicates, "reorders": self.reorders,
+               "losses": self.losses, "concealed": self.concealed, "concealed_frames": self.concealed_frames,
+               "wire_kbps": 8e-3 * self.bytes / (self.samples / sample_rate) if self.samples else None}
+        if buffered is not None:
+            out.update(late=self.late, underruns=self.underruns, faded_frames=self.faded_frames, pauses=self.pauses, buffered=buffered)
+        return out
 
 
 class ReceiverSessionServer(_SessionSlots):
@@ -770,17 +782,48 @@ class ReceiverSessionServer(_SessionSlots):
     PCM back in ONE copy.  With concealment the lookup is ONE ``lookup_packed_conceal`` instead, which also keeps every session's
     anchor row (a (capacity, code_dim) fp32 device tensor); a session that conceals this step stages b's first frame in place of a
     payload.  ``poll(session_id)`` returns the session's next decoded frame (frames x hop float32 samples) or None.  ``detach`` /
-    ``attach`` also carry the anchor row and any concealment still pending; a receiver without concealment drops them."""
+    ``attach`` also carry the anchor row and any concealment still pending; a receiver without concealment drops them.
+
+    ``playout_delay = D`` (None, the default, is the receiver above) runs a playout clock instead: a fixed-delay jitter buffer in which
+    ``step()`` is one packet period, ticked by the caller at the packet rate, and every playing session gets exactly one packet of PCM
+    per step.  ``submit_packet`` stamps a packet with the steps completed so far; one whose sequence number the session has decoded or
+    holds is a duplicate, one the clock has already given up is ``late``; both are dropped, and nothing is given up for the reorder
+    window.  A session starts playing at the first step where it holds a packet stamped at least D steps earlier.  Then, each step:
+    (1) the next packet is held: it is decoded.  (2) It is missing but a later packet m is held: one loss, and the next packet is
+    concealed as m.frames frames interpolated from the anchor (the session's last real frame) toward m's first frame, j = c + 1 ...
+    c + m.frames and den = c + (m - next) * m.frames + 1, where c counts the frames concealed or faded since the last real frame (m's
+    first frame itself with no anchor).  (3) Nothing is held: an underrun, played as a fade packet of the last real packet's frame
+    count (frames_per_packet before any) whose frames go from the anchor toward the codec's silence frame, j = c + 1 ... and
+    den = ``fade_frames``, the silence frame itself from j >= den on.  Rules 2 and 3 give the sequence number up.  After
+    ``max_fade_packets`` fade packets in a row the session pauses: it goes back to buffering and rewinds to the first sequence number
+    the fades gave up, so a sender that went quiet resumes at its own next packet; the decoder state runs on through the fade.  Each
+    step is ONE ``lookup_packed_playout`` over real, interpolated and fade rows (descriptors in two page-locked tables used in turn)
+    and ONE ``decode_streams``.  The silence frame is ``rx_encoder.silence_frame()`` unless ``silence_frame`` gives one.  This is a
+    continuity and timing rule: it keeps every session's output running at the packet rate; how the concealed and faded audio sounds
+    is not claimed.  ``detach`` / ``attach`` carry the playout position (SessionState.playout) between playout receivers; a session
+    cannot move between a playout receiver and one without."""
 
     _noun = "session"
     reorder_window = 4                 # packets held behind a missing one before it is given up
 
     def __init__(self, rx_encoder, decoder, capacity: int, frames_per_packet: int, sample_rate: int = 48000, device=None,
-                 conceal_packets: int = 0):
+                 conceal_packets: int = 0, playout_delay: Optional[int] = None, fade_frames: Optional[int] = None,
+                 max_fade_packets: int = 4, silence_frame=None):
         if frames_per_packet < 1:
             raise ValueError("frames_per_packet must be >= 1")
         if conceal_packets < 0:
             raise ValueError("conceal_packets must be >= 0")
+        if playout_delay is not None:
+            if conceal_packets:
+                raise ValueError("playout_delay and conceal_packets > 0 exclude each other: the playout clock conceals by itself")
+            if playout_delay < 0:
+                raise ValueError("playout_delay must be >= 0")
+            fade_frames = 2 * frames_per_packet if fade_frames is None else fade_frames
+            if fade_frames < 1:
+                raise ValueError("fade_frames must be >= 1")
+            if max_fade_packets < 1:
+                raise ValueError("max_fade_packets must be >= 1")
+        self.playout_delay, self.fade_frames, self.max_fade_packets = playout_delay, fade_frames, max_fade_packets
         self.rx_encoder, self.decoder = rx_encoder, decoder
         self.frames_per_packet, self.sample_rate = frames_per_packet, sample_rate
         self.conceal_packets = conceal_packets
@@ -800,9 +843,31 @@ class ReceiverSessionServer(_SessionSlots):
         self._y_host = None                            # the PCM of a step, sized on the first step
         # concealment: per slot the fp32 lookup sum of the last real frame decoded, whether there is one, and the pending plan
         # [packets left, frames per packet, frames concealed so far, frames in the gap]
-        self._anchors = torch.zeros(capacity, rx_encoder.code_dim, dtype=torch.float32, device=self.device) if conceal_packets else None
+        self._anchors = torch.zeros(capacity, rx_encoder.code_dim, dtype=torch.float32, device=self.device) \
+            if conceal_packets or playout_delay is not None else None
         self._has_anchor = [False] * capacity
         self._plan: List[Optional[list]] = [None] * capacity
+        # playout: steps completed; per slot the arrival stamp of each held packet, whether it plays, the frames concealed or faded
+        # since its last real frame, its consecutive fade packets, its last real packet's frame count and the sequence numbers the
+        # clock gave up (a later arrival of one is late)
+        self._steps = 0
+        self._stamp: List[Dict[int, int]] = [{} for _ in range(capacity)]
+        self._playing = [False] * capacity
+        self._c = [0] * capacity
+        self._fades = [0] * capacity
+        self._last_frames: List[Optional[int]] = [None] * capacity
+        self._given_up: List[set] = [set() for _ in range(capacity)]
+        if playout_delay is not None:
+            sf = rx_encoder.silence_frame() if silence_frame is None else silence_frame
+            sf = torch.as_tensor(sf, dtype=torch.float32).to(self.device)
+            if sf.numel() != rx_encoder.code_dim:
+                raise ValueError(f"silence_frame has {sf.numel()} values, the codec's frames have {rx_encoder.code_dim}")
+            self._targets = sf.reshape(1, -1).contiguous()
+            # the descriptors of a step go through two page-locked (R_max, 6) tables used in turn
+            r_max = capacity * frames_per_packet
+            self._rows_host = [_pinned(r_max * 6, torch.int32, self.device).view(r_max, 6) for _ in range(2)]
+            self._rows_np = [t.numpy() for t in self._rows_host]
+            self._rows_turn = 0
 
     def _reset_slot(self, s):
         self._held[s].clear()
@@ -811,8 +876,18 @@ class ReceiverSessionServer(_SessionSlots):
         self.stats[s] = ReceiveStats()
         self._has_anchor[s] = False
         self._plan[s] = None
+        self._stamp[s].clear()
+        self._playing[s] = False
+        self._c[s] = self._fades[s] = 0
+        self._last_frames[s] = None
+        self._given_up[s] = set()
 
     def _export_slot(self, s):
+        if self.playout_delay is not None:
+            return {"anchor": self._anchors[s].clone() if self._has_anchor[s] else None,
+                    "playout": {"playing": self._playing[s], "waited": [self._steps - self._stamp[s][q] for q in sorted(self._held[s])],
+                                "c": self._c[s], "fades": self._fades[s], "last_frames": self._last_frames[s],
+                                "given_up": sorted(self._given_up[s])}}
         if not self.conceal_packets:
             return {}
         plan = self._plan[s]
@@ -828,7 +903,12 @@ class ReceiverSessionServer(_SessionSlots):
         self._held[s].update((p.seq, p) for p in state.inputs)
         self._next[s] = state.seq
         self._out[s].extend(state.outputs)
-        if self.conceal_packets:
+        if self.playout_delay is not None:
+            po = state.playout
+            self._stamp[s].update((p.seq, self._steps - w) for p, w in zip(state.inputs, po["waited"]))
+            self._playing[s], self._c[s], self._fades[s] = po["playing"], po["c"], po["fades"]
+            self._last_frames[s], self._given_up[s] = po["last_frames"], set(po["given_up"])
+        if self.conceal_packets or self.playout_delay is not None:
             if state.anchor is not None:
                 self._anchors[s].copy_(state.anchor)
                 self._has_anchor[s] = True
@@ -857,6 +937,10 @@ class ReceiverSessionServer(_SessionSlots):
         The state must be on this server's device (SessionState.to)."""
         if state.session_id is None:
             raise ValueError("the session has no wire session id: it was not detached from a receiver server")
+        if (state.playout is None) != (self.playout_delay is None):
+            raise ValueError("a session moves between two receivers with a playout clock or two without: this one "
+                             + ("has one" if self.playout_delay is not None else "has none") + ", the session's had "
+                             + ("none" if state.playout is None else "one"))
         return self._attach_slot(state, state.session_id)
 
     @property
@@ -890,13 +974,19 @@ class ReceiverSessionServer(_SessionSlots):
                 self.unknown_session_packets += 1
                 return False
             held, st = self._held[s], self.stats[s]
+            if self.playout_delay is not None and p.seq in self._given_up[s]:
+                st.late += 1
+                return False
             if p.seq < self._next[s] or p.seq in held:
                 st.duplicates += 1
                 return False
             if any(q > p.seq for q in held):
                 st.reorders += 1
             held[p.seq] = p
-            self._give_up_gap(s)
+            if self.playout_delay is not None:
+                self._stamp[s][p.seq] = self._steps
+            else:
+                self._give_up_gap(s)
             return True
 
     def poll(self, session_id: int) -> Optional[np.ndarray]:
@@ -910,6 +1000,8 @@ class ReceiverSessionServer(_SessionSlots):
         """Decode the next in-order packet of every open session that has one, or its next concealed packet.  Returns the number of
         packets decoded, concealed ones included."""
         with self._step_lock:
+            if self.playout_delay is not None:
+                return self._playout_step()
             return self._step()
 
     def _step(self) -> int:
@@ -1014,11 +1106,140 @@ class ReceiverSessionServer(_SessionSlots):
         rows[:, 4] = np.repeat(den, f)
         return rows
 
+    def _playout_plan(self, s) -> Optional[tuple]:
+        """What playing slot s plays this step, with _lock held: (kind, packet or None, frames, j of the first row, den); kind 0 is a
+        real packet, 1 an interpolated packet toward held packet m (the packet), 2 a fade packet.  Updates the slot's position and
+        counters, pauses it after max_fade_packets fades."""
+        held, st, nxt, c = self._held[s], self.stats[s], self._next[s], self._c[s]
+        p = held.pop(nxt, None)
+        self._next[s] = nxt + 1
+        if p is not None:                                              # rule 1
+            del self._stamp[s][nxt]
+            self._c[s] = self._fades[s] = 0
+            self._last_frames[s] = p.frames
+            return 0, p, p.frames, 0, 0
+        self._given_up[s].add(nxt)
+        if held:                                                       # rule 2
+            m = min(held)
+            f = held[m].frames
+            st.losses += 1
+            st.concealed += 1
+            st.concealed_frames += f
+            self._c[s] = c + f
+            self._fades[s] = 0
+            return 1, held[m], f, c + 1, c + (m - nxt) * f + 1
+        f = self._last_frames[s] or self.frames_per_packet             # rule 3
+        st.underruns += 1
+        st.faded_frames += f
+        self._c[s] = c + f
+        self._fades[s] += 1
+        if self._fades[s] == self.max_fade_packets:                    # pause: back to buffering, rewound past the fades
+            st.pauses += 1
+            self._playing[s] = False
+            self._next[s] -= self.max_fade_packets
+            self._given_up[s].difference_update(range(self._next[s], self._next[s] + self.max_fade_packets))
+            self._fades[s] = 0
+        return 2, None, f, c + 1, self.fade_frames
+
+    def _playout_step(self) -> int:
+        """One packet period of the playout clock: one packet of PCM for every playing session."""
+        t0 = time.time()
+        now, delay = self._steps, self.playout_delay
+        taken = []                                     # (slot, open counter, kind, packet, frames, first j, den, anchor slot or -1)
+        with self._lock:
+            for sid, s in sorted(self._ids.items()):
+                if s not in self._open:
+                    continue
+                if not self._playing[s]:
+                    if not any(now - t >= delay for t in self._stamp[s].values()):
+                        continue
+                    self._playing[s] = True
+                kind, p, f, j, den = self._playout_plan(s)
+                taken.append((s, self._session[s], kind, p, f, j, den, s if self._has_anchor[s] or kind == 0 else -1))
+                if kind == 0:
+                    self._has_anchor[s] = True
+            self._steps += 1
+        if not taken:
+            self.step_times.append(time.time() - t0)
+            return 0
+        nb = self.frame_bytes
+        o = 0
+        staged = []                                    # per taken packet: its first frame in the staged bytes
+        for _, _, kind, p, *_ in taken:
+            staged.append(o // nb)
+            if kind == 2:
+                continue
+            n = len(p.payload) if kind == 0 else nb    # an interpolated packet stages only m's first frame
+            self._p_np[o:o + n] = np.frombuffer(p.payload, dtype=np.uint8, count=n)
+            o += n
+        frames = [t[4] for t in taken]
+        rows = self._playout_rows(taken, staged)
+        with torch.no_grad(), self._codec_lock:
+            packed = self._p_host[:o].to(self.device, non_blocking=True).view(o // nb, nb)
+            zq = self.rx_encoder.lookup_packed_playout(packed, rows, self._anchors, self._targets, **self._zq_kw)
+            ys = self.decoder.decode_streams(zq, frames, [t[0] for t in taken])
+            y = torch.cat([v.reshape(-1) for v in ys])
+            total = sum(frames)
+            hop = y.numel() // total
+            if self._y_host is None or self._y_host.dtype != y.dtype or self._y_host.numel() < y.numel():
+                self._y_host = _pinned(max(y.numel(), self.capacity * self.frames_per_packet * hop), y.dtype, self.device)
+            y_host = self._y_host[:y.numel()]
+            y_host.copy_(y, non_blocking=True)
+            if y.device.type == "cuda":
+                torch.cuda.current_stream(y.device).synchronize()
+        y_np = (y_host.float() if y_host.dtype == torch.bfloat16 else y_host.clone()).numpy()
+        with self._lock:
+            o = 0
+            for (s, session, kind, p, f, *_) in taken:
+                chunk = y_np[o * hop:(o + f) * hop]
+                o += f
+                if s not in self._open or self._session[s] != session:
+                    continue                        # closed while the step ran: the frame is dropped
+                self._out[s].append(chunk)
+                if kind == 0:
+                    st = self.stats[s]
+                    st.packets += 1
+                    st.frames += f
+                    st.bytes += HEADER_BYTES + len(p.payload)
+                    st.samples += chunk.size
+        self.step_times.append(time.time() - t0)
+        return len(taken)
+
+    def _playout_rows(self, taken, staged) -> np.ndarray:
+        """The (R, 6) adec_playout_row descriptors (src, next, target, slot, j, den) of a playout step, written into the next of the
+        two page-locked tables.  A real packet's rows read its staged frames and its last row stores the session's anchor; an
+        interpolated packet's rows read the one staged frame of m; a fade packet's rows read the silence frame (target 0).  The
+        step synchronises on its output before the table comes round again."""
+        table = self._rows_np[self._rows_turn]
+        self._rows_turn ^= 1
+        f = np.fromiter((t[4] for t in taken), dtype=np.int64, count=len(taken))
+        ends = np.cumsum(f)
+        rows = table[:int(ends[-1])]
+        if not any(t[2] for t in taken):               # every packet real: row r reads staged frame r
+            rows[:, 0] = np.arange(rows.shape[0])
+            rows[:, 1:4] = -1
+            rows[ends - 1, 3] = [t[0] for t in taken]
+            rows[:, 4:] = 0
+            return rows
+        kind = np.repeat(np.fromiter((t[2] for t in taken), dtype=np.int64, count=len(taken)), f)
+        k = np.arange(rows.shape[0]) - np.repeat(ends - f, f)                 # row within its packet
+        base = np.repeat(np.asarray(staged, dtype=np.int64), f)
+        real = kind == 0
+        rows[:, 0] = np.where(real, base + k, -1)
+        rows[:, 1] = np.where(kind == 1, base, -1)
+        rows[:, 2] = np.where(kind == 2, 0, -1)
+        rows[:, 3] = np.where(real & (k != np.repeat(f - 1, f)), -1, np.repeat([t[7] for t in taken], f))
+        rows[:, 4] = np.where(real, 0, np.repeat([t[5] for t in taken], f) + k)
+        rows[:, 5] = np.where(real, 0, np.repeat([t[6] for t in taken], f))
+        return rows
+
     def statistics(self) -> Dict:
         """steps, ms per step (mean, std), the open sessions, packets for sessions that were not open, and per open session: packets,
         frames, duplicates, reorders, losses, concealed packets and frames, and the wire kbps received (real packet bytes, headers
-        included, over the seconds of real audio decoded)."""
+        included, over the seconds of real audio decoded).  With a playout clock also late, underruns, faded_frames, pauses and
+        buffered (the packets held ahead of the playout point)."""
         with self._lock:
-            per = {sid: self.stats[s].as_dict(self.sample_rate) for sid, s in sorted(self._ids.items())}
+            po = self.playout_delay is not None
+            per = {sid: self.stats[s].as_dict(self.sample_rate, len(self._held[s]) if po else None) for sid, s in sorted(self._ids.items())}
         return {"capacity": self.capacity, "open_sessions": len(per), "steps": len(self.step_times), "step_ms": _ms(self.step_times),
                 "unknown_session_packets": self.unknown_session_packets, "per_session": per}

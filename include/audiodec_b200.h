@@ -282,6 +282,34 @@ int adec_lookup_packed_conceal(adec_handle *h, const uint8_t *packed, int F, con
 int adec_lookup_packed_conceal_bf16(adec_handle *h, const uint8_t *packed, int F, const adec_conceal_row *rows, int R, float *anchors,
                                     int n_anchors, uint16_t *zq, void *stream);
 
+/* -- the packed lookup of a receiver's playout clock -------------------------------------------------------------------------------
+ * One output row of adec_lookup_packed_playout.  Three kinds of row, in one launch:
+ *   real row (src >= 0, next = target = -1): adec_conceal_row's real row, bit for bit (with slot >= 0 it also stores the anchor);
+ *   interpolated row (src = -1, next >= 0, target = -1): adec_conceal_row's concealed row, bit for bit (1 <= j < den);
+ *   fade row (src = next = -1, target in [0, n_targets)): with t = targets[target] and a = anchors[slot],
+ *     zq = t when j >= den or slot = -1, and otherwise zq = fl(fl(fl(j / den) * fl(t - a)) + a) in fp32, every operation rounded to
+ *     nearest on its own (no contraction).  j >= 1 and den >= 1.  No packed frame is read.
+ * A receiver fades a session whose packets stopped toward the codec's silence frame (the target) over den frames. */
+typedef struct adec_playout_row {
+    int32_t src;     /* real row: packed frame in [0, F); -1 otherwise */
+    int32_t next;    /* interpolated row: packed frame in [0, F) after the loss; -1 otherwise */
+    int32_t target;  /* fade row: target row in [0, n_targets); -1 otherwise */
+    int32_t slot;    /* anchor row in [0, n_anchors), or -1: written by a real row, read by an interpolated or a fade row */
+    int32_t j;       /* interpolated row: 1 <= j < den; fade row: j >= 1 (ignored for a real row) */
+    int32_t den;     /* interpolated row: >= 2; fade row: >= 1 (ignored for a real row) */
+} adec_playout_row;
+/* packed (F, bytes; F = 0 and packed = NULL are allowed when no row reads a frame), anchors (n_anchors, code_dim) fp32 and targets
+ * (n_targets, code_dim) fp32, both 16-byte aligned, are device buffers; zq (R, code_dim).  rows (R) is a HOST array, checked before
+ * anything runs; an error names the field: src / next / target / slot out of range, a target on a row that is not a fade row, j or den
+ * outside their range for the row's kind, an anchor that one row reads and another writes, or that two rows write.  rows may be
+ * page-locked: the upload is then asynchronous, and the buffer must stay unchanged until the call's work on `stream` has completed
+ * (a pageable buffer may be reused as soon as the call returns).  One launch.  Full symAD handle only; an out-of-range code index sets
+ * the flag adec_index_error reads.  _bf16: zq is bf16, the fp32 result rounded once to nearest even; anchors and targets stay fp32. */
+int adec_lookup_packed_playout(adec_handle *h, const uint8_t *packed, int F, const adec_playout_row *rows, int R, float *anchors,
+                               int n_anchors, const float *targets, int n_targets, float *zq, void *stream);
+int adec_lookup_packed_playout_bf16(adec_handle *h, const uint8_t *packed, int F, const adec_playout_row *rows, int R, float *anchors,
+                                    int n_anchors, const float *targets, int n_targets, uint16_t *zq, void *stream);
+
 /* number of kernel launches issued by this handle since creation (bench.py's gpu_launches) */
 int64_t adec_launch_count(const adec_handle *h);
 
