@@ -61,7 +61,7 @@ class AdecConcealRow(ctypes.Structure):
 
 
 class AdecPlayoutRow(ctypes.Structure):
-    """struct adec_playout_row (include/audiodec_b200.h): one output row of adec_lookup_packed_playout."""
+    """struct adec_playout_row (include/audiodec_b200.h): one output row of adec_lookup_packed_playout / _timescale."""
     _fields_ = [("src", ctypes.c_int32), ("next", ctypes.c_int32), ("target", ctypes.c_int32), ("slot", ctypes.c_int32),
                 ("j", ctypes.c_int32), ("den", ctypes.c_int32)]
 
@@ -96,6 +96,10 @@ SYMBOLS = {
                                            c_void_p]),
     "adec_lookup_packed_playout_bf16": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int,
                                                 c_void_p, c_void_p]),
+    "adec_lookup_packed_timescale": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p,
+                                             c_void_p]),
+    "adec_lookup_packed_timescale_bf16": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int,
+                                                  c_void_p, c_void_p]),
     "adec_graph_create": (c_int, [c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, ctypes.POINTER(c_void_p)]),
     "adec_graph_launch": (c_int, [c_void_p, c_void_p]),
     "adec_graph_info": (c_int, [c_void_p, ctypes.POINTER(c_int), ctypes.POINTER(c_int), ctypes.POINTER(c_int)]),

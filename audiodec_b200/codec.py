@@ -672,8 +672,18 @@ class SymADStreamGenerator(_SymADTransmitter):
         and otherwise fl(fl(fl(j / den) * fl(t - a)) + a) with a = anchors[slot].  anchors: a contiguous float32 (n_anchors, code_dim)
         device tensor, updated in place; targets: a contiguous float32 (n_targets, code_dim) device tensor.  dtype=torch.bfloat16: bf16
         zq, the fp32 result rounded once."""
+        return self._lookup_playout("lookup_packed_playout", packed, rows, anchors, targets, dtype)
+
+    def lookup_packed_timescale(self, packed, rows, anchors, targets, dtype=torch.float32):
+        """The packed lookup of an adaptive playout clock, in ONE launch (adec_lookup_packed_timescale): lookup_packed_playout's
+        arguments and rows, bit for bit, plus two row kinds that start from packed frame src of the same call (slot = -1) rather than
+        an anchor, with s_x the fp32 sum of packed frame x.  A between row (src >= 0, next >= 0, target = -1, 1 <= j < den) is
+        fl(fl(fl(j / den) * fl(s_next - s_src)) + s_src).  A frame-started fade (src >= 0, next = -1, target >= 0) is the fade row with
+        a = s_src.  Both equal the anchor-read row of a later call, since a real row of frame src stores s_src as its anchor."""
+        return self._lookup_playout("lookup_packed_timescale", packed, rows, anchors, targets, dtype)
+
+    def _lookup_playout(self, what, packed, rows, anchors, targets, dtype):
         self._ready()
-        what = "lookup_packed_playout"
         packed = self._in(packed, torch.uint8)
         if packed.dim() == 3 and packed.size(0) == 1:
             packed = packed[0]
@@ -690,7 +700,7 @@ class SymADStreamGenerator(_SymADTransmitter):
         if desc.ndim != 2 or desc.shape[1] != 6:
             raise ValueError(f"audiodec_b200: {what}: rows must be (R, 6) (src, next, target, slot, j, den), got {desc.shape}")
         r = desc.shape[0]
-        fn = self._lookup_fn("adec_lookup_packed_playout", dtype)
+        fn = self._lookup_fn("adec_" + what, dtype)
         zq = torch.empty(1, r, self.code_dim, device=self._device, dtype=dtype)
         _check(fn(self._h, _ptr(packed) if packed.size(0) else None, packed.size(0), ctypes.c_void_p(desc.ctypes.data), r, _ptr(anchors),
                   anchors.size(0), _ptr(targets), targets.size(0), _ptr(zq), self._stream()), self._h)

@@ -280,7 +280,7 @@ struct adec_handle {
     DevBuf vl_tab;                // varlen row tables of the last call (ints)
     DevBuf mom_tab;               // row offsets of the last adec_zq_moments call (ints)
     DevBuf conceal_tab;           // row descriptors of the last adec_lookup_packed_conceal call (adec_conceal_row)
-    DevBuf playout_tab;           // row descriptors of the last adec_lookup_packed_playout call (adec_playout_row)
+    DevBuf playout_tab;           // row descriptors of the last adec_lookup_packed_playout / _timescale call (adec_playout_row)
     SlotBits enc_slots, dec_slots;
     DevBuf slot_tab;              // stream pairs of the last state copy (ints)
     // the state map: every reference pad_buffer the handle runs, in plan order (encoder ops, then decoder ops), one stream's exported
@@ -2082,11 +2082,12 @@ int adec_lookup_packed_conceal_bf16(adec_handle* h, const uint8_t* packed, int F
 
 static_assert(sizeof(adec_playout_row) == sizeof(PlayoutRow), "adec_playout_row and PlayoutRow must share a layout");
 
-// conceal_common with the fade row kind; every descriptor is checked before anything is enqueued
+// conceal_common with the fade row kind; with timescale also between rows and frame-started fades (a real row's src with a next or
+// a target).  Every descriptor is checked before anything is enqueued.
 static int playout_common(adec_handle* h, const uint8_t* packed, int F, const adec_playout_row* rows, int R, float* anchors,
-                          int n_anchors, const float* targets, int n_targets, void* zq, bool bf16, void* stream) {
+                          int n_anchors, const float* targets, int n_targets, void* zq, bool bf16, bool timescale, void* stream) {
     if (!h || !h->finalized) return h ? h->fail("not finalized") : 1;
-    const std::string what = bf16 ? "lookup_packed_playout_bf16" : "lookup_packed_playout";
+    const std::string what = std::string(timescale ? "lookup_packed_timescale" : "lookup_packed_playout") + (bf16 ? "_bf16" : "");
     if (need_full_symad(h, what)) return 1;
     if (F < 0 || R < 1) return h->fail(what + ": empty input (F must be >= 0 and R >= 1)");
     if (n_anchors < 0 || n_targets < 0) return h->fail(what + ": n_anchors and n_targets must be >= 0");
@@ -2099,21 +2100,31 @@ static int playout_common(adec_handle* h, const uint8_t* packed, int F, const ad
     for (int r = 0; r < R; ++r) {
         const adec_playout_row& d = rows[r];
         const bool real = d.src >= 0, fade = d.src == -1 && d.next == -1;
+        const bool between = timescale && real && d.next != -1, sfade = timescale && real && d.next == -1 && d.target != -1;
+        const bool from_frame = between || sfade;   // starts from frame src: reads no anchor and stores none
         if (real && d.src >= F) return h->fail(fmt("%s: rows[%d].src = %d is out of range [0, %d)", what.c_str(), r, d.src, F));
-        if (real && d.next != -1) return h->fail(fmt("%s: rows[%d].next = %d: a real row (src >= 0) has next = -1", what.c_str(), r, d.next));
+        if (real && !timescale && d.next != -1)
+            return h->fail(fmt("%s: rows[%d].next = %d: a real row (src >= 0) has next = -1", what.c_str(), r, d.next));
+        if (between && (d.next < 0 || d.next >= F))
+            return h->fail(fmt("%s: rows[%d].next = %d is out of range: a frame in [0, %d) or -1", what.c_str(), r, d.next, F));
         if (!real && d.src != -1) return h->fail(fmt("%s: rows[%d].src = %d is out of range: a frame in [0, %d) or -1", what.c_str(), r, d.src, F));
         if (!real && !fade && (d.next < 0 || d.next >= F))
             return h->fail(fmt("%s: rows[%d].next = %d is out of range: a frame in [0, %d) or -1", what.c_str(), r, d.next, F));
-        if (!fade && d.target != -1)
-            return h->fail(fmt("%s: rows[%d].target = %d: only a fade row (src = next = -1) has a target", what.c_str(), r, d.target));
-        if (fade && (d.target < 0 || d.target >= n_targets))
+        if (!fade && !sfade && d.target != -1)
+            return h->fail(fmt(timescale ? "%s: rows[%d].target = %d: only a fade row (next = -1, no src or a src to fade from) has a target"
+                                         : "%s: rows[%d].target = %d: only a fade row (src = next = -1) has a target", what.c_str(), r, d.target));
+        if ((fade || sfade) && (d.target < 0 || d.target >= n_targets))
             return h->fail(fmt("%s: rows[%d].target = %d is out of range [0, %d)", what.c_str(), r, d.target, n_targets));
         if (!real && !fade && d.den < 2)
             return h->fail(fmt("%s: rows[%d].den = %d: an interpolated row needs den >= 2", what.c_str(), r, d.den));
-        if (!real && !fade && (d.j < 1 || d.j >= d.den))
+        if (between && d.den < 2) return h->fail(fmt("%s: rows[%d].den = %d: a between row needs den >= 2", what.c_str(), r, d.den));
+        if (((!real && !fade) || between) && (d.j < 1 || d.j >= d.den))
             return h->fail(fmt("%s: rows[%d].j = %d is outside [1, den = %d)", what.c_str(), r, d.j, d.den));
-        if (fade && d.den < 1) return h->fail(fmt("%s: rows[%d].den = %d: a fade row needs den >= 1", what.c_str(), r, d.den));
-        if (fade && d.j < 1) return h->fail(fmt("%s: rows[%d].j = %d: a fade row needs j >= 1", what.c_str(), r, d.j));
+        if ((fade || sfade) && d.den < 1) return h->fail(fmt("%s: rows[%d].den = %d: a fade row needs den >= 1", what.c_str(), r, d.den));
+        if ((fade || sfade) && d.j < 1) return h->fail(fmt("%s: rows[%d].j = %d: a fade row needs j >= 1", what.c_str(), r, d.j));
+        if (from_frame && d.slot != -1)
+            return h->fail(fmt("%s: rows[%d].slot = %d: a %s starts from frame src and has slot = -1", what.c_str(), r, d.slot,
+                               between ? "between row" : "frame-started fade"));
         if (d.slot < -1 || d.slot >= n_anchors)
             return h->fail(fmt("%s: rows[%d].slot = %d is out of range: an anchor in [0, %d) or -1", what.c_str(), r, d.slot, n_anchors));
         if (d.slot < 0) continue;
@@ -2141,8 +2152,14 @@ static int playout_common(adec_handle* h, const uint8_t* packed, int F, const ad
     c.anchors = anchors;
     c.targets = targets;
     const long long nth = a.nfr * (a.D / 4);
-    if (bf16) lookup_conceal_kernel<true, true><<<(unsigned)((nth + 255) / 256), 256, 0, s>>>(c);
-    else lookup_conceal_kernel<false, true><<<(unsigned)((nth + 255) / 256), 256, 0, s>>>(c);
+    const unsigned blocks = (unsigned)((nth + 255) / 256);
+    if (timescale) {
+        if (bf16) lookup_conceal_kernel<true, true, true><<<blocks, 256, 0, s>>>(c);
+        else lookup_conceal_kernel<false, true, true><<<blocks, 256, 0, s>>>(c);
+    } else {
+        if (bf16) lookup_conceal_kernel<true, true><<<blocks, 256, 0, s>>>(c);
+        else lookup_conceal_kernel<false, true><<<blocks, 256, 0, s>>>(c);
+    }
     CK(h, cudaGetLastError());
     ++h->launches;
     return 0;
@@ -2150,12 +2167,22 @@ static int playout_common(adec_handle* h, const uint8_t* packed, int F, const ad
 
 int adec_lookup_packed_playout(adec_handle* h, const uint8_t* packed, int F, const adec_playout_row* rows, int R, float* anchors,
                                int n_anchors, const float* targets, int n_targets, float* zq, void* stream) {
-    return playout_common(h, packed, F, rows, R, anchors, n_anchors, targets, n_targets, zq, false, stream);
+    return playout_common(h, packed, F, rows, R, anchors, n_anchors, targets, n_targets, zq, false, false, stream);
 }
 
 int adec_lookup_packed_playout_bf16(adec_handle* h, const uint8_t* packed, int F, const adec_playout_row* rows, int R, float* anchors,
                                     int n_anchors, const float* targets, int n_targets, uint16_t* zq, void* stream) {
-    return playout_common(h, packed, F, rows, R, anchors, n_anchors, targets, n_targets, zq, true, stream);
+    return playout_common(h, packed, F, rows, R, anchors, n_anchors, targets, n_targets, zq, true, false, stream);
+}
+
+int adec_lookup_packed_timescale(adec_handle* h, const uint8_t* packed, int F, const adec_playout_row* rows, int R, float* anchors,
+                                 int n_anchors, const float* targets, int n_targets, float* zq, void* stream) {
+    return playout_common(h, packed, F, rows, R, anchors, n_anchors, targets, n_targets, zq, false, true, stream);
+}
+
+int adec_lookup_packed_timescale_bf16(adec_handle* h, const uint8_t* packed, int F, const adec_playout_row* rows, int R, float* anchors,
+                                      int n_anchors, const float* targets, int n_targets, uint16_t* zq, void* stream) {
+    return playout_common(h, packed, F, rows, R, anchors, n_anchors, targets, n_targets, zq, true, true, stream);
 }
 
 int adec_codec_host(adec_handle* enc, adec_handle* dec, const float* x_host, int B, int T, int64_t* idx_host,

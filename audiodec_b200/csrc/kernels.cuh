@@ -21,7 +21,8 @@
 //   lookup_kernel     - codebook gather-sum (fp32 zq, or bf16 zq rounded once).
 //   lookup_conceal_kernel - the packed lookup per row descriptor: real frames, plus concealed frames interpolated between a
 //                       session's last real frame (an fp32 anchor row) and the frame after a loss; with PLAYOUT also fade
-//                       frames interpolated from the anchor toward a device target row (a receiver's playout clock).
+//                       frames interpolated from the anchor toward a device target row (a receiver's playout clock);
+//                       with TIMESCALE also rows between two packed frames, and fades from a packed frame (time scaling).
 //   zq_moments_kernel - per-utterance fp64 sums and centred second moments of zq (corpus statistics).
 #pragma once
 #include <cuda_bf16.h>
@@ -973,8 +974,14 @@ struct PlayoutArgs {
 template <bool PLAYOUT> struct ConcealKind { using Args = ConcealArgs; };
 template <> struct ConcealKind<true> { using Args = PlayoutArgs; };
 
-template <bool BF16, bool PLAYOUT = false>
+// TIMESCALE (with PLAYOUT) adds two row kinds that start from a packed frame of the launch instead of an anchor, s_src = the sum of
+// frame src (slot = -1):
+//   between row (src >= 0, next >= 0):           zq[r] = fl(fl(fl(j / den) * fl(s_next - s_src)) + s_src), 1 <= j < den;
+//   frame-started fade (src >= 0, target >= 0):  the fade row with a = s_src.
+// s_src is the value a real row of frame src stores as its anchor, so such a row equals the anchor-read row bit for bit.
+template <bool BF16, bool PLAYOUT = false, bool TIMESCALE = false>
 __global__ void __launch_bounds__(256) lookup_conceal_kernel(const typename ConcealKind<PLAYOUT>::Args c) {
+    static_assert(PLAYOUT || !TIMESCALE, "the time-scaling rows are playout rows");
     const LookupArgs& a = c.l;
     const int vpf = a.D / 4;
     const long long gid = (long long)blockIdx.x * 256 + threadIdx.x;
@@ -1004,20 +1011,45 @@ __global__ void __launch_bounds__(256) lookup_conceal_kernel(const typename Conc
     }
     const auto d = c.rows[r];
     const bool real = d.src >= 0;
-    const unsigned char* in = a.packed + (long long)(real ? d.src : d.next) * a.bpf;
-    const unsigned long long mask = (1ull << a.bits) - 1ull;
-    unsigned long long accb = 0;
-    int nb = 0, ib = 0;
-    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int i = 0; i < a.nq; ++i) {
-        while (nb < a.bits) { accb |= (unsigned long long)in[ib++] << nb; nb += 8; }
-        const long long v = (long long)(accb & mask);
-        accb >>= a.bits; nb -= a.bits;
-        const long long row = v < a.N ? v + (long long)i * a.N : -1;
-        if (row < 0 || row >= a.n_rows) { atomicOr(a.err, 1); continue; }
-        const float4 q = __ldg(reinterpret_cast<const float4*>(a.codebook + row * a.D + k4));
-        if (i == 0) s = q;
-        else { s.x = __fadd_rn(s.x, q.x); s.y = __fadd_rn(s.y, q.y); s.z = __fadd_rn(s.z, q.z); s.w = __fadd_rn(s.w, q.w); }
+    const auto frame_sum = [&](int f) {
+        const unsigned char* in = a.packed + (long long)f * a.bpf;
+        const unsigned long long mask = (1ull << a.bits) - 1ull;
+        unsigned long long accb = 0;
+        int nb = 0, ib = 0;
+        float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int i = 0; i < a.nq; ++i) {
+            while (nb < a.bits) { accb |= (unsigned long long)in[ib++] << nb; nb += 8; }
+            const long long v = (long long)(accb & mask);
+            accb >>= a.bits; nb -= a.bits;
+            const long long row = v < a.N ? v + (long long)i * a.N : -1;
+            if (row < 0 || row >= a.n_rows) { atomicOr(a.err, 1); continue; }
+            const float4 q = __ldg(reinterpret_cast<const float4*>(a.codebook + row * a.D + k4));
+            if (i == 0) s = q;
+            else { s.x = __fadd_rn(s.x, q.x); s.y = __fadd_rn(s.y, q.y); s.z = __fadd_rn(s.z, q.z); s.w = __fadd_rn(s.w, q.w); }
+        }
+        return s;
+    };
+    float4 s = frame_sum(real ? d.src : d.next);
+    if constexpr (TIMESCALE) {
+        if (real && (d.next >= 0 || d.target >= 0)) {  // between row or frame-started fade: from s_src, no anchor
+            const float4 t = d.next >= 0 ? frame_sum(d.next)
+                                         : __ldg(reinterpret_cast<const float4*>(c.targets + (long long)d.target * a.D + k4));
+            if (d.next >= 0 || d.j < d.den) {
+                const float w = __fdiv_rn((float)d.j, (float)d.den);
+                s.x = __fadd_rn(__fmul_rn(w, __fsub_rn(t.x, s.x)), s.x);
+                s.y = __fadd_rn(__fmul_rn(w, __fsub_rn(t.y, s.y)), s.y);
+                s.z = __fadd_rn(__fmul_rn(w, __fsub_rn(t.z, s.z)), s.z);
+                s.w = __fadd_rn(__fmul_rn(w, __fsub_rn(t.w, s.w)), s.w);
+            } else {
+                s = t;
+            }
+            if constexpr (BF16)
+                *reinterpret_cast<uint2*>(reinterpret_cast<uint16_t*>(a.zq) + r * a.D + k4) =
+                    make_uint2(bf2_bits(s.x, s.y), bf2_bits(s.z, s.w));
+            else
+                *reinterpret_cast<float4*>(a.zq + r * a.D + k4) = s;
+            return;
+        }
     }
     float4* anchor = d.slot >= 0 ? reinterpret_cast<float4*>(c.anchors + (long long)d.slot * a.D + k4) : nullptr;
     if (real) {

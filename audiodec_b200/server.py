@@ -281,8 +281,9 @@ class SessionState:
     before its first real frame) and the concealment still pending, (packets left, frames per packet, frames concealed so far, frames in
     the gap), or None.  On a ReceiverSessionServer with a playout clock also `playout`, a dict of the playout position: whether the
     session is playing, the steps each held packet has waited (in the order of `inputs`), the frames concealed or faded since the last
-    real frame, the consecutive fade packets, the last real packet's frame count and the sequence numbers given up by the clock; None
-    elsewhere."""
+    real frame, the consecutive fade packets, the last real packet's frame count and the sequence numbers given up by the clock, and with
+    an adaptive delay also the content queue (frames not yet played; o is frames_per_packet minus their count), the frame the anchor
+    was taken from, and the talk spurt's lateness window (relative to the step count); None elsewhere."""
 
     def __init__(self, layouts, states, inputs, outputs, session_id=None, seq=0, anchor=None, conceal=None, playout=None):
         self.layouts: List[list] = layouts
@@ -737,15 +738,20 @@ class ReceiveStats:
         self.underruns = 0         # playout steps with nothing held: a fade packet was played
         self.faded_frames = 0      # code frames of those fade packets
         self.pauses = 0            # times the session stopped playing after max_fade_packets fade packets in a row
+        self.compressed = 0        # adaptive playout steps that played frames_per_packet + 1 content frames
+        self.expanded = 0          # adaptive playout steps that played frames_per_packet - 1 content frames
+        self.delay_frames = None   # the delay in code frames at the session's last adaptive playout step
 
-    def as_dict(self, sample_rate, buffered=None):
+    def as_dict(self, sample_rate, buffered=None, target=None):
         """packets, frames and wire_kbps count the real packets only; buffered (the packets held ahead of the playout point) adds the
-        playout counters"""
+        playout counters, target (the adaptive clock's target delay in packets) the adaptive ones"""
         out = {"packets": self.packets, "frames": self.frames, "duplicates": self.duplicates, "reorders": self.reorders,
                "losses": self.losses, "concealed": self.concealed, "concealed_frames": self.concealed_frames,
                "wire_kbps": 8e-3 * self.bytes / (self.samples / sample_rate) if self.samples else None}
         if buffered is not None:
             out.update(late=self.late, underruns=self.underruns, faded_frames=self.faded_frames, pauses=self.pauses, buffered=buffered)
+        if target is not None:
+            out.update(target_delay=target, delay_frames=self.delay_frames, compressed=self.compressed, expanded=self.expanded)
         return out
 
 
@@ -801,16 +807,43 @@ class ReceiverSessionServer(_SessionSlots):
     and ONE ``decode_streams``.  The silence frame is ``rx_encoder.silence_frame()`` unless ``silence_frame`` gives one.  This is a
     continuity and timing rule: it keeps every session's output running at the packet rate; how the concealed and faded audio sounds
     is not claimed.  ``detach`` / ``attach`` carry the playout position (SessionState.playout) between playout receivers; a session
-    cannot move between a playout receiver and one without."""
+    cannot move between a playout receiver and one without.
+
+    ``max_playout_delay = D_max`` (with ``playout_delay = D``, D <= D_max) adapts the delay to the jitter it measures, by playing
+    buffered content faster or slower in the latent domain.  Every packet must then carry P = frames_per_packet >= 2 frames.  Rules 1 - 3
+    above, unchanged, fill a per-session queue of content frames one packet at a time; every step plays exactly P output frames of every
+    playing session, made from C = P - 1, P or P + 1 content frames.  Each packet that is not a duplicate (late ones included) has
+    lateness stamp - seq; the session keeps the last ``jitter_window`` of the current talk spurt (a pause clears them).  The target is
+    T = min(max(J, D), D_max) packets with J = max - min of that window (0 with fewer than two values); a buffering session starts
+    playing under the rule above with T for D.  The delay at step k (steps completed) is Delta = (k - min lateness + 1) * P - p frames,
+    p = q * P + o, where q is the sequence number of the next content frame and o the frames of it already played; without jitter it
+    stays at Lambda = (T + 1) * P.  With L the real frames available in a row from the playout point (queued, then held in sequence),
+    a step compresses (C = P + 1) when Delta > Lambda and L >= P + 1, else expands (C = P - 1) when Delta < Lambda and L >= P - 1, else
+    plays C = P; so only runs of real frames are scaled.  Output frame i of a scaled window q_0 ... q_{C-1} is, with
+    m, r = divmod(i * (C - 1), P - 1), the real frame q_m when r = 0 and otherwise q_m interpolated toward q_{m+1} with j = r,
+    den = P - 1; the first and last output frames are real.  A concealed or fade frame that shares a step with the real frame it
+    starts from is computed from that frame staged in the same launch.  The pause of rule 3 plays the rest of that step's P frames from
+    the fade packet, then drops the queue.  Each step is ONE ``lookup_packed_timescale`` and ONE ``decode_streams``.  statistics() adds
+    target_delay, delay_frames, compressed and expanded; a session moves only between two adaptive receivers.  When every step plays
+    C = P from o = 0 (a jitter-free session, for one), the rows and the PCM are the fixed clock's."""
 
     _noun = "session"
     reorder_window = 4                 # packets held behind a missing one before it is given up
 
     def __init__(self, rx_encoder, decoder, capacity: int, frames_per_packet: int, sample_rate: int = 48000, device=None,
                  conceal_packets: int = 0, playout_delay: Optional[int] = None, fade_frames: Optional[int] = None,
-                 max_fade_packets: int = 4, silence_frame=None):
+                 max_fade_packets: int = 4, silence_frame=None, max_playout_delay: Optional[int] = None, jitter_window: int = 64):
         if frames_per_packet < 1:
             raise ValueError("frames_per_packet must be >= 1")
+        if max_playout_delay is not None:
+            if playout_delay is None:
+                raise ValueError("max_playout_delay needs playout_delay: the delay adapts between the two")
+            if max_playout_delay < playout_delay:
+                raise ValueError(f"max_playout_delay = {max_playout_delay} is below playout_delay = {playout_delay}")
+            if frames_per_packet < 2:
+                raise ValueError("frames_per_packet must be >= 2 with max_playout_delay: a scaled step interpolates between frames")
+            if jitter_window < 2:
+                raise ValueError("jitter_window must be >= 2")
         if conceal_packets < 0:
             raise ValueError("conceal_packets must be >= 0")
         if playout_delay is not None:
@@ -824,6 +857,7 @@ class ReceiverSessionServer(_SessionSlots):
             if max_fade_packets < 1:
                 raise ValueError("max_fade_packets must be >= 1")
         self.playout_delay, self.fade_frames, self.max_fade_packets = playout_delay, fade_frames, max_fade_packets
+        self.max_playout_delay, self.jitter_window = max_playout_delay, jitter_window
         self.rx_encoder, self.decoder = rx_encoder, decoder
         self.frames_per_packet, self.sample_rate = frames_per_packet, sample_rate
         self.conceal_packets = conceal_packets
@@ -838,7 +872,9 @@ class ReceiverSessionServer(_SessionSlots):
         self.step_times: List[float] = []
         # a decoder with bf16 activations takes bf16 zq: the lookup rounds its fp32 sum once, as the decoder's own cast would
         self._zq_kw = {"dtype": torch.bfloat16} if getattr(decoder, "_act_bf16", False) else {}
-        self._p_host = _pinned(capacity * frames_per_packet * self.frame_bytes, torch.uint8, self.device)
+        # an adaptive step stages up to P + 2 frames of a session: its window, the packet a concealment leads to, the anchor's frame
+        staged = frames_per_packet + (2 if max_playout_delay is not None else 0)
+        self._p_host = _pinned(capacity * staged * self.frame_bytes, torch.uint8, self.device)
         self._p_np = self._p_host.numpy()
         self._y_host = None                            # the PCM of a step, sized on the first step
         # concealment: per slot the fp32 lookup sum of the last real frame decoded, whether there is one, and the pending plan
@@ -857,6 +893,12 @@ class ReceiverSessionServer(_SessionSlots):
         self._fades = [0] * capacity
         self._last_frames: List[Optional[int]] = [None] * capacity
         self._given_up: List[set] = [set() for _ in range(capacity)]
+        # adaptive playout: per slot the content frames not yet played ((0, packet, frame index, 0) real, (1, packet m, j, den)
+        # interpolated toward m's first frame, (2, None, j, den) fade), the (packet, frame index) the anchor was taken from, and the
+        # lateness of the talk spurt's last jitter_window packets
+        self._queue: List[list] = [[] for _ in range(capacity)]
+        self._anchor_frame: List[Optional[tuple]] = [None] * capacity
+        self._lat: List[Deque[int]] = [collections.deque(maxlen=jitter_window) for _ in range(capacity)]
         if playout_delay is not None:
             sf = rx_encoder.silence_frame() if silence_frame is None else silence_frame
             sf = torch.as_tensor(sf, dtype=torch.float32).to(self.device)
@@ -881,13 +923,18 @@ class ReceiverSessionServer(_SessionSlots):
         self._c[s] = self._fades[s] = 0
         self._last_frames[s] = None
         self._given_up[s] = set()
+        self._queue[s] = []
+        self._anchor_frame[s] = None
+        self._lat[s].clear()
 
     def _export_slot(self, s):
         if self.playout_delay is not None:
-            return {"anchor": self._anchors[s].clone() if self._has_anchor[s] else None,
-                    "playout": {"playing": self._playing[s], "waited": [self._steps - self._stamp[s][q] for q in sorted(self._held[s])],
-                                "c": self._c[s], "fades": self._fades[s], "last_frames": self._last_frames[s],
-                                "given_up": sorted(self._given_up[s])}}
+            po = {"playing": self._playing[s], "waited": [self._steps - self._stamp[s][q] for q in sorted(self._held[s])],
+                  "c": self._c[s], "fades": self._fades[s], "last_frames": self._last_frames[s], "given_up": sorted(self._given_up[s])}
+            if self.max_playout_delay is not None:
+                po.update(queue=list(self._queue[s]), anchor_frame=self._anchor_frame[s],
+                          lateness=[v - self._steps for v in self._lat[s]])
+            return {"anchor": self._anchors[s].clone() if self._has_anchor[s] else None, "playout": po}
         if not self.conceal_packets:
             return {}
         plan = self._plan[s]
@@ -908,6 +955,9 @@ class ReceiverSessionServer(_SessionSlots):
             self._stamp[s].update((p.seq, self._steps - w) for p, w in zip(state.inputs, po["waited"]))
             self._playing[s], self._c[s], self._fades[s] = po["playing"], po["c"], po["fades"]
             self._last_frames[s], self._given_up[s] = po["last_frames"], set(po["given_up"])
+            if self.max_playout_delay is not None:
+                self._queue[s], self._anchor_frame[s] = list(po["queue"]), po["anchor_frame"]
+                self._lat[s].extend(v + self._steps for v in po["lateness"])
         if self.conceal_packets or self.playout_delay is not None:
             if state.anchor is not None:
                 self._anchors[s].copy_(state.anchor)
@@ -941,6 +991,10 @@ class ReceiverSessionServer(_SessionSlots):
             raise ValueError("a session moves between two receivers with a playout clock or two without: this one "
                              + ("has one" if self.playout_delay is not None else "has none") + ", the session's had "
                              + ("none" if state.playout is None else "one"))
+        if state.playout is not None and ("queue" in state.playout) != (self.max_playout_delay is not None):
+            raise ValueError("a session moves between two receivers with an adaptive playout delay or two with a fixed one: this one's is "
+                             + ("adaptive" if self.max_playout_delay is not None else "fixed") + ", the session's was "
+                             + ("adaptive" if "queue" in state.playout else "fixed"))
         return self._attach_slot(state, state.session_id)
 
     @property
@@ -968,6 +1022,8 @@ class ReceiverSessionServer(_SessionSlots):
         p = decode_packet(buf, self.codebook_num, self.frame_bytes)
         if p.frames > self.frames_per_packet:
             raise ValueError(f"frames: packet has {p.frames}, this receiver takes at most {self.frames_per_packet}")
+        if self.max_playout_delay is not None and p.frames != self.frames_per_packet:
+            raise ValueError(f"frames: packet has {p.frames}, an adaptive playout delay needs exactly {self.frames_per_packet}")
         with self._lock:
             s = self._ids.get(p.session_id)
             if s is None or s not in self._open:
@@ -976,6 +1032,8 @@ class ReceiverSessionServer(_SessionSlots):
             held, st = self._held[s], self.stats[s]
             if self.playout_delay is not None and p.seq in self._given_up[s]:
                 st.late += 1
+                if self.max_playout_delay is not None:
+                    self._lat[s].append(self._steps - p.seq)
                 return False
             if p.seq < self._next[s] or p.seq in held:
                 st.duplicates += 1
@@ -985,6 +1043,8 @@ class ReceiverSessionServer(_SessionSlots):
             held[p.seq] = p
             if self.playout_delay is not None:
                 self._stamp[s][p.seq] = self._steps
+                if self.max_playout_delay is not None:
+                    self._lat[s].append(self._steps - p.seq)
             else:
                 self._give_up_gap(s)
             return True
@@ -1000,6 +1060,8 @@ class ReceiverSessionServer(_SessionSlots):
         """Decode the next in-order packet of every open session that has one, or its next concealed packet.  Returns the number of
         packets decoded, concealed ones included."""
         with self._step_lock:
+            if self.max_playout_delay is not None:
+                return self._adaptive_step()
             if self.playout_delay is not None:
                 return self._playout_step()
             return self._step()
@@ -1177,17 +1239,7 @@ class ReceiverSessionServer(_SessionSlots):
         with torch.no_grad(), self._codec_lock:
             packed = self._p_host[:o].to(self.device, non_blocking=True).view(o // nb, nb)
             zq = self.rx_encoder.lookup_packed_playout(packed, rows, self._anchors, self._targets, **self._zq_kw)
-            ys = self.decoder.decode_streams(zq, frames, [t[0] for t in taken])
-            y = torch.cat([v.reshape(-1) for v in ys])
-            total = sum(frames)
-            hop = y.numel() // total
-            if self._y_host is None or self._y_host.dtype != y.dtype or self._y_host.numel() < y.numel():
-                self._y_host = _pinned(max(y.numel(), self.capacity * self.frames_per_packet * hop), y.dtype, self.device)
-            y_host = self._y_host[:y.numel()]
-            y_host.copy_(y, non_blocking=True)
-            if y.device.type == "cuda":
-                torch.cuda.current_stream(y.device).synchronize()
-        y_np = (y_host.float() if y_host.dtype == torch.bfloat16 else y_host.clone()).numpy()
+            y_np, hop = self._decode_to_host(zq, frames, [t[0] for t in taken])
         with self._lock:
             o = 0
             for (s, session, kind, p, f, *_) in taken:
@@ -1202,6 +1254,163 @@ class ReceiverSessionServer(_SessionSlots):
                     st.frames += f
                     st.bytes += HEADER_BYTES + len(p.payload)
                     st.samples += chunk.size
+        self.step_times.append(time.time() - t0)
+        return len(taken)
+
+    def _decode_to_host(self, zq, frames, slots):
+        """ONE decode_streams of the step's zq, and its PCM back in ONE copy -> (float32 samples, hop)"""
+        ys = self.decoder.decode_streams(zq, frames, slots)
+        y = torch.cat([v.reshape(-1) for v in ys])
+        hop = y.numel() // sum(frames)
+        if self._y_host is None or self._y_host.dtype != y.dtype or self._y_host.numel() < y.numel():
+            self._y_host = _pinned(max(y.numel(), self.capacity * self.frames_per_packet * hop), y.dtype, self.device)
+        y_host = self._y_host[:y.numel()]
+        y_host.copy_(y, non_blocking=True)
+        if y.device.type == "cuda":
+            torch.cuda.current_stream(y.device).synchronize()
+        return (y_host.float() if y_host.dtype == torch.bfloat16 else y_host.clone()).numpy(), hop
+
+    def _target(self, s) -> int:
+        """the adaptive clock's target delay of slot s in packets: the window's lateness spread, within [D, D_max]"""
+        lat = self._lat[s]
+        j = max(lat) - min(lat) if len(lat) >= 2 else 0
+        return min(max(j, self.playout_delay), self.max_playout_delay)
+
+    def _adaptive_window(self, s, k) -> list:
+        """The content frames playing slot s plays at step k (steps completed), with _lock held: decides C from the delay, fills the
+        queue by rules 1 - 3 (_playout_plan) one packet at a time, and takes C frames off it."""
+        P, q, st = self.frames_per_packet, self._queue[s], self.stats[s]
+        lam = (self._target(s) + 1) * P
+        nxt = self._next[s]
+        seq, o = (nxt - 1, P - len(q)) if q else (nxt, 0)
+        delta = (k - min(self._lat[s]) + 1) * P - (seq * P + o)
+        st.delay_frames = delta
+        avail = 0                                                      # L: real frames in a row from the playout point
+        if not q or q[0][0] == 0:
+            avail, held = len(q), self._held[s]
+            while avail < P + 1 and nxt in held:
+                avail += P
+                nxt += 1
+        c = P
+        if delta > lam and avail >= P + 1:
+            c = P + 1
+            st.compressed += 1
+        elif delta < lam and avail >= P - 1:
+            c = P - 1
+            st.expanded += 1
+        while len(q) < c:
+            kind, p, f, j, den = self._playout_plan(s)
+            if kind == 0:
+                q.extend((0, p, i, 0) for i in range(f))
+                st.packets += 1
+                st.frames += f
+                st.bytes += HEADER_BYTES + len(p.payload)
+            else:
+                q.extend((kind, p, j + i, den) for i in range(f))
+        win = q[:c]
+        del q[:c]
+        if not self._playing[s]:                                       # paused by a fade packet: what it did not play is dropped
+            q.clear()
+            self._lat[s].clear()
+        return win
+
+    def _window_rows(self, s, win, stage, rows) -> None:
+        """Append slot s's P adec_playout_row descriptors for the content frames `win` to `rows`; stage(packet, i) stages frame i of a
+        packet (once per step) and returns its index.  The last real frame of the window stores the anchor; a concealed or fade frame
+        in a window with a real frame starts from a staged frame (the last real one before it, or the frame the old anchor came from),
+        since a launch may not both write and read one anchor."""
+        P, C = self.frames_per_packet, len(win)
+        if C != P:                                                     # a scaled run of real frames
+            for i in range(P):
+                m, r = divmod(i * (C - 1), P - 1)
+                a = win[m]
+                if r == 0:
+                    rows.append((stage(a[1], a[2]), -1, -1, s if m == C - 1 else -1, 0, 0))
+                else:
+                    b = win[m + 1]
+                    rows.append((stage(a[1], a[2]), stage(b[1], b[2]), -1, -1, r, P - 1))
+            return
+        last = -1
+        for i, e in enumerate(win):
+            if e[0] == 0:
+                last = i
+        for i, (kind, p, j, den) in enumerate(win):
+            if kind == 0:
+                rows.append((stage(p, j), -1, -1, s if i == last else -1, 0, 0))
+                continue
+            src = (win[last][1], win[last][2]) if i > last >= 0 else self._anchor_frame[s] if last >= 0 else None
+            src = -1 if src is None else stage(*src)
+            slot = s if last < 0 and self._has_anchor[s] else -1
+            if kind == 1:
+                rows.append((src, stage(p, 0), -1, -1 if src >= 0 else slot, j, den))
+            else:
+                rows.append((src, -1, 0, -1 if src >= 0 else slot, j, den))
+
+    def _adaptive_step(self) -> int:
+        """One packet period of the adaptive playout clock: P output frames for every playing session."""
+        t0 = time.time()
+        now, P = self._steps, self.frames_per_packet
+        taken, rows, chunks = [], [], []               # taken: (slot, open counter, real content frames played)
+        nst = [0]                                      # frames staged so far
+        nb = self.frame_bytes
+        with self._lock:
+            for sid, s in sorted(self._ids.items()):
+                if s not in self._open:
+                    continue
+                if not self._playing[s]:
+                    target = self._target(s)
+                    if not any(now - t >= target for t in self._stamp[s].values()):
+                        continue
+                    self._playing[s] = True
+                win = self._adaptive_window(s, now)
+                p = win[0][1]
+                if len(win) == P and win[0][0] == 0 and win[0][2] == 0 and win[-1][1] is p:
+                    # one whole real packet, the common step: its payload staged in one piece, the fixed clock's rows
+                    base = nst[0]
+                    chunks.append(p.payload)
+                    nst[0] += P
+                    rows.extend([(base + i, -1, -1, -1, 0, 0) for i in range(P - 1)])
+                    rows.append((base + P - 1, -1, -1, s, 0, 0))
+                    self._anchor_frame[s] = (p, P - 1)
+                    self._has_anchor[s] = True
+                    taken.append((s, self._session[s], P))
+                    continue
+                staged = {}
+
+                def stage(p, i):
+                    key = (id(p), i)
+                    if key not in staged:
+                        staged[key] = nst[0]
+                        chunks.append(p.payload[i * nb:(i + 1) * nb])
+                        nst[0] += 1
+                    return staged[key]
+
+                self._window_rows(s, win, stage, rows)
+                real = [e for e in win if e[0] == 0]
+                if real:
+                    self._anchor_frame[s] = (real[-1][1], real[-1][2])
+                    self._has_anchor[s] = True
+                taken.append((s, self._session[s], len(real)))
+            self._steps += 1
+        if not taken:
+            self.step_times.append(time.time() - t0)
+            return 0
+        o = nst[0] * nb
+        self._p_np[:o] = np.frombuffer(b"".join(chunks), dtype=np.uint8)
+        table = self._rows_np[self._rows_turn]
+        self._rows_turn ^= 1
+        table[:len(rows)] = rows
+        with torch.no_grad(), self._codec_lock:
+            packed = self._p_host[:o].to(self.device, non_blocking=True).view(o // nb, nb)
+            zq = self.rx_encoder.lookup_packed_timescale(packed, table[:len(rows)], self._anchors, self._targets, **self._zq_kw)
+            y_np, hop = self._decode_to_host(zq, [P] * len(taken), [t[0] for t in taken])
+        with self._lock:
+            for i, (s, session, real) in enumerate(taken):
+                if s not in self._open or self._session[s] != session:
+                    continue                        # closed while the step ran: the frame is dropped
+                chunk = y_np[i * P * hop:(i + 1) * P * hop]
+                self._out[s].append(chunk)
+                self.stats[s].samples += real * hop
         self.step_times.append(time.time() - t0)
         return len(taken)
 
@@ -1237,9 +1446,11 @@ class ReceiverSessionServer(_SessionSlots):
         """steps, ms per step (mean, std), the open sessions, packets for sessions that were not open, and per open session: packets,
         frames, duplicates, reorders, losses, concealed packets and frames, and the wire kbps received (real packet bytes, headers
         included, over the seconds of real audio decoded).  With a playout clock also late, underruns, faded_frames, pauses and
-        buffered (the packets held ahead of the playout point)."""
+        buffered (the packets held ahead of the playout point).  With an adaptive delay also target_delay (packets), delay_frames (the
+        delay at the session's last played step, in code frames) and the compressed and expanded step counts."""
         with self._lock:
-            po = self.playout_delay is not None
-            per = {sid: self.stats[s].as_dict(self.sample_rate, len(self._held[s]) if po else None) for sid, s in sorted(self._ids.items())}
+            po, ad = self.playout_delay is not None, self.max_playout_delay is not None
+            per = {sid: self.stats[s].as_dict(self.sample_rate, len(self._held[s]) if po else None, self._target(s) if ad else None)
+                   for sid, s in sorted(self._ids.items())}
         return {"capacity": self.capacity, "open_sessions": len(per), "steps": len(self.step_times), "step_ms": _ms(self.step_times),
                 "unknown_session_packets": self.unknown_session_packets, "per_session": per}

@@ -310,6 +310,22 @@ int adec_lookup_packed_playout(adec_handle *h, const uint8_t *packed, int F, con
 int adec_lookup_packed_playout_bf16(adec_handle *h, const uint8_t *packed, int F, const adec_playout_row *rows, int R, float *anchors,
                                     int n_anchors, const float *targets, int n_targets, uint16_t *zq, void *stream);
 
+/* -- the packed lookup of an adaptive playout clock (time scaling in the latent domain) ---------------------------------------------
+ * adec_lookup_packed_playout with two more kinds of adec_playout_row, both starting from packed frame src of the same call instead of
+ * an anchor (s_x is the fp32 lookup sum of packed frame x):
+ *   between row (src >= 0, next >= 0, target = -1, slot = -1, 1 <= j < den):
+ *     zq = fl(fl(fl(j / den) * fl(s_next - s_src)) + s_src), every operation rounded to nearest on its own (no contraction);
+ *   frame-started fade (src >= 0, next = -1, target in [0, n_targets), slot = -1, j >= 1, den >= 1):
+ *     the fade row with the anchor a replaced by s_src: zq = t when j >= den, otherwise fl(fl(fl(j / den) * fl(t - s_src)) + s_src).
+ * s_src is what a real row of frame src stores as its anchor, so either row equals the anchor-read row of a later call bit for bit; a
+ * receiver uses them when a concealed or fade frame follows, in the same call, the real frame that is its anchor.  Every other row is
+ * adec_lookup_packed_playout's, bit for bit, with the same checks and the same conditions on the arguments; an error names the field.
+ * One launch.  Full symAD handle only.  _bf16: zq is bf16, the fp32 result rounded once to nearest even. */
+int adec_lookup_packed_timescale(adec_handle *h, const uint8_t *packed, int F, const adec_playout_row *rows, int R, float *anchors,
+                                 int n_anchors, const float *targets, int n_targets, float *zq, void *stream);
+int adec_lookup_packed_timescale_bf16(adec_handle *h, const uint8_t *packed, int F, const adec_playout_row *rows, int R, float *anchors,
+                                      int n_anchors, const float *targets, int n_targets, uint16_t *zq, void *stream);
+
 /* number of kernel launches issued by this handle since creation (bench.py's gpu_launches) */
 int64_t adec_launch_count(const adec_handle *h);
 
