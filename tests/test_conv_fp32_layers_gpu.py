@@ -953,24 +953,28 @@ def decidable_frames(z64, embeds64, delta):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("engine", ["f16", "tf32"])
-def test_encoder_amplitude_sweep(engine, monkeypatch, golden_dir, symad_sd):
+@pytest.mark.parametrize("model", ["symAD", "symAAD", "c16"])
+def test_encoder_amplitude_sweep(model, engine, monkeypatch, golden_dir):
     """The golden symAD clip scaled by 2^-k, k in {0, 4, 8, 12, 16, 20, 24} (quiet audio: the ELU's small-activation gap is where
-    it would show), exact digital silence and isolated clicks in silence: offline z within 4x the fp32 oracle's own error against the
-    fp64 oracle, and the code indices equal to the fp32 oracle's on every frame whose fp64 decisions are wider than the measured z
-    error.  The biases keep the activations O(1) past the first layer, so even silence stays inside the fp16-split activation
-    envelope (test_activation_envelope)."""
+    it would show), exact digital silence and isolated clicks in silence, through the symAD, symAAD (ELU before the projector) and
+    c16 (strides 2 / 4 / 5 / 8, 16 codebooks) encoders: offline z within 4x the fp32 oracle's own error against the fp64 oracle, and
+    the code indices equal to the fp32 oracle's on every frame whose fp64 decisions are wider than the measured z error.  The biases
+    keep the activations O(1) past the first layer, so even silence stays inside the fp16-split activation envelope
+    (test_activation_envelope)."""
     from audiodec_b200 import synthetic as S
     from audiodec_b200.codec import SymADStreamGenerator
     from oracle import audiodec_oracle as O
     monkeypatch.setenv("ADEC_CONV_PATH", engine)
     dev = torch.device("cuda:0")
-    g = SymADStreamGenerator(**S.SYMAD_PARAMS)
-    g.load_state_dict(symad_sd)
+    params = {"symAD": S.SYMAD_PARAMS, "symAAD": S.SYMAAD_PARAMS, "c16": S.SYMAD_C16_PARAMS}[model]
+    sd = S.symad_state_dict(params, seed=0)
+    g = SymADStreamGenerator(**params)
+    g.load_state_dict(sd)
     g = g.eval().to(dev)
-    o32 = O.SymADOracle(S.SYMAD_PARAMS, symad_sd)
-    o64 = O.SymADOracle(S.SYMAD_PARAMS, symad_sd, dtype=torch.float64)
+    o32 = O.SymADOracle(params, sd)
+    o64 = O.SymADOracle(params, sd, dtype=torch.float64)
     embeds64 = [e.numpy() for e in o64.embeds]
-    n = S.SYMAD_PARAMS["codebook_size"]
+    n = params["codebook_size"]
     x0 = torch.from_numpy(np.load(os.path.join(golden_dir, "symad_oneshot.npz"))["x"])
     clicks = torch.zeros_like(x0)
     clicks[..., [100, 2345, 2346, 7001, x0.shape[-1] - 1]] = torch.tensor([0.5, -0.25, 0.125, -1.0, 0.75])
@@ -988,7 +992,7 @@ def test_encoder_amplitude_sweep(engine, monkeypatch, golden_dir, symad_sd):
         delta = max(np.linalg.norm(zk - z64, axis=0).max(), np.linalg.norm(z32 - z64, axis=0).max())
         ok, idx64 = decidable_frames(z64, embeds64, delta)
         idx64 = idx64 + n * np.arange(len(embeds64))[:, None]
-        REPORT.append(f"{tag:18s} {engine:5s} max|z| = {np.abs(z64).max():.3g}  z err = {ek:.3g}  fp32 oracle z err = {e32:.3g}  "
+        REPORT.append(f"{model:6s} {tag:18s} {engine:5s} max|z| = {np.abs(z64).max():.3g}  z err = {ek:.3g}  fp32 oracle z err = {e32:.3g}  "
                       f"decidable frames {ok.sum()}/{ok.size}  index mismatches vs fp32 oracle: {(idx_k != idx32).any(0).sum()}")
         print(REPORT[-1])
         assert ek <= 4 * max(e32, 2.0 ** -23 * np.abs(z64).max()), REPORT[-1]
